@@ -32,6 +32,11 @@ constexpr int COOP_MAX_LANES = 33;       // >32 = never: measured on C3/C5, the 
 constexpr int BAND_ROWS = 16;
 constexpr uint32_t LARGE_CAP = 1u << 22; // queued large sub-triangles (160 MB)
 constexpr uint32_t BAND_CAP = 1u << 24;  // queued (sub-triangle, band) items (128 MB)
+// A sub-triangle that does not fit the queues is rasterised by the set-up kernel instead.  Its band reservation is one atomicAdd
+// and may straddle BAND_CAP; raster_band_kernel walks every slot below min(counters[1], BAND_CAP), and the scratch they live in is
+// never cleared, so the reservation that crosses the cap fills its in-range slots with BAND_SKIP and the band kernel skips them.
+// (A reservation that never overshoots needs a compare-and-swap loop on the counter every large sub-triangle contends for.)
+constexpr uint32_t BAND_SKIP = 0xFFFFFFFFu;   // band item whose sub-triangle index is >= LARGE_CAP: nothing to rasterise
 constexpr int MODE_COLOUR = 0;           // opaque + cutout forward routines into the visibility buffer
 constexpr int MODE_DEPTH = 1;            // shadow passes into the atlas
 constexpr int MODE_BLEND = 2;            // blend routine: collect per-sample fragment lists
@@ -381,6 +386,7 @@ __device__ bool process_subtriangle(const RasterParams& p, const float4 a, const
         if (queued) {
             bi = atomicAdd(&p.counters[1], nb);
             queued = bi + nb <= BAND_CAP;
+            if (!queued) for (uint32_t k = bi; k < BAND_CAP; ++k) p.bands[k] = make_uint2(BAND_SKIP, 0u);   // the one reservation that straddles the cap
         }
         if (queued) {
             p.large[li] = s;
@@ -571,6 +577,7 @@ __global__ void __launch_bounds__(RS_THREADS) raster_band_kernel(const __grid_co
         item = __shfl_sync(0xFFFFFFFFu, item, 0);
         if (item >= n_bands) break;
         const uint2 it = p.bands[item];
+        if (it.x >= LARGE_CAP) continue;   // BAND_SKIP
         const SubTri s = p.large[it.x];
         int px0, py0, px1, py1;
         pixel_bounds(p, s, px0, py0, px1, py1);
