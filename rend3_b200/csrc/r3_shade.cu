@@ -374,7 +374,7 @@ __device__ __noinline__ float4 skybox_at_pixel(const ShadeParams& p, uint32_t px
 }
 
 // TEX = the context holds a texture table: kernels are instantiated with and without the texture path, so that scenes without
-// textures keep the register budget (75 instead of 104) of the lean kernel.
+// textures keep the register budget (80 instead of 128 on sm_90a) of the lean kernel.
 template <bool TEX>
 __device__ __forceinline__ float4 shade_inputs(const ShadeParams& p, const DirPrep* __restrict__ s_dir, const PointPrep* __restrict__ s_point, const FragIn& f,
                                                const LightMask& mask, const r3_tri_record* tp, uint32_t px, uint32_t py, uint32_t* lights_evaluated = nullptr) {
@@ -456,8 +456,9 @@ __device__ __forceinline__ float4 shade_inputs(const ShadeParams& p, const DirPr
                 const PointPrep& L = i < MAX_SMEM_POINT ? s_point[i] : p.point[i];
                 const float3 delta = make_float3(L.pos[0] - vp.x, L.pos[1] - vp.y, L.pos[2] - vp.z);
                 const float d2 = dot3(delta, delta);
-                // att = (1 - s^2)^2 / (1 + s^2) with s = saturate(d / radius) is exactly 0 at and beyond the radius
-                if (d2 >= L.radius * L.radius && pxl.roughness > 0.0f) continue;
+                // att = (1 - s^2)^2 / (1 + s^2) with s = saturate(d / radius) is exactly 0 at and beyond a positive radius; a
+                // negative or NaN radius saturates d / radius to 0, so that light reaches every fragment with att = 1
+                if (L.radius > 0.0f && d2 >= L.radius * L.radius && pxl.roughness > 0.0f) continue;
                 const float inv_d = rsqrtf(d2), d = d2 * inv_d;
                 const float sdist = saturate(d * rcp_approx(L.radius)), s2 = sdist * sdist, inv_s2 = 1.0f - s2;
                 const float att = inv_s2 * inv_s2 * rcp_approx(1.0f + s2);
@@ -555,7 +556,8 @@ __global__ void __launch_bounds__(256) resolve_kernel(const __grid_constant__ Sh
                         const float c = L.pos[a], e = fmaxf(fmaxf(blo[a] - c, c - bhi[a]), 0.0f);   // distance to the box along this axis
                         d2 += e * e;
                     }
-                    reach = blo[0] <= bhi[0] && d2 <= L.radius * L.radius * 1.001f;
+                    // only a positive radius bounds a light (see shade_inputs); a NaN radius fails every comparison
+                    reach = blo[0] <= bhi[0] && (!(L.radius > 0.0f) || d2 <= L.radius * L.radius * 1.001f);
                 }
                 const uint32_t bal = __ballot_sync(0xFFFFFFFFu, reach);
                 if (lane == 0) s_mask[warp] = bal;
