@@ -28,6 +28,12 @@
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
  *     has to grow (first frame, larger world, new resolution) is reallocated with a stream synchronisation as well.
+ *   - incremental world updates — r3_update_object_sort_info, r3_resize_objects, r3_update_mesh_buffer, r3_update_textures — block
+ *     like the other host-pointer uploads.  Every argument is checked before anything is written: a rejected call returns
+ *     R3_E_INVALID or R3_E_STATE and leaves the context as it was.  A count of 0 is a no-op.  Their result equals the full upload
+ *     of the updated arrays (r3_set_object_sort_info, r3_set_objects + r3_set_object_sort_info, r3_set_mesh_buffer, r3_set_textures);
+ *     what they save is the host loop and the PCIe copy of everything that did not change.  Growth keeps the old contents by a
+ *     device copy, as the reference does (copy_buffer_to_buffer into the larger buffer).
  *   - `camera` is R3_CAMERA_VIEWPORT or a shadow index 0..R3_MAX_SHADOWS-1
  *     (CameraSpecifier, rend3-routine/src/common/camera.rs).
  */
@@ -98,12 +104,31 @@ int r3_set_objects_device(r3_ctx*, const void* device_records, uint32_t n_slots)
  * ("atomic capable"), bit2 = SortingOrder::BackToFront.  location = InternalObject::location. */
 int r3_set_object_sort_info(r3_ctx*, const uint64_t* material_key, const uint8_t* flags,
                             const float* location_xyz, uint32_t n_slots);
+/* FreelistDerivedBuffer::apply's scatter of the stale entries (util/freelist/buffer.rs:85-97, object.rs:302-316): entry i sets slot
+ * slots[i] exactly as r3_set_object_sort_info would; every slot must be below the current sort-info count.  A slot listed twice takes
+ * its later entry.  Starts a new frame epoch, like the full call.  The per-frame call for objects that move (location) or change. */
+int r3_update_object_sort_info(r3_ctx*, const uint32_t* slots, const uint64_t* material_key, const uint8_t* flags,
+                               const float* location_xyz, uint32_t n);
+/* FreelistDerivedBuffer::apply's growth (buffer.rs:66-83, object.rs:363): the object buffer grows to n_slots (never shrinks) by a device
+ * copy; the new slots are zero records (enabled 0).  When sort info is set it grows too (key 0, flags 0, location 0).  Equals
+ * r3_set_objects + r3_set_object_sort_info of the old contents followed by zeros.  R3_E_STATE while the records are borrowed
+ * (r3_set_objects_device) or a visible-set exchange / peer plumbing is connected (their buffers are sized at creation). */
+int r3_resize_objects(r3_ctx*, uint32_t n_slots);
 int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);               /* eval_output.mesh_buffer (mesh.rs:99) */
+/* MeshManager::add (mesh.rs:123-184): write nbytes at byte_offset of the megabuffer (both multiples of 4).  A write past the end extends it;
+ * words between the old end and byte_offset read 0.  The allocation grows to the next power of two, keeping its contents (also what
+ * r3_skin wrote) — MeshManager::reallocate_buffers (mesh.rs:264-308). */
+int r3_update_mesh_buffer(r3_ctx*, uint64_t byte_offset, const void* bytes, uint64_t nbytes);
 int r3_set_materials(r3_ctx*, const r3_material* records, uint32_t count);         /* material_manager.archetype_view::<M>().buffer() */
 /* the bindless d2 texture table the material records index (TextureManager::add / fill, rend3/src/managers/texture.rs;
  * `textures[material.albedo_tex - 1u]`, opaque.wgsl:152-161): descriptors + one blob with every mip level.  Sampling is
  * textureSampleGrad with the linear or nearest Repeat sampler of common/samplers.rs:42-56 (trilinear, no anisotropy). */
 int r3_set_textures(r3_ctx*, const r3_texture_desc* descs, uint32_t count, const void* texels, uint64_t nbytes);
+/* TextureManager::add / fill (texture.rs:98-251) a range at a time: write nbytes of texels at blob_offset (16-aligned; the blob grows like the
+ * mesh buffer, contents kept), then table entries [first, first + count) — first <= the current count, so a call overwrites or appends
+ * but leaves no gap.  Each descriptor is checked as r3_set_textures checks it, against the blob after the write. */
+int r3_update_textures(r3_ctx*, uint32_t first, const r3_texture_desc* descs, uint32_t count, uint64_t blob_offset,
+                       const void* texels, uint64_t nbytes);
 /* SkyboxRoutine::set_background_texture (rend3-routine/src/skybox.rs:47-60): the cube map skybox.wgsl samples wherever the depth buffer
  * still holds its clear value.  desc->width = face size (height is ignored), six faces in the order +X, -X, +Y, -Y, +Z, -Z, each with
  * its `mip_count` levels stored tightly, face after face, from desc->byte_offset.  desc == NULL removes the skybox. */

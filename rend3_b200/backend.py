@@ -40,6 +40,7 @@ ENTRY_POINTS = [
     "readback_hiz", "forward_stats", "forward_light_evaluations", "device_ptr", "set_scissor_rows", "skin", "readback_mesh_buffer",
     "exchange_create", "exchange_connect", "exchange_words", "exchange_merge", "exchange_merged", "exchange_count", "exchange_counts", "exchange_destroy",
     "peer_create", "peer_connect", "peer_send_atlas_rect", "peer_send_rows", "peer_signal", "peer_wait", "peer_destroy", "clear_shadow_rect", "set_cull_shard",
+    "update_object_sort_info", "resize_objects", "update_mesh_buffer", "update_textures",
 ]
 
 
@@ -140,9 +141,31 @@ class Backend:
         assert len(f) == len(k) and len(l) == 3 * len(k)
         self._call("set_object_sort_info", _ptr(k), _ptr(f), _ptr(l), C.c_uint32(len(k)))
 
+    def update_object_sort_info(self, slots, material_key, flags, location):
+        s = np.ascontiguousarray(slots, dtype=np.uint32)
+        k = np.ascontiguousarray(material_key, dtype=np.uint64)
+        f = np.ascontiguousarray(flags, dtype=np.uint8)
+        l = np.ascontiguousarray(location, dtype=np.float32).reshape(-1)
+        assert len(k) == len(s) and len(f) == len(s) and len(l) == 3 * len(s)
+        self._call("update_object_sort_info", _ptr(s), _ptr(k), _ptr(f), _ptr(l), C.c_uint32(len(s)))
+
+    def resize_objects(self, n_slots: int):
+        self._call("resize_objects", C.c_uint32(n_slots))
+
     def set_mesh_buffer(self, words: np.ndarray):
         words = np.ascontiguousarray(words, dtype=np.uint32)
         self._call("set_mesh_buffer", _ptr(words), C.c_uint64(words.nbytes))
+
+    def update_mesh_buffer(self, byte_offset: int, data: np.ndarray):
+        raw = np.ascontiguousarray(data).view(np.uint8).reshape(-1)
+        self._call("update_mesh_buffer", C.c_uint64(byte_offset), _ptr(raw) if len(raw) else None, C.c_uint64(len(raw)))
+
+    def update_textures(self, first: int, descs: np.ndarray, blob_offset: int, texels: np.ndarray):
+        descs = np.ascontiguousarray(descs)
+        texels = np.ascontiguousarray(texels).view(np.uint8).reshape(-1)
+        assert descs.dtype.itemsize == 32
+        self._call("update_textures", C.c_uint32(first), _ptr(descs) if len(descs) else None, C.c_uint32(len(descs)), C.c_uint64(blob_offset),
+                   _ptr(texels) if len(texels) else None, C.c_uint64(len(texels)))
 
     def set_materials(self, records: np.ndarray):
         records = np.ascontiguousarray(records)

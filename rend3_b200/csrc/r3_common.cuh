@@ -110,6 +110,7 @@ struct r3_ctx {
     std::vector<uint64_t> sort_key; std::vector<uint8_t> sort_flags; std::vector<float> sort_loc;
     uint32_t* d_live_bits = nullptr; uint32_t live_bits_cap = 0; bool have_live = false;
     uint8_t* d_sort_key8 = nullptr; float* d_sort_loc = nullptr; uint32_t sort_dev_cap = 0; bool gpu_batching_ok = false;
+    uint32_t sort_live_blend = 0, sort_wide_keys = 0;   // live slots with material key 2 (any_blend), slots with a key >= 64 (host batching)
     // frame-wide sort shared by the cameras of one frame (r3_gpu_batching.cu)
     unsigned long long* d_gsort_keys[2] = {nullptr, nullptr}; uint64_t gsort_cap[2] = {0, 0}; uint32_t* d_gsort_hist = nullptr; uint64_t gsort_hist_cap = 0;
     uint32_t* d_gsort_header = nullptr; int gsort_src = 0; uint32_t gsort_n = 0; bool gsort_valid = false; float gsort_loc[3] = {0, 0, 0};
@@ -118,7 +119,7 @@ struct r3_ctx {
     uint32_t* d_mesh = nullptr; uint64_t mesh_words = 0, mesh_cap = 0;
     r3_material* d_materials = nullptr; uint32_t n_materials = 0, materials_cap = 0;
     bool has_skybox = false; r3_texture_desc sky_desc{}; uint8_t* d_sky_texels = nullptr; uint64_t sky_cap = 0;   // cube map of the skybox routine
-    r3_texture_desc* d_tex_descs = nullptr; uint32_t n_textures = 0, tex_descs_cap = 0; uint8_t* d_texels = nullptr; uint64_t texels_cap = 0;
+    r3_texture_desc* d_tex_descs = nullptr; uint32_t n_textures = 0, tex_descs_cap = 0; uint8_t* d_texels = nullptr; uint64_t texels_cap = 0, texel_bytes = 0;
     r3_directional_light* d_dir = nullptr; uint32_t n_dir = 0, dir_cap = 0;
     r3_point_light* d_point = nullptr; uint32_t n_point = 0, point_cap = 0;
     float* d_light_mats = nullptr; uint64_t light_mats_cap = 0;   // view-space light tables built by light_prep_kernel
@@ -201,6 +202,9 @@ int r3_reserve_t(r3_ctx* c, T** ptr, C* cap, uint64_t need, bool keep = false, b
 int r3_launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode);
 int r3_split_objects(r3_ctx* c);
 int r3_split_slots(r3_ctx* c, const uint32_t* d_slots, uint32_t n);
+int r3_grow_hot(r3_ctx* c, uint32_t old_n, uint32_t n);   // r3_resize_objects: keep the hot copies of slots < old_n, zero slots [old_n, n)
+uint64_t r3_hot_capacity(uint64_t want);                    // slots the hot arrays (and a grown object buffer) are allocated for
+int r3_launch_mask_word(r3_ctx* c, uint32_t* word_a, uint32_t* word_b, uint32_t keep_mask);   // *word &= keep_mask (either may be null)
 int r3_launch_triangle_cull(r3_ctx* c, r3_camera* cam);
 int r3_host_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], uint32_t max_dispatch_count);
 int r3_upload_jobs(r3_ctx* c, r3_camera* cam);

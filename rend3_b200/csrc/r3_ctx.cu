@@ -1,5 +1,6 @@
 // r3_ctx.cu — context, uploads, readbacks and the C ABI glue of librend3_b200.so (include/rend3_b200.h).
 // Host logic only; the kernels live in r3_cull_bake.cu, r3_tri_cull.cu, r3_raster.cu, r3_shade.cu.
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -174,6 +175,9 @@ R3_EXPORT int r3_frame_begin(r3_ctx* c) {
     cudaSetDevice(c->device);
     if (c->capturing) return r3_fail(c, R3_E_STATE, "frame_begin: a frame is already being recorded");
     if (c->timer.enabled) return R3_OK;       // per-kernel timing needs real event records: the frame runs eagerly
+    // the invocation bounds of the device batching are read back once after the records changed: do it before the recording starts, so
+    // that a frame after r3_update_objects / r3_set_objects does not have to flush in its middle for them
+    if (c->gpu_batching_ok) R3_TRY(r3_compute_max_invocations(c));
     R3_CUDA(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeRelaxed));
     c->capturing = true;
     return R3_OK;
@@ -281,6 +285,19 @@ R3_EXPORT int r3_update_objects(r3_ctx* c, const uint32_t* slots, const r3_objec
     R3_CUDA(c, r3_stream_sync(c));
     return R3_OK;
 }
+// The sort facts of one slot as the device batching reads them: key8 = ((material_key << 1 | reason) << 1) | back_to_front, and the
+// two counts the context derives any_blend and gpu_batching_ok from (r3_set_object_sort_info, r3_update_object_sort_info).
+static inline uint8_t sort_key8(uint64_t key, uint8_t flags) {
+    const uint32_t reason = (flags & 2) ? 0u : 1u;
+    return (uint8_t)(((((uint32_t)key & 63u) << 1 | reason) << 1) | ((flags & 4) ? 1u : 0u));
+}
+static inline uint32_t sort_live_blend(uint64_t key, uint8_t flags) { return key == 2 && (flags & 1) ? 1u : 0u; }   // TransparencyType::Blend as u64 (pbr/material.rs:497-503)
+static inline uint32_t sort_wide_key(uint64_t key) { return key >= 64 ? 1u : 0u; }                                 // only the host batching sorts such keys
+static void sort_derive(r3_ctx* c) {
+    c->any_blend = c->sort_live_blend != 0;
+    c->gpu_batching_ok = c->sort_wide_keys == 0 && c->sort_key.size() < (1u << 24) && !getenv("R3_HOST_BATCHING");
+}
+
 R3_EXPORT int r3_set_object_sort_info(r3_ctx* c, const uint64_t* key, const uint8_t* flags, const float* loc, uint32_t n) {
     if (!c || !key || !flags || !loc) return r3_fail(c, R3_E_INVALID, "set_object_sort_info: null");
     cudaSetDevice(c->device);
@@ -293,15 +310,13 @@ R3_EXPORT int r3_set_object_sort_info(r3_ctx* c, const uint64_t* key, const uint
         if (flags[i] & 1) bits[i >> 5] |= 1u << (i & 31);
     R3_TRY(r3_reserve_t(c, &c->d_live_bits, &c->live_bits_cap, words));
     R3_CUDA(c, cudaMemcpyAsync(c->d_live_bits, bits.data(), (size_t)words * 4, cudaMemcpyHostToDevice, c->stream));
-    // device copies for the on-device batch_objects: key8 = ((material_key << 1 | reason) << 1) | back_to_front
-    bool ok = true;
+    // device copies for the on-device batch_objects
     std::vector<uint8_t> key8(n ? n : 1, 0);
-    c->any_blend = false;
+    c->sort_live_blend = 0; c->sort_wide_keys = 0;
     for (uint32_t i = 0; i < n; ++i) {
-        if (key[i] >= 64) ok = false;
-        if (key[i] == 2 && (flags[i] & 1)) c->any_blend = true;   // TransparencyType::Blend as u64 (pbr/material.rs:497-503)
-        const uint32_t reason = (flags[i] & 2) ? 0u : 1u;
-        key8[i] = (uint8_t)(((((uint32_t)key[i] & 63u) << 1 | reason) << 1) | ((flags[i] & 4) ? 1u : 0u));
+        c->sort_wide_keys += sort_wide_key(key[i]);
+        c->sort_live_blend += sort_live_blend(key[i], flags[i]);
+        key8[i] = sort_key8(key[i], flags[i]);
     }
     uint32_t cap2 = c->sort_dev_cap;
     R3_TRY(r3_reserve_t(c, &c->d_sort_key8, &c->sort_dev_cap, n));
@@ -317,7 +332,7 @@ R3_EXPORT int r3_set_object_sort_info(r3_ctx* c, const uint64_t* key, const uint
     R3_CUDA(c, r3_stream_sync(c));
     r3_new_frame_epoch(c);
     c->have_live = true;
-    c->gpu_batching_ok = ok && n < (1u << 24) && !getenv("R3_HOST_BATCHING");
+    sort_derive(c);
     return R3_OK;
 }
 R3_EXPORT int r3_set_mesh_buffer(r3_ctx* c, const void* bytes, uint64_t nbytes) {
@@ -357,6 +372,186 @@ R3_EXPORT int r3_set_textures(r3_ctx* c, const r3_texture_desc* descs, uint32_t 
     if (nbytes) R3_CUDA(c, cudaMemcpyAsync(c->d_texels, texels, nbytes, cudaMemcpyHostToDevice, c->stream));
     R3_CUDA(c, r3_stream_sync(c));
     c->n_textures = n;
+    c->texel_bytes = nbytes;
+    return R3_OK;
+}
+
+// ------------------------------------------------------------------ incremental world updates
+// MeshManager::add / reallocate_buffers (managers/mesh.rs:123-184,264-308) for the mesh megabuffer and the texel blob: write
+// `nbytes` at `offset` of a blob whose first `used` bytes are live.  A write past the capacity grows the allocation to the next power of
+// two of end + slack, keeping its contents by a device copy (r3_reserve with keep); bytes between the old end and `offset` read 0; the
+// `slack` bytes past the end stay allocated (the triangle test's bulk copies may read into them).  Returns the new live size in *used.
+static int blob_write(r3_ctx* c, void** ptr, uint64_t* cap_bytes, uint64_t* used, uint64_t offset, const void* src, uint64_t nbytes, uint64_t slack) {
+    const uint64_t end = offset + nbytes;
+    if (end + slack > *cap_bytes || !*ptr) {
+        uint64_t p = 16;
+        while (p < end + slack) p <<= 1;
+        R3_TRY(r3_reserve(c, ptr, cap_bytes, p, 1, true, false));
+    }
+    if (offset > *used) R3_CUDA(c, cudaMemsetAsync((uint8_t*)*ptr + *used, 0, offset - *used, c->stream));
+    if (nbytes) R3_CUDA(c, cudaMemcpyAsync((uint8_t*)*ptr + offset, src, nbytes, cudaMemcpyHostToDevice, c->stream));
+    R3_CUDA(c, r3_stream_sync(c));   // the host bytes are only borrowed for the call
+    if (end > *used) *used = end;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_update_mesh_buffer(r3_ctx* c, uint64_t byte_offset, const void* bytes, uint64_t nbytes) {
+    if (!c) return R3_E_INVALID;
+    if (nbytes == 0) return R3_OK;
+    if (!bytes || (byte_offset & 3) || (nbytes & 3)) return r3_fail(c, R3_E_INVALID, "update_mesh_buffer: offset and size must be multiples of 4");
+    if (byte_offset + nbytes < byte_offset || (byte_offset + nbytes) / 4 + 4 > (1ull << 62)) return r3_fail(c, R3_E_INVALID, "update_mesh_buffer: range overflows");
+    cudaSetDevice(c->device);
+    uint64_t cap = c->d_mesh ? c->mesh_cap * 4 : 0, used = c->mesh_words * 4;
+    void* p = c->d_mesh;
+    const int rc = blob_write(c, &p, &cap, &used, byte_offset, bytes, nbytes, 16);   // >= 4 words of slack, as r3_set_mesh_buffer keeps
+    c->d_mesh = (uint32_t*)p; c->mesh_cap = cap / 4;
+    if (rc == R3_OK) c->mesh_words = used / 4;
+    return rc;
+}
+
+static int check_texture_desc(r3_ctx* c, const r3_texture_desc& d, uint64_t blob_bytes, const char* who) {
+    if (!d.width || !d.height || !d.mip_count || d.mip_count > 32 || d.format >= R3_TEXFMT_COUNT) return r3_fail(c, R3_E_INVALID, who);
+    uint64_t total = 0;
+    for (uint32_t l = 0; l < d.mip_count; ++l) total += R3_TEXFMT_LEVEL_BYTES(d.format, (d.width >> l) ? (d.width >> l) : 1u, (d.height >> l) ? (d.height >> l) : 1u);
+    if (d.byte_offset % 16 || d.byte_offset + total > blob_bytes) return r3_fail(c, R3_E_INVALID, who);
+    return R3_OK;
+}
+
+// TextureManager::add / fill (managers/texture.rs:98-251), a range of the table at a time
+R3_EXPORT int r3_update_textures(r3_ctx* c, uint32_t first, const r3_texture_desc* descs, uint32_t n, uint64_t blob_offset, const void* texels, uint64_t nbytes) {
+    if (!c) return R3_E_INVALID;
+    if (n == 0 && nbytes == 0) return R3_OK;
+    if ((!descs && n) || (!texels && nbytes)) return r3_fail(c, R3_E_INVALID, "update_textures: null");
+    if (first > c->n_textures || (uint64_t)first + n > 0xFFFFFFFFull) return r3_fail(c, R3_E_INVALID, "update_textures: first entry past the end of the table");
+    if (blob_offset % 16 || blob_offset + nbytes < blob_offset) return r3_fail(c, R3_E_INVALID, "update_textures: texel offset must be 16-aligned");
+    const uint64_t blob = blob_offset + nbytes > c->texel_bytes ? blob_offset + nbytes : c->texel_bytes;
+    for (uint32_t i = 0; i < n; ++i) R3_TRY(check_texture_desc(c, descs[i], blob, "update_textures: bad descriptor or mip chain outside the texel blob"));
+    cudaSetDevice(c->device);
+    if (nbytes) {
+        void* p = c->d_texels;
+        uint64_t used = c->texel_bytes;
+        const int rc = blob_write(c, &p, &c->texels_cap, &used, blob_offset, texels, nbytes, 16);
+        c->d_texels = (uint8_t*)p;
+        R3_TRY(rc);
+        c->texel_bytes = used;
+    }
+    if (n) {
+        const uint64_t need = (uint64_t)first + n;
+        if (need > c->tex_descs_cap || !c->d_tex_descs) {
+            uint64_t p = 16;
+            while (p < need) p <<= 1;
+            R3_TRY(r3_reserve_t(c, &c->d_tex_descs, &c->tex_descs_cap, p, true));
+        }
+        R3_CUDA(c, cudaMemcpyAsync(c->d_tex_descs + first, descs, (size_t)n * sizeof(r3_texture_desc), cudaMemcpyHostToDevice, c->stream));
+        R3_CUDA(c, r3_stream_sync(c));
+        if (need > c->n_textures) c->n_textures = (uint32_t)need;
+    }
+    return R3_OK;
+}
+
+// one thread per distinct slot: upd = slots[m] | key8 + live << 8 [m] | location bits [3 m]
+__global__ void scatter_sort_info_kernel(const uint32_t* __restrict__ upd, uint32_t m, uint8_t* __restrict__ key8, float* __restrict__ loc, uint32_t* __restrict__ live_bits) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint32_t s = upd[i], kl = upd[m + i];
+    key8[s] = (uint8_t)(kl & 255u);
+    const uint32_t* l = upd + 2 * (size_t)m + 3 * (size_t)i;
+    loc[3 * (size_t)s] = __uint_as_float(l[0]); loc[3 * (size_t)s + 1] = __uint_as_float(l[1]); loc[3 * (size_t)s + 2] = __uint_as_float(l[2]);
+    const uint32_t bit = 1u << (s & 31u);   // slots of one word are written by different threads: as split_slots_kernel does
+    if (kl & 256u) atomicOr(&live_bits[s >> 5], bit);
+    else atomicAnd(&live_bits[s >> 5], ~bit);
+}
+
+// FreelistDerivedBuffer::apply's scatter of the stale entries (util/freelist/buffer.rs:85-97) for the facts batch_objects reads
+R3_EXPORT int r3_update_object_sort_info(r3_ctx* c, const uint32_t* slots, const uint64_t* key, const uint8_t* flags, const float* loc, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (n == 0) return R3_OK;
+    if (!slots || !key || !flags || !loc) return r3_fail(c, R3_E_INVALID, "update_object_sort_info: null");
+    const size_t count = c->sort_key.size();
+    if (!c->have_live) return r3_fail(c, R3_E_STATE, "update_object_sort_info before set_object_sort_info");
+    for (uint32_t i = 0; i < n; ++i)
+        if (slots[i] >= count) return r3_fail(c, R3_E_INVALID, "update_object_sort_info: slot beyond the sort info");
+    cudaSetDevice(c->device);
+    // the host mirrors (read by the host batching) take the entries in order: of a slot listed twice, the later entry wins
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t s = slots[i];
+        c->sort_wide_keys += sort_wide_key(key[i]) - sort_wide_key(c->sort_key[s]);
+        c->sort_live_blend += sort_live_blend(key[i], flags[i]) - sort_live_blend(c->sort_key[s], c->sort_flags[s]);
+        c->sort_key[s] = key[i]; c->sort_flags[s] = flags[i];
+        memcpy(&c->sort_loc[3 * (size_t)s], loc + 3 * (size_t)i, 12);
+    }
+    // the device gets the final value of each distinct slot once
+    std::vector<uint32_t> distinct;
+    const uint32_t* list = slots;
+    uint32_t m = n;
+    for (uint32_t i = 1; i < n; ++i)
+        if (slots[i] <= slots[i - 1]) {   // not strictly ascending: there may be repeats
+            distinct.assign(slots, slots + n);
+            std::sort(distinct.begin(), distinct.end());
+            distinct.erase(std::unique(distinct.begin(), distinct.end()), distinct.end());
+            list = distinct.data(); m = (uint32_t)distinct.size();
+            break;
+        }
+    std::vector<uint32_t> upd((size_t)m * 5);
+    for (uint32_t i = 0; i < m; ++i) {
+        const uint32_t s = list[i];
+        upd[i] = s;
+        upd[(size_t)m + i] = sort_key8(c->sort_key[s], c->sort_flags[s]) | ((c->sort_flags[s] & 1u) << 8);
+        memcpy(&upd[2 * (size_t)m + 3 * (size_t)i], &c->sort_loc[3 * (size_t)s], 12);
+    }
+    R3_TRY(r3_reserve(c, &c->d_scratch, &c->scratch_cap, upd.size() * 4, 1, false, false));
+    R3_CUDA(c, cudaMemcpyAsync(c->d_scratch, upd.data(), upd.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    scatter_sort_info_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>((const uint32_t*)c->d_scratch, m, c->d_sort_key8, c->d_sort_loc, c->d_live_bits);
+    R3_CHECK_LAUNCH(c, "scatter_sort_info_kernel");
+    R3_CUDA(c, r3_stream_sync(c));
+    r3_new_frame_epoch(c);
+    sort_derive(c);
+    return R3_OK;
+}
+
+// FreelistDerivedBuffer::apply's growth (util/freelist/buffer.rs:66-83): a larger buffer that starts with a device copy of the old one
+R3_EXPORT int r3_resize_objects(r3_ctx* c, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (n < c->n_slots) return r3_fail(c, R3_E_INVALID, "resize_objects: the object buffer only grows");
+    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "resize_objects: the object buffer is borrowed (r3_set_objects_device)");
+    if (c->peer.connected) return r3_fail(c, R3_E_STATE, "resize_objects: peer buffers are sized for the current world");
+    for (const r3_camera& k : c->cams)
+        if (k.ex_connected) return r3_fail(c, R3_E_STATE, "resize_objects: a visible-set exchange is sized for the current world");
+    if (n == c->n_slots) return R3_OK;
+    cudaSetDevice(c->device);
+    const uint32_t old_n = c->n_slots;
+    if (n > c->objects_cap || !c->d_objects) R3_TRY(r3_reserve_t(c, &c->d_objects, &c->objects_cap, r3_hot_capacity(n), true));
+    R3_CUDA(c, cudaMemsetAsync(c->d_objects + old_n, 0, (size_t)(n - old_n) * sizeof(r3_object), c->stream));
+    R3_TRY(r3_grow_hot(c, old_n, n));
+    c->n_slots = n;   // zero records have no triangles: the cached invocation bounds stay valid
+    const size_t sorted = c->sort_key.size();
+    if (c->have_live && sorted < n) {
+        // the sort info grows with zeros as well: key 0, flags 0 (not live), location 0
+        c->sort_key.resize(n, 0); c->sort_flags.resize(n, 0); c->sort_loc.resize(3 * (size_t)n, 0.0f);
+        const uint32_t old_words = (uint32_t)((sorted + 31) / 32), words = (n + 31) / 32;
+        R3_TRY(r3_reserve_t(c, &c->d_live_bits, &c->live_bits_cap, words, true));
+        const uint32_t whole = (sorted & 31u) ? old_words : (uint32_t)(sorted / 32);
+        if (words > whole) R3_CUDA(c, cudaMemsetAsync(c->d_live_bits + whole, 0, (size_t)(words - whole) * 4, c->stream));
+        if (sorted & 31u) R3_TRY(r3_launch_mask_word(c, c->d_live_bits + sorted / 32, nullptr, (1u << (sorted & 31u)) - 1u));
+        if (n > c->sort_dev_cap || !c->d_sort_key8) {
+            const uint32_t cap = (uint32_t)r3_hot_capacity(n);
+            uint8_t* k8 = nullptr; float* l = nullptr;
+            R3_CUDA(c, cudaMalloc((void**)&k8, cap));
+            R3_CUDA(c, cudaMalloc((void**)&l, ((size_t)cap * 3 + 4) * 4));
+            if (sorted) {
+                R3_CUDA(c, cudaMemcpyAsync(k8, c->d_sort_key8, sorted, cudaMemcpyDeviceToDevice, c->stream));
+                R3_CUDA(c, cudaMemcpyAsync(l, c->d_sort_loc, sorted * 12, cudaMemcpyDeviceToDevice, c->stream));
+            }
+            R3_CUDA(c, r3_stream_sync(c));
+            cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc);
+            c->d_sort_key8 = k8; c->d_sort_loc = l; c->sort_dev_cap = cap;
+        }
+        R3_CUDA(c, cudaMemsetAsync(c->d_sort_key8 + sorted, 0, n - sorted, c->stream));
+        R3_CUDA(c, cudaMemsetAsync(c->d_sort_loc + 3 * sorted, 0, (n - sorted) * 12, c->stream));
+        r3_new_frame_epoch(c);
+        sort_derive(c);
+    }
+    R3_CUDA(c, r3_stream_sync(c));
     return R3_OK;
 }
 R3_EXPORT int r3_set_skybox(r3_ctx* c, const r3_texture_desc* desc, const void* texels, uint64_t nbytes) {

@@ -403,6 +403,12 @@ int r3_launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode) {
     return R3_OK;
 }
 
+uint64_t r3_hot_capacity(uint64_t want) {
+    uint64_t cap = 1024;
+    while (cap < want) cap *= 2;
+    if (cap > want + want / 8 && want > (1u << 20)) cap = want + want / 8;   // large worlds: 12.5% head room instead of a power of two
+    return cap;
+}
 // (re)build the dense hot arrays from the AoS records (all slots)
 int r3_split_objects(r3_ctx* c) {
     const uint32_t n = c->n_slots;
@@ -410,9 +416,7 @@ int r3_split_objects(r3_ctx* c) {
     if (want > c->hot_cap) {
         cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits);
         c->d_hot_xyz = nullptr; c->d_hot_w = nullptr; c->d_hot_sphere = nullptr; c->d_enabled_bits = nullptr; c->d_affine_bits = nullptr; c->hot_cap = 0;
-        uint64_t cap = 1024;
-        while (cap < want) cap *= 2;
-        if (cap > want + want / 8 && want > (1u << 20)) cap = want + want / 8;   // large worlds: 12.5% head room instead of a power of two
+        const uint64_t cap = r3_hot_capacity(want);
         R3_CUDA(c, cudaMalloc((void**)&c->d_hot_xyz, cap * 48));
         R3_CUDA(c, cudaMalloc((void**)&c->d_hot_w, cap * 16));
         R3_CUDA(c, cudaMalloc((void**)&c->d_hot_sphere, cap * 16));
@@ -436,6 +440,58 @@ int r3_split_slots(r3_ctx* c, const uint32_t* d_slots, uint32_t n) {
                                                                     reinterpret_cast<float*>(c->d_hot_xyz), reinterpret_cast<float*>(c->d_hot_w), c->d_hot_sphere,
                                                                     c->d_enabled_bits, c->d_affine_bits);
     R3_CHECK_LAUNCH(c, "split_slots_kernel");
+    return R3_OK;
+}
+namespace {
+__global__ void mask_word_kernel(uint32_t* word_a, uint32_t* word_b, uint32_t keep_mask) {
+    if (word_a) *word_a &= keep_mask;
+    if (word_b) *word_b &= keep_mask;
+}
+}  // namespace
+int r3_launch_mask_word(r3_ctx* c, uint32_t* word_a, uint32_t* word_b, uint32_t keep_mask) {
+    mask_word_kernel<<<1, 1, 0, c->stream>>>(word_a, word_b, keep_mask);
+    R3_CHECK_LAUNCH(c, "mask_word_kernel");
+    return R3_OK;
+}
+// r3_resize_objects: the hot copies of slots [0, old_n) are kept by a device copy (FreelistDerivedBuffer::apply, buffer.rs:66-83);
+// slots [old_n, n) are zero records: rows, row 3 and sphere 0, enabled 0, affine 0 (row 3 is not (0, 0, 0, 1)) — what
+// split_objects_kernel derives from them.  Bits at or past old_n read 0, also in the old last partial word.
+int r3_grow_hot(r3_ctx* c, uint32_t old_n, uint32_t n) {
+    if (!c->hot_valid) old_n = 0;
+    const uint64_t old_words = ((uint64_t)old_n + 31) / 32;
+    if ((uint64_t)n > c->hot_cap || !c->d_hot_xyz) {
+        const uint64_t cap = r3_hot_capacity(n ? n : 1), bit_words = (cap + 31) / 32 + 1;
+        float4 *xyz = nullptr, *w = nullptr, *sph = nullptr;
+        uint32_t *en = nullptr, *af = nullptr;
+        R3_CUDA(c, cudaMalloc((void**)&xyz, cap * 48));
+        R3_CUDA(c, cudaMalloc((void**)&w, cap * 16));
+        R3_CUDA(c, cudaMalloc((void**)&sph, cap * 16));
+        R3_CUDA(c, cudaMalloc((void**)&en, bit_words * 4));
+        R3_CUDA(c, cudaMalloc((void**)&af, bit_words * 4));
+        if (old_n) {
+            R3_CUDA(c, cudaMemcpyAsync(xyz, c->d_hot_xyz, (size_t)old_n * 48, cudaMemcpyDeviceToDevice, c->stream));
+            R3_CUDA(c, cudaMemcpyAsync(w, c->d_hot_w, (size_t)old_n * 16, cudaMemcpyDeviceToDevice, c->stream));
+            R3_CUDA(c, cudaMemcpyAsync(sph, c->d_hot_sphere, (size_t)old_n * 16, cudaMemcpyDeviceToDevice, c->stream));
+            R3_CUDA(c, cudaMemcpyAsync(en, c->d_enabled_bits, old_words * 4, cudaMemcpyDeviceToDevice, c->stream));
+            R3_CUDA(c, cudaMemcpyAsync(af, c->d_affine_bits, old_words * 4, cudaMemcpyDeviceToDevice, c->stream));
+        }
+        R3_CUDA(c, r3_stream_sync(c));
+        cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits);
+        c->d_hot_xyz = xyz; c->d_hot_w = w; c->d_hot_sphere = sph; c->d_enabled_bits = en; c->d_affine_bits = af; c->hot_cap = cap;
+    }
+    const uint64_t first_word = old_n / 32, new_words = ((uint64_t)n + 31) / 32;
+    if (n > old_n) {
+        R3_CUDA(c, cudaMemsetAsync(c->d_hot_xyz + (size_t)old_n * 3, 0, (size_t)(n - old_n) * 48, c->stream));
+        R3_CUDA(c, cudaMemsetAsync(c->d_hot_w + old_n, 0, (size_t)(n - old_n) * 16, c->stream));
+        R3_CUDA(c, cudaMemsetAsync(c->d_hot_sphere + old_n, 0, (size_t)(n - old_n) * 16, c->stream));
+    }
+    const uint64_t whole = (old_n & 31u) ? first_word + 1 : first_word;   // first word that holds no kept slot
+    if (new_words > whole) {
+        R3_CUDA(c, cudaMemsetAsync(c->d_enabled_bits + whole, 0, (new_words - whole) * 4, c->stream));
+        R3_CUDA(c, cudaMemsetAsync(c->d_affine_bits + whole, 0, (new_words - whole) * 4, c->stream));
+    }
+    if (old_n & 31u) R3_TRY(r3_launch_mask_word(c, c->d_enabled_bits + first_word, c->d_affine_bits + first_word, (1u << (old_n & 31u)) - 1u));
+    c->hot_valid = true;
     return R3_OK;
 }
 
