@@ -165,10 +165,10 @@ int r3_batch_objects(r3_ctx*, uint32_t camera, const float viewport_location[3],
 int r3_batch_counts(r3_ctx*, uint32_t camera, uint32_t* n_batches, uint32_t* n_regions, uint32_t* total_invocations);
 int r3_readback_batches(r3_ctx*, uint32_t camera, r3_batch_data* batches, r3_region* regions);
 /* which implementation of batch_objects ran last for this camera, and what it built: info[0] = 0 none / 1 on the device (radix sort +
- * block scans, no host sync) / 2 on the host (material keys >= 64, >= 2^24 slots, or a mesh large enough that a batch could reach the
- * max_dispatch_count x 256 split of batching.rs:196, which only the host path implements) / 3 on the device, order taken from the
- * frame-wide sort the cameras of one frame share (the sort key does not depend on the camera, batching.rs:156-157); info[1] = device overflow flag (always 0
- * given the check above; kept as a tripwire); info[2] = batches, info[3] = regions.  Blocks (one 32-byte readback). */
+ * block scans, no host sync; batches split at the max_dispatch_count x 256 limit of batching.rs:196 as on the host) / 2 on the host
+ * (material keys >= 64, >= 2^24 slots, or R3_HOST_BATCHING set) / 3 on the device, order taken from the
+ * frame-wide sort the cameras of one frame share (the sort key does not depend on the camera, batching.rs:156-157); info[1] = device overflow flag (always 0:
+ * the batch tables are sized by a proven bound; kept as a tripwire); info[2] = batches, info[3] = regions.  Blocks (one 32-byte readback). */
 int r3_batching_info(r3_ctx*, uint32_t camera, uint32_t info[4]);
 /* GpuCuller::cull (culler.rs:531-659) + cull.wgsl.  batches/regions == NULL uses the jobs of the last
  * r3_batch_objects call; otherwise the caller's own ShaderBatchDatas (a Rust batch_objects). */

@@ -749,13 +749,14 @@ R3_EXPORT int r3_batch_objects(r3_ctx* c, uint32_t camera, const float vp_loc[3]
     R3_CAM_OR_FAIL(c, camera);
     if (!vp_loc) return r3_fail(c, R3_E_INVALID, "batch_objects: null location");
     cudaSetDevice(c->device);
-    // The device path never splits a batch at the dispatch limit (batching.rs:196); it is only taken when no batch can reach it:
-    // 256 objects x the largest padded triangle count of any slot stays below max_dispatch_count x 256 invocations.  Worlds with
-    // such meshes (> ~65k triangles in one object), material keys >= 64 or >= 2^24 slots take the host path, which splits.
+    // Both paths split batches at the dispatch limit (batching.rs:196).  Material keys >= 64 and >= 2^24 slots (the sort key has no
+    // room for them) or R3_HOST_BATCHING take the host path.  So does a world whose padded total reaches 2^31 when a batch can reach the
+    // limit: the device path counts invocations in 32 bits and refuses it, and such a world always batched on the host.
     bool device = c->gpu_batching_ok && c->sort_key.size() >= cam->header.object_count;
     if (device) {
         R3_TRY(r3_compute_max_invocations(c));   // cached: one small reduction per object upload, never per frame
-        device = c->max_object_invocations * R3_BATCH_SIZE < (uint64_t)max_dispatch_count * R3_WORKGROUP_SIZE;
+        device = !(c->max_total_invocations >= (1ull << 31) &&
+                   c->max_object_invocations * R3_BATCH_SIZE >= (uint64_t)max_dispatch_count * R3_WORKGROUP_SIZE);
     }
     cam->batching_path = device ? 1 : 2;   // the device path raises it to 3 when it takes the frame-wide sort
     if (device) return r3_device_batch_objects(c, cam, vp_loc, max_dispatch_count);

@@ -10,15 +10,20 @@
 //   2. stable LSD radix sort on the 39 significant bits (5 passes of 8 bits; histogram, scan, stable scatter with
 //      __match_any_sync ranking) — ties keep the ascending-handle order of the visible list, the same tie rule the
 //      oracle and the host path use;
-//   3. batch build: one CTA per 256 sorted objects (block scans give invocation_start, region boundaries, local ids),
+//   3. batch partition, only for worlds where a batch can reach the dispatch limit of batching.rs:196 (256 x the largest
+//      padded triangle count >= max_dispatch_count x 256): where each batch starts, found on the device (see
+//      "dispatch-limit partition" below); otherwise a batch is a tile of 256 sorted objects;
+//   4. batch build: one CTA per batch (block scans give invocation_start, region boundaries, local ids),
 //      one scan over the batches (batch_base_invocation, global region ids), one fix-up pass that also swaps the
 //      per-camera previous-invocation map (batching.rs:226,230).
 // All counts stay on the device in the job header; the cull / raster kernels read them there.
-// Not covered on the device (the host path remains for them): material keys >= 64, more than 2^24 visible objects, a
-// single batch exceeding max_compute_workgroups_per_dimension*256 invocations (reported through the overflow flag).
+// Not covered on the device (the host path remains for them): material keys >= 64 and more than 2^24 visible objects (the
+// position no longer fits in the low 24 key bits; reported through the overflow flag).
+#include <algorithm>
 #include <cstring>
 
 #include <cooperative_groups.h>
+#include <cuda/atomic>
 
 #include "r3_common.cuh"
 #include "r3_scan.cuh"
@@ -220,17 +225,38 @@ __global__ void __launch_bounds__(SORT_THREADS) radix_scatter_kernel(const unsig
     radix_tile_scatter(keys_in, keys_out, nv, shift, base, s_gbase);
 }
 
-// ---- batch build (batching.rs:180-246), one CTA per 256 sorted objects
+// object slot of sorted position j: the low 24 key bits are the slot (frame-wide sort) or a position in `visible`
+__device__ __forceinline__ uint32_t sorted_slot(const unsigned long long* keys, const uint32_t* visible, uint32_t keys_hold_slots, uint32_t j) {
+    const uint32_t low = (uint32_t)(keys[j] & 0xFFFFFFull);
+    return keys_hold_slots ? low : visible[low];
+}
+
+// ---- batch build (batching.rs:180-246), one CTA per batch
 struct BuildParams {
     const unsigned long long* keys; const uint32_t* visible; const r3_object* objects;
     r3_batch_data* batches; uint32_t* header;
     uint32_t* batch_inv; uint32_t* batch_regions;         // per batch: total_invocations, number of regions
-    uint32_t* region_key; uint32_t* region_start;         // per (batch, batch-local region): material key, first invocation in the batch
+    const uint32_t* batch_start;                          // [header[1] + 1] first sorted object of each batch (dispatch-limit partition), or
+                                                          // nullptr: batch b is the sorted objects [256 b, 256 b + 256)
     r3_region* regions; uint32_t* region_first_inv;
     const uint32_t* prev_map; uint32_t* cur_map; uint32_t map_cap;
-    uint32_t n_batches_cap; uint64_t dispatch_limit;
+    uint64_t dispatch_limit;
     uint32_t keys_hold_slots;                             // low 24 key bits = the object slot (frame-wide sort) instead of a position in `visible`
 };
+
+// the sorted objects [*lo, *lo + *n) of batch b; false past the last batch
+__device__ __forceinline__ bool batch_range(const BuildParams& p, uint32_t nv, uint32_t b, uint32_t* lo, uint32_t* n) {
+    if (p.batch_start) {
+        if (b >= p.header[1]) return false;
+        *lo = p.batch_start[b];
+        *n = min(p.batch_start[b + 1] - *lo, 256u);
+    } else {
+        if (b * 256u >= nv) return false;
+        *lo = b * 256u;
+        *n = min(256u, nv - *lo);
+    }
+    return true;
+}
 
 // Mid-sized worlds (more than one CTA's worth, up to 256 tiles = 524288 visible objects): the whole sort — key generation and
 // the five histogram / offset / scatter passes — in ONE cooperative launch with grid-wide barriers between the phases instead of
@@ -277,14 +303,16 @@ __global__ void __launch_bounds__(256) batch_build_kernel(const __grid_constant_
     __shared__ uint32_t s_warp[256 / 32 + 1];
     __shared__ uint32_t s_start[256];
     __shared__ uint32_t s_first[256];
-    const uint32_t nv = p.header[0], b = blockIdx.x, i = threadIdx.x, j = b * 256u + i;
-    if (b * 256u >= nv) { if (i == 0) { p.batch_inv[b] = 0; p.batch_regions[b] = 0; } return; }
-    const bool valid = j < nv;
+    const uint32_t nv = p.header[0], b = blockIdx.x, i = threadIdx.x;
+    uint32_t lo, n;
+    if (!batch_range(p, nv, b, &lo, &n)) { if (i == 0) { p.batch_inv[b] = 0; p.batch_regions[b] = 0; } return; }
+    const uint32_t j = lo + i;
+    const bool valid = i < n;
     unsigned long long key = 0ull, prev_key = 0ull;
     uint32_t h = 0, tri = 0;
     if (valid) {
         key = p.keys[j];
-        h = p.keys_hold_slots ? (uint32_t)(key & 0xFFFFFFull) : p.visible[(uint32_t)(key & 0xFFFFFFull)];
+        h = sorted_slot(p.keys, p.visible, p.keys_hold_slots, j);
         tri = p.objects[h].index_count / 3u;                                  // batching.rs:192
         if (j > 0) prev_key = p.keys[j - 1];
     }
@@ -318,13 +346,13 @@ __global__ void __launch_bounds__(256) batch_build_kernel(const __grid_constant_
         info.previous_global_invocation = (h < p.map_cap) ? p.prev_map[h] : R3_NO_PREVIOUS;   // batching.rs:226
         info.atomic_capable = (k7 & 1u) ? 0u : 1u;         // SortingReason::Optimization (batching.rs:227)
         bd->object_culling_information[i] = info;
-        if (flag) { p.region_key[b * 256u + region_local] = mat; p.region_start[b * 256u + region_local] = start; }
     }
     if (i == 0) {
-        const uint32_t n_obj = min(256u, nv - b * 256u);
-        bd->total_objects = n_obj; bd->total_invocations = total_inv; bd->batch_base_invocation = 0;
-        p.batch_inv[b] = total_inv; p.batch_regions[b] = n_regions;
-        if ((uint64_t)total_inv >= p.dispatch_limit) atomicExch(&p.header[4], 1u);   // batching.rs:196 would have split the batch
+        bd->total_objects = n; bd->total_invocations = total_inv; bd->batch_base_invocation = 0;
+        p.batch_inv[b] = total_inv;
+        p.batch_regions[b] = n ? n_regions : 1u;           // the leading empty batch still closes one region (batching.rs:197-199)
+        // without the partition no batch may reach the limit (r3_device_batch_objects only skips it then): tripwire
+        if (!p.batch_start && (uint64_t)total_inv >= p.dispatch_limit) atomicExch(&p.header[4], 1u);
     }
 }
 
@@ -333,7 +361,7 @@ __global__ void __launch_bounds__(256) batch_build_kernel(const __grid_constant_
 // half, and the high half wraps exactly as a uint32_t sum of the invocations would.
 __global__ void __launch_bounds__(1024) batch_scan_kernel(const __grid_constant__ BuildParams p) {
     __shared__ unsigned long long s_warp[1024 / 32 + 1];
-    const uint32_t nv = p.header[0], nb = (nv + 255u) / 256u;
+    const uint32_t nv = p.header[0], nb = p.batch_start ? p.header[1] : (nv + 255u) / 256u;
     const unsigned long long tot = block_scan_excl_chunked<1024>(
         nb, s_warp, [&](uint32_t b) { return (unsigned long long)p.batch_inv[b] << 32 | p.batch_regions[b]; },
         [&](uint32_t b, unsigned long long e) { p.batch_inv[b] = (uint32_t)(e >> 32); p.batch_regions[b] = (uint32_t)e; });
@@ -345,22 +373,29 @@ __global__ void __launch_bounds__(1024) batch_scan_kernel(const __grid_constant_
 }
 
 __global__ void __launch_bounds__(256) batch_finalize_kernel(const __grid_constant__ BuildParams p) {
-    const uint32_t nv = p.header[0], b = blockIdx.x, i = threadIdx.x, j = b * 256u + i;
-    if (b * 256u >= nv) return;
+    const uint32_t nv = p.header[0], b = blockIdx.x, i = threadIdx.x;
+    uint32_t lo, n;
+    if (!batch_range(p, nv, b, &lo, &n)) return;
     r3_batch_data* bd = &p.batches[b];
     const uint32_t base_inv = p.batch_inv[b], base_reg = p.batch_regions[b];
     if (i == 0) bd->batch_base_invocation = base_inv;
-    if (j < nv) {
+    if (i < n) {
         r3_object_culling_info* info = &bd->object_culling_information[i];
         const uint32_t local_region = info->region_id;
         info->region_id = base_reg + local_region;
         if (info->object_id < p.map_cap) p.cur_map[info->object_id] = info->invocation_start + base_inv;   // batching.rs:230
         if (info->local_region_id == 0) {
             r3_region r;
-            r.job_index = b; r.bind_group_index = 0u; r.material_key = p.region_key[b * 256u + local_region];
+            r.job_index = b; r.bind_group_index = 0u; r.material_key = p.keys[lo + i] >> 57;
             p.regions[base_reg + local_region] = r;                                                            // batching.rs:199,238
-            p.region_first_inv[base_reg + local_region] = base_inv + p.region_start[b * 256u + local_region];
+            p.region_first_inv[base_reg + local_region] = base_inv + info->invocation_start;
         }
+    } else if (n == 0 && i == 0) {
+        // the leading empty batch (the first sorted object alone reaches the dispatch limit): its region carries that object's key
+        r3_region r;
+        r.job_index = b; r.bind_group_index = 0u; r.material_key = p.keys[lo] >> 57;
+        p.regions[base_reg] = r;
+        p.region_first_inv[base_reg] = base_inv;
     }
 }
 
@@ -388,18 +423,112 @@ __global__ void __launch_bounds__(RC_THREADS) rank_scatter_kernel(const unsigned
                                                                   const uint32_t* __restrict__ tile_counts, unsigned long long* __restrict__ keys_out,
                                                                   uint32_t* __restrict__ header) {
     __shared__ uint32_t s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t base = block_sum_u32<RC_THREADS>(tile_counts, blockIdx.x, s_warp);
     unsigned long long key = 0ull;
     const bool vis = rank_visible(gkeys, blockIdx.x * RC_THREADS + threadIdx.x, n, words, cap, &key);
-    const uint32_t bal = __ballot_sync(0xFFFFFFFFu, vis);
-    if (lane == 0) s_warp[warp] = __popc(bal);
-    __syncthreads();
-    uint32_t wbase = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < 32; ++w) { const uint32_t c = s_warp[w]; if (w < warp) wbase += c; total += c; }
-    if (vis) keys_out[base + wbase + __popc(bal & ((1u << lane) - 1u))] = key;
+    uint32_t total;
+    const uint32_t rank = block_flag_rank<RC_THREADS>(vis, s_warp, &total);
+    if (vis) keys_out[base + rank] = key;
     if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) { header[0] = base + total; header[4] = 0u; }
+}
+
+// ---- dispatch-limit partition (batching.rs:194-209): where the batches start when a batch can reach L = max_dispatch_count x 256
+// invocations.  Over the sorted objects j: T_j = triangles, P_j = round_up(T_j, 256), S_j = exclusive prefix of P.  The batch that
+// starts at s ends at next(s) = the first e in (s, min(s + 256, nv)) with S_e - S_s + T_e >= L, else min(s + 256, nv).  S_e + T_e is
+// non-decreasing in e (S_e + T_e <= S_e + P_e = S_{e+1}), so next(s) is one binary search.  The batch starts are the chain
+// 0 -> next(0) -> ..., marked without the host by pointer doubling: with J = next, K times  mark |= J(mark), J = J o J; after K steps
+// every n^i(0), i < 2^K, is marked.  The marks are set in place, read and written with relaxed atomics by the threads of one step: a
+// thread that already sees a mark set in the same step only marks a further chain member earlier, so the final set is the same.
+// Then the marks are compacted into batch_start[].  When T_0 >= L the reference first closes an EMPTY batch (batching.rs:196 with
+// nothing in it): batch_start then begins with a 0 of its own.  Launch counts and grids depend only on the capacity and K.
+struct PartitionParams {
+    const unsigned long long* keys; const uint32_t* visible; const r3_object* objects; uint32_t keys_hold_slots;
+    uint32_t* header;
+    uint32_t* s_local; uint32_t* f_local;   // [cap] S_j and S_j + T_j inside j's tile of 256
+    uint32_t* tile_sum;                     // [tiles] P summed over each tile, then their exclusive prefix
+    uint32_t* jump[2];                      // [cap + 1] J, ping-pong; J[nv] = nv
+    uint32_t* mark;                         // [cap + 1]
+    uint32_t* mark_count;                   // [cap / 1024 + 1] marks per 1024-object tile
+    uint32_t* batch_start;                  // [nb_max + 1]
+    uint64_t dispatch_limit; uint32_t nb_max;
+};
+
+__global__ void __launch_bounds__(256) partition_tile_kernel(const __grid_constant__ PartitionParams p) {
+    __shared__ uint32_t s_warp[256 / 32 + 1];
+    const uint32_t nv = p.header[0], j = blockIdx.x * 256u + threadIdx.x;
+    if (blockIdx.x * 256u >= nv) return;
+    const uint32_t tri = j < nv ? p.objects[sorted_slot(p.keys, p.visible, p.keys_hold_slots, j)].index_count / 3u : 0u;
+    uint32_t total;
+    const uint32_t s = block_scan_excl<256>((tri + 255u) & ~255u, s_warp, &total);
+    if (j < nv) { p.s_local[j] = s; p.f_local[j] = s + tri; }
+    if (threadIdx.x == 0) p.tile_sum[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(1024) partition_scan_kernel(const __grid_constant__ PartitionParams p) {
+    __shared__ uint32_t s_warp[1024 / 32 + 1];
+    block_scan_excl_chunked<1024>((p.header[0] + 255u) / 256u, s_warp, [&](uint32_t t) { return p.tile_sum[t]; },
+                                  [&](uint32_t t, uint32_t e) { p.tile_sum[t] = e; });
+}
+
+// next(s) for every s < nv (S and S + T of the 511 objects from this tile's first on are staged in shared memory), J[nv] = nv, mark = {0}
+__global__ void __launch_bounds__(256) partition_next_kernel(const __grid_constant__ PartitionParams p) {
+    __shared__ uint32_t s_f[512];
+    const uint32_t nv = p.header[0], base = blockIdx.x * 256u, s = base + threadIdx.x;
+    if (base > nv) return;
+    for (uint32_t k = threadIdx.x; k < 512u; k += 256u) {
+        const uint32_t e = base + k;
+        s_f[k] = e < nv ? p.tile_sum[e >> 8] + p.f_local[e] : 0u;   // S_e + T_e < 2^32: the padded total is below 2^31
+    }
+    __syncthreads();
+    if (s < nv) {
+        const uint32_t ss = p.tile_sum[s >> 8] + p.s_local[s];
+        uint32_t lo = s + 1u, hi = min(s + 256u, nv);
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if ((uint64_t)(s_f[mid - base] - ss) >= p.dispatch_limit) hi = mid;
+            else lo = mid + 1u;
+        }
+        p.jump[0][s] = lo;
+        p.mark[s] = s == 0u ? 1u : 0u;
+    } else if (s == nv) {
+        p.jump[0][s] = nv;
+        p.mark[s] = 0u;
+    }
+}
+
+// one doubling step: mark |= J(mark), out = J o J (out == nullptr on the last step)
+__global__ void __launch_bounds__(256) partition_jump_kernel(const uint32_t* __restrict__ header, const uint32_t* __restrict__ in, uint32_t* __restrict__ out, uint32_t* mark) {
+    using mark_ref = cuda::atomic_ref<uint32_t, cuda::thread_scope_device>;
+    const uint32_t s = blockIdx.x * 256u + threadIdx.x;
+    if (s > header[0]) return;
+    const uint32_t js = in[s];
+    if (mark_ref(mark[s]).load(cuda::memory_order_relaxed)) mark_ref(mark[js]).store(1u, cuda::memory_order_relaxed);
+    if (out) out[s] = in[js];
+}
+
+__global__ void __launch_bounds__(1024) partition_count_kernel(const __grid_constant__ PartitionParams p) {
+    const uint32_t nv = p.header[0], j = blockIdx.x * 1024u + threadIdx.x;
+    const int c = __syncthreads_count(j < nv && p.mark[j]);
+    if (threadIdx.x == 0) p.mark_count[blockIdx.x] = (uint32_t)c;
+}
+
+// the marked objects in ascending order -> batch_start[lead + rank]; the last CTA writes the batch count and the closing entry
+__global__ void __launch_bounds__(1024) partition_scatter_kernel(const __grid_constant__ PartitionParams p) {
+    __shared__ uint32_t s_warp[32];
+    const uint32_t nv = p.header[0], j = blockIdx.x * 1024u + threadIdx.x;
+    const uint32_t lead = (nv > 0u && (uint64_t)p.f_local[0] >= p.dispatch_limit) ? 1u : 0u;   // T_0 >= L: the leading empty batch
+    const uint32_t base = lead + block_sum_u32<1024>(p.mark_count, blockIdx.x, s_warp);
+    const bool m = j < nv && p.mark[j];
+    uint32_t total;
+    const uint32_t pos = base + block_flag_rank<1024>(m, s_warp, &total);
+    if (m && pos < p.nb_max) p.batch_start[pos] = j;
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
+        uint32_t nb = base + total;
+        if (nb > p.nb_max) { nb = p.nb_max; atomicExch(&p.header[4], 1u); }   // beyond the bound of r3_device_batch_objects: tripwire
+        p.header[1] = nb;
+        p.batch_start[nb] = nv;
+        if (lead) p.batch_start[0] = 0u;
+    }
 }
 
 // out[0] = sum over the slots of round_up(triangles, 256), out[1] = the largest such term
@@ -511,7 +640,20 @@ int r3_device_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], ui
     const int w = (cam->cache_idx == 0) ? 1 : 0;   // never overwrite the DrawCallSet cached for the predicted pass
     cam->cur = w;
     r3_jobs& j = cam->jobs[w];
-    const uint32_t nb_cap = (cap + 255u) / 256u + 1u, nr_cap = nb_cap + 64u;
+    // The partition only runs when some batch can reach the dispatch limit L: 256 objects of the largest padded size reach it.  Bound
+    // on the batch count then: at most floor(nv / 256) batches end at the object limit; if batch i ends at the dispatch limit because of
+    // object e, batches i and i + 1 hold >= (invocations of i) + T_e >= L invocations together, so every other such batch owns a
+    // disjoint pair worth >= L: at most 2 floor(total / L) + 1 of them end at the limit (the leading empty batch included).  With one
+    // batch left open at the end, nb <= ceil(nv / 256) + 2 floor(total / L) + 3.  Every batch but the leading empty one holds an object,
+    // so also nb <= nv + 1 (the only bound when L = 0).  total = the padded sum over every slot, nv <= cap.
+    const uint64_t dispatch_limit = (uint64_t)max_dispatch_count * R3_WORKGROUP_SIZE;
+    const bool partition = c->max_object_invocations * R3_BATCH_SIZE >= dispatch_limit;
+    uint64_t nb_max = (cap + 255u) / 256u;
+    if (partition) {
+        nb_max = (uint64_t)cap + 1u;
+        if (dispatch_limit) nb_max = std::min<uint64_t>(nb_max, (cap + 255u) / 256u + 2u * (c->max_total_invocations / dispatch_limit) + 3u);
+    }
+    const uint32_t nb_cap = (uint32_t)nb_max + 1u, nr_cap = nb_cap + 64u;
     R3_TRY(r3_reserve_t(c, &j.d_batches, &j.batches_cap, nb_cap));
     uint32_t rcap = j.regions_cap;
     R3_TRY(r3_reserve_t(c, &j.d_regions, &j.regions_cap, nr_cap));
@@ -525,8 +667,11 @@ int r3_device_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], ui
     R3_TRY(r3_reserve_t(c, &cam->d_sort_keys[1], &cam->sort_keys_cap2, (uint64_t)cap + 1));
     const uint32_t sort_blocks = (cap + SORT_TILE - 1) / SORT_TILE;
     R3_TRY(r3_reserve_t(c, &cam->d_sort_hist, &cam->sort_hist_cap, (uint64_t)sort_blocks * 256 + 1));
-    // batch scratch: batch_inv[nb] | batch_regions[nb] | region_key[nb*256] | region_start[nb*256]
-    R3_TRY(r3_reserve_t(c, &cam->d_batch_tmp, &cam->batch_tmp_cap, (uint64_t)nb_cap * (2 + 512)));
+    // batch scratch: batch_inv[nb] | batch_regions[nb], and with the partition:
+    //   batch_start[nb] | s_local[cap] | f_local[cap] | tile_sum[tiles] | jump[2][cap + 1] | mark_count[mtiles] | mark[cap + 1]
+    const uint32_t part_tiles = (cap + 255u) / 256u, mark_tiles = (cap + 1023u) / 1024u;
+    const uint64_t part_words = partition ? (uint64_t)nb_cap + 2ull * cap + part_tiles + 2ull * (cap + 1u) + mark_tiles + (cap + 1u) : 0u;
+    R3_TRY(r3_reserve_t(c, &cam->d_batch_tmp, &cam->batch_tmp_cap, (uint64_t)nb_cap * 2 + part_words));
     if (cam->prev_inv_cap < cap || !cam->d_prev_inv[0]) {
         for (int k = 0; k < 2; ++k) {
             uint32_t* n = nullptr;
@@ -572,10 +717,38 @@ int r3_device_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], ui
         BuildParams p;
         p.keys = sorted_keys; p.visible = cam->d_visible; p.objects = c->d_objects; p.keys_hold_slots = keys_hold_slots ? 1u : 0u;
         p.batches = j.d_batches; p.header = j.d_header;
-        p.batch_inv = cam->d_batch_tmp; p.batch_regions = p.batch_inv + nb_cap; p.region_key = p.batch_regions + nb_cap; p.region_start = p.region_key + (size_t)nb_cap * 256;
+        p.batch_inv = cam->d_batch_tmp; p.batch_regions = p.batch_inv + nb_cap; p.batch_start = nullptr;
         p.regions = j.d_regions; p.region_first_inv = j.d_region_first_inv;
         p.prev_map = cam->d_prev_inv[prev]; p.cur_map = cam->d_prev_inv[cur]; p.map_cap = cam->prev_inv_cap;
-        p.n_batches_cap = nb_cap; p.dispatch_limit = (uint64_t)max_dispatch_count * R3_WORKGROUP_SIZE;
+        p.dispatch_limit = dispatch_limit;
+        if (partition) {
+            PartitionParams q;
+            q.keys = sorted_keys; q.visible = cam->d_visible; q.objects = c->d_objects; q.keys_hold_slots = p.keys_hold_slots;
+            q.header = j.d_header;
+            q.batch_start = p.batch_regions + nb_cap;
+            q.s_local = q.batch_start + nb_cap; q.f_local = q.s_local + cap; q.tile_sum = q.f_local + cap;
+            q.jump[0] = q.tile_sum + part_tiles; q.jump[1] = q.jump[0] + cap + 1; q.mark_count = q.jump[1] + cap + 1;
+            q.mark = q.mark_count + mark_tiles;
+            q.dispatch_limit = dispatch_limit; q.nb_max = (uint32_t)nb_max;
+            const uint32_t jump_blocks = (cap + 1u + 255u) / 256u;
+            partition_tile_kernel<<<part_tiles, 256, 0, c->stream>>>(q);
+            R3_CHECK_LAUNCH(c, "partition_tile_kernel");
+            partition_scan_kernel<<<1, 1024, 0, c->stream>>>(q);
+            R3_CHECK_LAUNCH(c, "partition_scan_kernel");
+            partition_next_kernel<<<jump_blocks, 256, 0, c->stream>>>(q);
+            R3_CHECK_LAUNCH(c, "partition_next_kernel");
+            int steps = 0;                                 // K = ceil(log2(nb_max)): 2^K >= the batches a chain can start
+            while ((1ull << steps) < nb_max) ++steps;
+            for (int k = 0; k < steps; ++k) {
+                partition_jump_kernel<<<jump_blocks, 256, 0, c->stream>>>(j.d_header, q.jump[k & 1], k + 1 < steps ? q.jump[(k + 1) & 1] : nullptr, q.mark);
+                R3_CHECK_LAUNCH(c, "partition_jump_kernel");
+            }
+            partition_count_kernel<<<mark_tiles, 1024, 0, c->stream>>>(q);
+            R3_CHECK_LAUNCH(c, "partition_count_kernel");
+            partition_scatter_kernel<<<mark_tiles, 1024, 0, c->stream>>>(q);
+            R3_CHECK_LAUNCH(c, "partition_scatter_kernel");
+            p.batch_start = q.batch_start;
+        }
         batch_build_kernel<<<nb_cap - 1, 256, 0, c->stream>>>(p);
         R3_CHECK_LAUNCH(c, "batch_build_kernel");
         batch_scan_kernel<<<1, 1024, 0, c->stream>>>(p);
@@ -598,7 +771,7 @@ int r3_download_jobs(r3_ctx* c, r3_camera* cam) {
     uint32_t hdr[8] = {0};
     R3_CUDA(c, cudaMemcpyAsync(hdr, j.d_header, 32, cudaMemcpyDeviceToHost, c->stream));
     R3_CUDA(c, r3_stream_sync(c));
-    if (hdr[4]) return r3_fail(c, R3_E_INVALID, "device batch_objects overflow (batch beyond the dispatch limit or > 2^24 visible objects): use host batching");
+    if (hdr[4]) return r3_fail(c, R3_E_INVALID, "device batch_objects overflow (batch count beyond its bound, or > 2^24 visible objects): use host batching");
     j.batches.resize(hdr[1]); j.regions.resize(hdr[2]);
     if (hdr[1]) R3_CUDA(c, cudaMemcpyAsync(j.batches.data(), j.d_batches, (size_t)hdr[1] * sizeof(r3_batch_data), cudaMemcpyDeviceToHost, c->stream));
     if (hdr[2]) R3_CUDA(c, cudaMemcpyAsync(j.regions.data(), j.d_regions, (size_t)hdr[2] * sizeof(r3_region), cudaMemcpyDeviceToHost, c->stream));

@@ -92,6 +92,27 @@ __device__ __forceinline__ uint32_t block_sum_u32(const uint32_t* __restrict__ c
     return v;
 }
 
+// Stream compaction inside a block of THREADS threads: the number of set flags of the threads in front of this one (thread order),
+// and the block's count in *total.  s_warp: THREADS / 32 entries; writing it after the call needs a __syncthreads() first.
+template <int THREADS>
+__device__ __forceinline__ uint32_t block_flag_rank(bool flag, uint32_t* s_warp, uint32_t* total) {
+    constexpr int WARPS = THREADS / 32;
+    static_assert(THREADS % 32 == 0 && WARPS <= 32, "block_flag_rank: whole warps, at most 1024 threads");
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t bal = __ballot_sync(0xFFFFFFFFu, flag);
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    __syncthreads();
+    uint32_t before = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < WARPS; ++w) {
+        const uint32_t c = s_warp[w];
+        if (w < warp) before += c;
+        tot += c;
+    }
+    *total = tot;
+    return before + __popc(bal & ((1u << lane) - 1u));
+}
+
 // Ordered expansion of the warp's 32 visibility words (one per lane, lane j's word covering ids id_base + 32 j .. + 31) into
 // ascending ids: set bit b of lane j's word goes to position pos_j + (set bits of that word below b), pos_j being lane j's
 // exclusive prefix.  store(position, id) writes one entry.

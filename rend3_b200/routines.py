@@ -83,10 +83,12 @@ class BaseRenderGraphSettings:
 
 
 class GpuCuller:
-    """culling/culler.rs:185-714, bound to one backend context."""
+    """culling/culler.rs:185-714, bound to one backend context.  `max_compute_workgroups_per_dimension` stands in for
+    renderer.limits (batching.rs:189): batch_objects closes a batch before it reaches that many 256-invocation workgroups."""
 
-    def __init__(self, backend: Backend):
+    def __init__(self, backend: Backend, max_compute_workgroups_per_dimension: int = 65535):
         self.backend = backend
+        self.max_compute_workgroups_per_dimension = max_compute_workgroups_per_dimension
 
     def object_uniform_upload(self, eval_output: EvalOutput, camera: CameraState, camera_specifier: int,
                               resolution: Tuple[int, int], samples: int = 1, mode: int = CB_BAKE | CB_CULL):
@@ -95,16 +97,16 @@ class GpuCuller:
 
     def cull(self, eval_output: EvalOutput, camera_specifier: int):
         """add_culling_to_graph (culler.rs:682-713): batch_objects then cull."""
-        self.backend.batch_objects(camera_specifier, eval_output.camera.location())
+        self.backend.batch_objects(camera_specifier, eval_output.camera.location(), self.max_compute_workgroups_per_dimension)
         self.backend.cull(camera_specifier)
 
 
 class BaseRenderGraph:
     """base.rs:103-186 collapsed to a call sequence."""
 
-    def __init__(self, backend: Backend):
+    def __init__(self, backend: Backend, max_compute_workgroups_per_dimension: int = 65535):
         self.backend = backend
-        self.gpu_culler = GpuCuller(backend)
+        self.gpu_culler = GpuCuller(backend, max_compute_workgroups_per_dimension)
         self._resolution: Optional[Tuple[int, int]] = None
 
     def upload_world(self, ev: EvalOutput):
