@@ -1,0 +1,121 @@
+/* r3_anim_check.h — argument checks of r3_set_animations / r3_set_pose_jobs, shared by the library and its CPU oracle so that both
+ * reject exactly the same inputs.  Plain C99 / C++, header only.
+ *
+ * The checks turn the reference's panic sites into errors (rend3-anim/src/lib.rs:166-175, 190; skeleton.rs:151-162):
+ *   an empty key channel (`times.len() - 1` underflow), fewer values than key times, a NaN or negative duration (f32::clamp's assert),
+ *   a target joint count above the skin's (set_joint_matrices' assert), a target outside the joint buffer, an index out of range, an
+ *   order that is not a permutation listing parents first.
+ * One departure: key times must be finite, >= 0 and strictly increasing (glTF 2.0 §3.11 requires it).  That is what lets a binary
+ * search return the reference's linear "first key with time > t" for every t, NaN included (no key compares greater: the last key).
+ * Two jobs may not write overlapping joint ranges (the order in which they land would be unspecified). */
+#ifndef R3_ANIM_CHECK_H
+#define R3_ANIM_CHECK_H
+
+#include <math.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "rend3_b200.h"
+
+/* returns R3_OK, or R3_E_INVALID with *msg set; allocates nothing that outlives the call */
+static inline int r3_anim_check_track(const r3_anim_track* t, uint32_t stride, const float* keys, uint64_t n_keys, const char** msg) {
+    if (t->times == R3_ANIM_ABSENT) return R3_OK;
+    if (t->count == 0) { *msg = "animation: empty key channel"; return R3_E_INVALID; }
+    if (t->value_count < t->count) { *msg = "animation: fewer values than key times"; return R3_E_INVALID; }
+    if ((uint64_t)t->times + t->count > n_keys || (uint64_t)t->values + (uint64_t)t->value_count * stride > n_keys) {
+        *msg = "animation: key range outside the key blob"; return R3_E_INVALID;
+    }
+    for (uint32_t i = 0; i < t->count; ++i) {
+        const float v = keys[(uint64_t)t->times + i];
+        if (!(v >= 0.0f) || !isfinite(v) || (i > 0 && !(v > keys[(uint64_t)t->times + i - 1]))) {
+            *msg = "animation: key times must be finite, >= 0 and strictly increasing"; return R3_E_INVALID;
+        }
+    }
+    return R3_OK;
+}
+
+static inline int r3_anim_check_library(const r3_anim_library* L, const char** msg) {
+    *msg = "";
+    if (!L) { *msg = "set_animations: null library"; return R3_E_INVALID; }
+    if ((!L->skins && L->n_skins) || (!L->joints && L->n_joints) || (!L->order && L->n_joints) || (!L->clips && L->n_clips) ||
+        (!L->channels && L->n_channels) || (!L->keys && L->n_keys)) {
+        *msg = "set_animations: null array"; return R3_E_INVALID;
+    }
+    uint8_t* seen = (uint8_t*)malloc(L->n_joints ? L->n_joints : 1);
+    if (!seen) { *msg = "set_animations: out of host memory"; return R3_E_INVALID; }
+    int rc = R3_OK;
+    for (uint32_t s = 0; s < L->n_skins && rc == R3_OK; ++s) {
+        const r3_anim_skin sk = L->skins[s];
+        if ((uint64_t)sk.first_joint + sk.joint_count > L->n_joints) { *msg = "set_animations: skin joint range out of range"; rc = R3_E_INVALID; break; }
+        memset(seen, 0, sk.joint_count ? sk.joint_count : 1);
+        for (uint32_t i = 0; i < sk.joint_count; ++i) {
+            const uint32_t j = L->order[sk.first_joint + i];
+            if (j >= sk.joint_count || seen[j]) { *msg = "set_animations: order is not a permutation of the skin's joints"; rc = R3_E_INVALID; break; }
+            const uint32_t p = L->joints[sk.first_joint + j].parent;
+            if (p != R3_ANIM_NO_PARENT && p != R3_ANIM_PARENT_NOT_JOINT) {
+                if (p >= sk.joint_count) { *msg = "set_animations: parent joint index out of range"; rc = R3_E_INVALID; break; }
+                if (!seen[p]) { *msg = "set_animations: order lists a joint before its parent"; rc = R3_E_INVALID; break; }
+            }
+            seen[j] = 1;
+        }
+    }
+    free(seen);
+    if (rc != R3_OK) return rc;
+    for (uint32_t c = 0; c < L->n_clips; ++c) {
+        const r3_anim_clip cl = L->clips[c];
+        if (cl.skin >= L->n_skins) { *msg = "set_animations: clip skin out of range"; return R3_E_INVALID; }
+        if (!(cl.duration >= 0.0f)) { *msg = "set_animations: clip duration is NaN or negative"; return R3_E_INVALID; }
+        const r3_anim_skin sk = L->skins[cl.skin];
+        if ((uint64_t)cl.first_channel + sk.joint_count > L->n_channels) { *msg = "set_animations: clip channel range out of range"; return R3_E_INVALID; }
+        for (uint32_t k = 0; k < sk.joint_count; ++k) {
+            const r3_anim_channel* ch = &L->channels[cl.first_channel + k];
+            if (!ch->animated) continue;
+            if (r3_anim_check_track(&ch->translation, 3, L->keys, L->n_keys, msg) != R3_OK) return R3_E_INVALID;
+            if (r3_anim_check_track(&ch->rotation, 4, L->keys, L->n_keys, msg) != R3_OK) return R3_E_INVALID;
+            if (r3_anim_check_track(&ch->scale, 3, L->keys, L->n_keys, msg) != R3_OK) return R3_E_INVALID;
+        }
+    }
+    return R3_OK;
+}
+
+static inline int r3_anim_range_cmp(const void* a, const void* b) {
+    const uint64_t x = ((const uint64_t*)a)[0], y = ((const uint64_t*)b)[0];
+    return x < y ? -1 : x > y ? 1 : 0;
+}
+
+/* jobs against the skins / clips of the library that is set and a joint buffer of n_joint_matrices matrices */
+static inline int r3_anim_check_jobs(const r3_anim_skin* skins, const r3_anim_clip* clips, uint32_t n_clips, uint32_t n_joint_matrices,
+                                     const r3_pose_job* jobs, uint32_t n_jobs, const r3_pose_target* targets, uint32_t n_targets,
+                                     const char** msg) {
+    *msg = "";
+    if ((!jobs && n_jobs) || (!targets && n_targets)) { *msg = "set_pose_jobs: null array"; return R3_E_INVALID; }
+    uint64_t n_ranges = 0;
+    for (uint32_t i = 0; i < n_jobs; ++i) {
+        const r3_pose_job j = jobs[i];
+        if (j.clip >= n_clips) { *msg = "set_pose_jobs: clip out of range"; return R3_E_INVALID; }
+        if ((uint64_t)j.first_target + j.target_count > n_targets) { *msg = "set_pose_jobs: target range out of range"; return R3_E_INVALID; }
+        const uint32_t skin_joints = skins[clips[j.clip].skin].joint_count;
+        for (uint32_t t = 0; t < j.target_count; ++t) {
+            const r3_pose_target tg = targets[j.first_target + t];
+            if (tg.joint_count > skin_joints) { *msg = "set_pose_jobs: target joint count above the skin's"; return R3_E_INVALID; }
+            if ((uint64_t)tg.joint_matrix_base_offset + tg.joint_count > n_joint_matrices) { *msg = "set_pose_jobs: target outside the joint buffer"; return R3_E_INVALID; }
+            n_ranges += tg.joint_count != 0;
+        }
+    }
+    uint64_t* r = (uint64_t*)malloc(n_ranges ? n_ranges * 2 * sizeof(uint64_t) : 16);
+    if (!r) { *msg = "set_pose_jobs: out of host memory"; return R3_E_INVALID; }
+    uint64_t n = 0;
+    for (uint32_t i = 0; i < n_jobs; ++i)
+        for (uint32_t t = 0; t < jobs[i].target_count; ++t) {
+            const r3_pose_target tg = targets[jobs[i].first_target + t];
+            if (tg.joint_count) { r[2 * n] = tg.joint_matrix_base_offset; r[2 * n + 1] = (uint64_t)tg.joint_matrix_base_offset + tg.joint_count; ++n; }
+        }
+    qsort(r, n, 2 * sizeof(uint64_t), r3_anim_range_cmp);
+    int rc = R3_OK;
+    for (uint64_t i = 1; i < n; ++i)
+        if (r[2 * i] < r[2 * (i - 1) + 1]) { *msg = "set_pose_jobs: two targets write overlapping joint ranges"; rc = R3_E_INVALID; break; }
+    free(r);
+    return rc;
+}
+
+#endif /* R3_ANIM_CHECK_H */

@@ -278,4 +278,84 @@ typedef struct r3_skinning_input {
 } r3_skinning_input;
 R3_STATIC_ASSERT(sizeof(r3_skinning_input) == 40, "GpuSkinningInput");
 
+/* ---- skeletal animation (rend3-anim/src/lib.rs:37-263, posed on the device by r3_pose_skeletons) */
+#define R3_ANIM_NO_PARENT 0xFFFFFFFFu        /* the joint's node has no parent: global = local (lib.rs:253-255) */
+#define R3_ANIM_PARENT_NOT_JOINT 0xFFFFFFFEu /* the parent node is not a joint of the skin: global = IDENTITY * local (lib.rs:249) */
+#define R3_ANIM_ABSENT 0xFFFFFFFFu           /* r3_anim_track.times: the clip has no channel for this property */
+
+/* Skin — rend3-gltf Skin (inverse_bind_matrices, joints) + PerSkinData.joint_nodes_topological_order (lib.rs:39-52): the skin's joints
+ * are r3_anim_library.joints[first_joint, first_joint + joint_count), joint k of the skin being joints[first_joint + k] (k is the index
+ * into inverse_bind_matrices and into the skeleton's joint matrices); order[first_joint, first_joint + joint_count) lists the skin's joint
+ * indices in topological order, parents first. */
+typedef struct r3_anim_skin {
+    uint32_t first_joint;
+    uint32_t joint_count;
+} r3_anim_skin;
+R3_STATIC_ASSERT(sizeof(r3_anim_skin) == 8, "r3_anim_skin");
+
+/* One joint: its node's parent (node.parent through node_to_joint_idx, lib.rs:246), the node's bind pose
+ * (local_transform.to_scale_rotation_translation(), lib.rs:227-228, decomposed on the host) and inverse_bind_matrices[k] (lib.rs:216). */
+typedef struct r3_anim_joint {
+    float bind_translation[3];    /* @0 */
+    uint32_t parent;              /* @12 joint index within the skin, R3_ANIM_NO_PARENT or R3_ANIM_PARENT_NOT_JOINT */
+    float bind_rotation[4];       /* @16 quaternion x, y, z, w */
+    float bind_scale[3];          /* @32 */
+    uint32_t _pad;
+    float inverse_bind[16];       /* @48 column major */
+} r3_anim_joint;
+R3_STATIC_ASSERT(sizeof(r3_anim_joint) == 112, "r3_anim_joint");
+R3_STATIC_ASSERT(offsetof(r3_anim_joint, parent) == 12, "parent");
+R3_STATIC_ASSERT(offsetof(r3_anim_joint, bind_rotation) == 16, "bind_rotation");
+R3_STATIC_ASSERT(offsetof(r3_anim_joint, inverse_bind) == 48, "inverse_bind");
+
+/* AnimationChannel<T> (rend3-gltf/src/lib.rs:742-760): `count` key times at keys[times ..] and `value_count` values of 3 (translation,
+ * scale) or 4 (rotation x, y, z, w) floats at keys[values ..].  times == R3_ANIM_ABSENT: no channel for this property. */
+typedef struct r3_anim_track {
+    uint32_t times;
+    uint32_t values;
+    uint32_t count;
+    uint32_t value_count;
+} r3_anim_track;
+R3_STATIC_ASSERT(sizeof(r3_anim_track) == 16, "r3_anim_track");
+
+/* AnimationChannels of one joint in one clip (Animation::channels, keyed by node).  animated == 0: the clip has no channel for the
+ * joint's node, whose local matrix is then IDENTITY (lib.rs:219), not its bind pose. */
+typedef struct r3_anim_channel {
+    r3_anim_track translation;    /* @0 */
+    r3_anim_track rotation;       /* @16 */
+    r3_anim_track scale;          /* @32 */
+    uint32_t animated;            /* @48 */
+    uint32_t _pad[3];
+} r3_anim_channel;
+R3_STATIC_ASSERT(sizeof(r3_anim_channel) == 64, "r3_anim_channel");
+R3_STATIC_ASSERT(offsetof(r3_anim_channel, animated) == 48, "animated");
+
+/* Animation (rend3-gltf) bound to one skin, as AnimationData::from_gltf_scene binds them through node_to_joint_idx: channel k of the
+ * clip, for joint k of the skin, is r3_anim_library.channels[first_channel + k]. */
+typedef struct r3_anim_clip {
+    uint32_t skin;
+    uint32_t first_channel;
+    float duration;               /* Animation::duration: time is clamped to [0, duration] (lib.rs:190) */
+    uint32_t _pad;
+} r3_anim_clip;
+R3_STATIC_ASSERT(sizeof(r3_anim_clip) == 16, "r3_anim_clip");
+
+/* One skin posed with `clip` at `time` (pose_animation_frame, per skin of the scene), its matrices written to
+ * targets[first_target, first_target + target_count): every skeleton bound to the skin (PerSkinData::skeletons, lib.rs:259-261). */
+typedef struct r3_pose_job {
+    uint32_t clip;
+    float time;
+    uint32_t first_target;
+    uint32_t target_count;
+} r3_pose_job;
+R3_STATIC_ASSERT(sizeof(r3_pose_job) == 16, "r3_pose_job");
+
+/* A skeleton's range of the joint buffer (GpuSkinningInput::joint_matrix_base_offset) and its joint count: set_joint_matrices keeps the
+ * first joint_count matrices (rend3/src/managers/skeleton.rs:151-162). */
+typedef struct r3_pose_target {
+    uint32_t joint_matrix_base_offset;
+    uint32_t joint_count;
+} r3_pose_target;
+R3_STATIC_ASSERT(sizeof(r3_pose_target) == 8, "r3_pose_target");
+
 #endif /* R3_LAYOUTS_H */

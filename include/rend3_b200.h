@@ -20,11 +20,12 @@
  *   - one context per GPU; calls on a context must be externally serialised (this is the
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
- *     r3_skin's kernel, r3_exchange_merge, r3_peer_*) only enqueue work on the context's stream and return.
+ *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_exchange_merge, r3_peer_*) only enqueue work on the context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
  *     r3_batch_counts / r3_batching_info / r3_forward_stats / r3_stage_times (small device-to-host reads), and the
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
- *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload —
+ *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
+ *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
  *     has to grow (first frame, larger world, new resolution) is reallocated with a stream synchronisation as well.
@@ -144,6 +145,40 @@ int r3_set_frame_uniforms(r3_ctx*, const r3_frame_uniforms* uniforms);          
  * overridden ranges of the mesh buffer, one launch for all skeletons.  joint_matrices = global_joint_count mat4. */
 int r3_skin(r3_ctx*, const r3_skinning_input* inputs, uint32_t n_skeletons, const float* joint_matrices, uint32_t n_joints);
 int r3_readback_mesh_buffer(r3_ctx*, void* bytes, uint64_t capacity_bytes);
+
+/* ------------------------------------------------------------------ skeletal animation on the device
+ * The joint half of rend3-anim's pose_animation_frame (rend3-anim/src/lib.rs:165-176, 190, 214-262) with the arithmetic of rule R12
+ * (DESIGN.md §2), and skinning from joint matrices that stay in device memory.  The object-transform half (lib.rs:192-212) stays on the
+ * host (r3_update_objects).
+ *   r3_set_animations  the skins, their joints, the clips and their key channels (blocking upload).
+ *   r3_set_skeletons   r3_skin's arguments, kept resident: the skinning records and the joint buffer, which starts with the given
+ *                      matrices (Skeleton::joint_matrices at creation).  Blocking.
+ *   r3_set_pose_jobs   which skin is posed with which clip at which time, and which skeleton ranges receive it.  Blocking; call it
+ *                      before r3_frame_begin like the other world uploads.  r3_set_animations / r3_set_skeletons drop the jobs.
+ *   r3_pose_skeletons  enqueue only: every job's joint matrices into the joint buffer; ranges no job targets keep their matrices.
+ *   r3_skin_posed      enqueue only: r3_skin's kernel over the resident records and joint buffer.
+ * Validation: every argument is checked before anything is written; a rejected call returns R3_E_INVALID (R3_E_STATE when the data it
+ * depends on is not set) and leaves the context as it was.  The reference's panics are errors: an empty key channel, fewer values than
+ * key times, a NaN or negative clip duration, a target joint count above the skin's, a target outside the joint buffer, a clip / skin /
+ * joint / channel / key index out of range, an order that is not a permutation listing parents first.  Departures: key times must be
+ * finite, >= 0 and strictly increasing (glTF requires it), so that a binary search finds the reference's "first key with time > t";
+ * the targets of all jobs (those with joint_count > 0) must write disjoint joint ranges, since the order in which two jobs' stores
+ * land is unspecified.  Skins may share joint records (their ranges may overlap); each skin's topological order is its own stretch
+ * of `order`, read from first_joint, and must be a parents-first permutation of that skin's joints. */
+typedef struct r3_anim_library {
+    const r3_anim_skin* skins; uint32_t n_skins;
+    const r3_anim_joint* joints; uint32_t n_joints;
+    const uint32_t* order;        /* n_joints: per skin, its joint indices in topological order (see r3_anim_skin) */
+    const r3_anim_clip* clips; uint32_t n_clips;
+    const r3_anim_channel* channels; uint32_t n_channels;
+    const float* keys; uint64_t n_keys;   /* key times and values of every track */
+} r3_anim_library;
+int r3_set_animations(r3_ctx*, const r3_anim_library* library);
+int r3_set_skeletons(r3_ctx*, const r3_skinning_input* inputs, uint32_t n_skeletons, const float* joint_matrices, uint32_t n_joints);
+int r3_set_pose_jobs(r3_ctx*, const r3_pose_job* jobs, uint32_t n_jobs, const r3_pose_target* targets, uint32_t n_targets);
+int r3_pose_skeletons(r3_ctx*);
+int r3_skin_posed(r3_ctx*);
+int r3_readback_joint_matrices(r3_ctx*, float* out /* n x 16 */, uint32_t first, uint32_t n);
 
 /* ------------------------------------------------------------------ per-object cull + uniform bake
  * GpuCuller::object_uniform_upload (culler.rs:427-529) fused with the sphere-frustum test of

@@ -66,6 +66,9 @@ struct EvalOutput {
     float viewport_location[3] = {0, 0, 0};   // CameraState::location()
     // GPU skinning (skinning.rs:54-199): one record per skeleton + the global joint matrices; empty = no animated meshes this frame
     const r3_skinning_input* skinning_inputs = nullptr; uint32_t n_skeletons = 0; const float* joint_matrices = nullptr; uint32_t n_joints = 0;
+    // instead: pose on the device and skin from the resident records and joint buffer (r3_set_animations / r3_set_skeletons /
+    // r3_set_pose_jobs made before the frame); only enqueues work, so the frame stays one graph
+    bool posed_skinning = false;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -120,6 +123,10 @@ class GpuSkinner {   // skinning.rs:54-199: add_skinning_to_graph — skinned po
 public:
     void add_skinning_to_graph(Renderer& r, const EvalOutput& ev) const {
         if (ev.n_skeletons) r.check(r3_skin(r.raw(), ev.skinning_inputs, ev.n_skeletons, ev.joint_matrices, ev.n_joints));
+        if (ev.posed_skinning) {
+            r.check(r3_pose_skeletons(r.raw()));
+            r.check(r3_skin_posed(r.raw()));
+        }
     }
 };
 

@@ -41,7 +41,15 @@ ENTRY_POINTS = [
     "exchange_create", "exchange_connect", "exchange_words", "exchange_merge", "exchange_merged", "exchange_count", "exchange_counts", "exchange_destroy",
     "peer_create", "peer_connect", "peer_send_atlas_rect", "peer_send_rows", "peer_signal", "peer_wait", "peer_destroy", "clear_shadow_rect", "set_cull_shard",
     "update_object_sort_info", "resize_objects", "update_mesh_buffer", "update_textures",
+    "set_animations", "set_skeletons", "set_pose_jobs", "pose_skeletons", "skin_posed", "readback_joint_matrices",
 ]
+
+
+class _AnimLibrary(C.Structure):
+    """r3_anim_library (include/rend3_b200.h)"""
+    _fields_ = [("skins", C.c_void_p), ("n_skins", C.c_uint32), ("joints", C.c_void_p), ("n_joints", C.c_uint32), ("order", C.c_void_p),
+                ("clips", C.c_void_p), ("n_clips", C.c_uint32), ("channels", C.c_void_p), ("n_channels", C.c_uint32),
+                ("keys", C.c_void_p), ("n_keys", C.c_uint64)]
 
 
 class R3Error(RuntimeError):
@@ -208,6 +216,38 @@ class Backend:
         out = np.empty(n_words, dtype=np.uint32)
         self._call("readback_mesh_buffer", _ptr(out), C.c_uint64(out.nbytes))
         return out
+
+    # ---- skeletal animation (posed on the device, skinned from resident joint matrices)
+    def set_animations(self, skins: np.ndarray, joints: np.ndarray, order: np.ndarray, clips: np.ndarray, channels: np.ndarray, keys: np.ndarray):
+        arrays = [np.ascontiguousarray(skins), np.ascontiguousarray(joints), np.ascontiguousarray(order, dtype=np.uint32),
+                  np.ascontiguousarray(clips), np.ascontiguousarray(channels), np.ascontiguousarray(keys, dtype=np.float32)]
+        s, j, o, c, ch, k = arrays
+        assert (s.dtype.itemsize, j.dtype.itemsize, c.dtype.itemsize, ch.dtype.itemsize) == (8, 112, 16, 64) and len(o) == len(j)
+        lib = _AnimLibrary(_ptr(s) if len(s) else None, len(s), _ptr(j) if len(j) else None, len(j), _ptr(o) if len(o) else None,
+                           _ptr(c) if len(c) else None, len(c), _ptr(ch) if len(ch) else None, len(ch), _ptr(k) if len(k) else None, len(k))
+        self._call("set_animations", C.byref(lib))
+
+    def set_skeletons(self, inputs: np.ndarray, joint_matrices: np.ndarray):
+        inputs = np.ascontiguousarray(inputs)
+        assert inputs.dtype.itemsize == 40
+        jm = np.ascontiguousarray(joint_matrices, dtype=np.float32).reshape(-1, 16)
+        self._call("set_skeletons", _ptr(inputs) if len(inputs) else None, C.c_uint32(len(inputs)), _ptr(jm) if len(jm) else None, C.c_uint32(len(jm)))
+
+    def set_pose_jobs(self, jobs: np.ndarray, targets: np.ndarray):
+        jobs, targets = np.ascontiguousarray(jobs), np.ascontiguousarray(targets)
+        assert jobs.dtype.itemsize == 16 and targets.dtype.itemsize == 8
+        self._call("set_pose_jobs", _ptr(jobs) if len(jobs) else None, C.c_uint32(len(jobs)), _ptr(targets) if len(targets) else None, C.c_uint32(len(targets)))
+
+    def pose_skeletons(self):
+        self._call("pose_skeletons")
+
+    def skin_posed(self):
+        self._call("skin_posed")
+
+    def readback_joint_matrices(self, first: int, n: int) -> np.ndarray:
+        out = np.empty((max(n, 1), 16), dtype=np.float32)
+        self._call("readback_joint_matrices", _ptr(out), C.c_uint32(first), C.c_uint32(n))
+        return out[:n]
 
     # ---- object cull + bake
     def object_uniform_upload(self, camera: int, header: np.ndarray, mode: int = CB_BAKE | CB_CULL):

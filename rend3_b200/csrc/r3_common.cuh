@@ -90,6 +90,8 @@ struct r3_camera {
     unsigned long long* d_block_sums = nullptr; uint64_t block_sums_cap = 0;
 };
 
+struct r3_anim_state;                        // skeletal animation + resident skinning data (r3_animation.cu)
+
 struct r3_tri_record { float xyw[3][3]; uint32_t object_id; uint32_t vid[3]; uint32_t _pad[3]; };   // 64 B
 static_assert(sizeof(r3_tri_record) == 64, "triangle record");
 
@@ -145,6 +147,7 @@ struct r3_ctx {
     r3_stage_timer timer;
     r3_peer_state peer;
     uint32_t tri_shard_index = 0, tri_shard_count = 1;   // r3_set_cull_shard
+    r3_anim_state* anim = nullptr;            // created by the first r3_set_animations / r3_set_skeletons
     // frame graph
     bool capturing = false;                   // between r3_frame_begin and the submission (or an early flush)
     cudaGraphExec_t frame_exec[2] = {nullptr, nullptr};   // instantiated graphs of even / odd frames (the culling buffers ping-pong), updated in place
@@ -215,6 +218,10 @@ void r3_new_frame_epoch(r3_ctx* c);          // the frame-wide sort of the previ
 int r3_blend_collect(r3_ctx* c, bool* ran);   // r3_raster.cu: per-sample fragment lists of the blend routine
 int r3_iobuf_new(r3_ctx* c, r3_iobuf* b, uint64_t elems, uint64_t elem_size, bool clear_on_swap);
 int r3_iobuf_swap(r3_ctx* c, r3_iobuf* b, uint64_t new_elems);
+// r3_skinning.cu: skinning_kernel over device-resident records, chunk prefix and joint matrices (r3_skin, r3_skin_posed)
+int r3_launch_skinning(r3_ctx* c, const r3_skinning_input* d_inputs, const uint32_t* d_chunk_prefix, uint32_t n_skeletons, uint32_t total_chunks,
+                       const float* d_joints, uint32_t n_joints);
+void r3_anim_destroy(r3_ctx* c);             // r3_animation.cu: frees c->anim (r3_ctx_destroy)
 
 #ifdef __CUDACC__
 // IEEE, never-contracted arithmetic for the bit-exact stages (SURVEY D7)

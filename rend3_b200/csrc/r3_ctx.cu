@@ -75,6 +75,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     r3_stream_sync(c);
     if (c->side_stream) cudaStreamSynchronize(c->side_stream);
     r3_peer_destroy(c);
+    r3_anim_destroy(c);
     if (!c->objects_borrowed) cudaFree(c->d_objects);
     cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
     cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc); cudaFree(c->d_gsort_keys[0]); cudaFree(c->d_gsort_keys[1]); cudaFree(c->d_gsort_hist); cudaFree(c->d_gsort_header);

@@ -104,10 +104,16 @@ R3_EXPORT int r3_skin(r3_ctx* c, const r3_skinning_input* inputs, uint32_t n_ske
     R3_CUDA(c, cudaMemcpyAsync(base, inputs, b_in, cudaMemcpyHostToDevice, c->stream));
     R3_CUDA(c, cudaMemcpyAsync(base + off_pre, prefix.data(), b_pre, cudaMemcpyHostToDevice, c->stream));
     if (n_joints) R3_CUDA(c, cudaMemcpyAsync(base + off_j, joint_matrices, b_j, cudaMemcpyHostToDevice, c->stream));
-    skinning_kernel<<<total_chunks, 256, 0, c->stream>>>(c->d_mesh, c->mesh_words, (const r3_skinning_input*)base, (const uint32_t*)(base + off_pre), n_skeletons,
-                                                         (const float*)(base + off_j), n_joints);
-    R3_CHECK_LAUNCH(c, "skinning_kernel");
+    R3_TRY(r3_launch_skinning(c, (const r3_skinning_input*)base, (const uint32_t*)(base + off_pre), n_skeletons, total_chunks, (const float*)(base + off_j), n_joints));
     R3_CUDA(c, r3_stream_sync(c));   // host pointers are only borrowed for the call
+    return R3_OK;
+}
+
+int r3_launch_skinning(r3_ctx* c, const r3_skinning_input* d_inputs, const uint32_t* d_chunk_prefix, uint32_t n_skeletons, uint32_t total_chunks,
+                       const float* d_joints, uint32_t n_joints) {
+    if (total_chunks == 0) return R3_OK;
+    skinning_kernel<<<total_chunks, 256, 0, c->stream>>>(c->d_mesh, c->mesh_words, d_inputs, d_chunk_prefix, n_skeletons, d_joints, n_joints);
+    R3_CHECK_LAUNCH(c, "skinning_kernel");
     return R3_OK;
 }
 

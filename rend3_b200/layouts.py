@@ -172,3 +172,17 @@ SKINNING_INPUT_DTYPE = _dt(
     ],
     40,
 )
+
+# skeletal animation (include/r3_layouts.h: rend3-anim/src/lib.rs:37-263)
+ANIM_NO_PARENT = 0xFFFFFFFF
+ANIM_PARENT_NOT_JOINT = 0xFFFFFFFE
+ANIM_ABSENT = 0xFFFFFFFF
+ANIM_SKIN_DTYPE = _dt([("first_joint", u4, 0), ("joint_count", u4, 4)], 8)
+ANIM_JOINT_DTYPE = _dt([("bind_translation", (f4, 3), 0), ("parent", u4, 12), ("bind_rotation", (f4, 4), 16), ("bind_scale", (f4, 3), 32),
+                        ("inverse_bind", (f4, 16), 48)], 112)
+ANIM_TRACK_DTYPE = _dt([("times", u4, 0), ("values", u4, 4), ("count", u4, 8), ("value_count", u4, 12)], 16)
+ANIM_CHANNEL_DTYPE = _dt([("translation", ANIM_TRACK_DTYPE, 0), ("rotation", ANIM_TRACK_DTYPE, 16), ("scale", ANIM_TRACK_DTYPE, 32),
+                          ("animated", u4, 48)], 64)
+ANIM_CLIP_DTYPE = _dt([("skin", u4, 0), ("first_channel", u4, 4), ("duration", f4, 8)], 16)
+POSE_JOB_DTYPE = _dt([("clip", u4, 0), ("time", f4, 4), ("first_target", u4, 8), ("target_count", u4, 12)], 16)
+POSE_TARGET_DTYPE = _dt([("joint_matrix_base_offset", u4, 0), ("joint_count", u4, 4)], 8)

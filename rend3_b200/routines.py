@@ -126,7 +126,8 @@ class BaseRenderGraph:
     def add_to_graph(self, ev: EvalOutput, resolution: Tuple[int, int], samples: int = 1,
                      settings: BaseRenderGraphSettings = BaseRenderGraphSettings(), srgb_target: bool = True,
                      upload: bool = True, scissor_rows: Optional[Tuple[int, int]] = None, shadow_filter=None, after_shadows=None,
-                     after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None):
+                     after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
+                     posed_skinning: bool = False):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -135,7 +136,10 @@ class BaseRenderGraph:
         the atlas exist (peer mappings are created there); `tonemap=False` leaves the blit to the caller (the assembling rank
         runs it after the other ranks' rows have arrived); `frame_graph` records the frame's stream work and submits it as ONE CUDA
         graph launch (r3_frame_begin / r3_frame_end; the reference submits once per frame, graph.rs:510) — default: the R3_FRAME_GRAPH
-        environment variable."""
+        environment variable.  `skinning` = (records, joint matrices) skins with r3_skin, which uploads the matrices and waits for the
+        stream (a recorded frame flushes there); `posed_skinning` instead poses the skeletons on the device and skins from the resident
+        records and joint buffer (r3_pose_skeletons + r3_skin_posed after r3_set_animations / r3_set_skeletons / r3_set_pose_jobs):
+        only enqueued work, so the frame stays one graph."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -160,6 +164,9 @@ class BaseRenderGraph:
         b.set_frame_uniforms(frame_uniforms(ev.camera, settings.ambient_color, resolution))  # :142
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
+        if posed_skinning:                                                        # :145 from resident data (r3_set_skeletons / r3_set_pose_jobs)
+            b.pose_skeletons()
+            b.skin_posed()
         mine = [(i, s) for i, s in enumerate(ev.shadows) if shadow_filter is None or shadow_filter(i)]
         for i, s in mine:                                                         # :148
             culler.object_uniform_upload(ev, s.camera, i, (s.size, s.size), 1)

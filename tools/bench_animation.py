@@ -1,0 +1,177 @@
+"""Crowd animation benchmark: device posing (r3_pose_skeletons) and skinning from resident joint matrices (r3_skin_posed) against the
+host path they replace (the oracle's pose on the CPU + r3_skin's per-frame upload and stream drain).  Prints one JSON line.
+
+Workload: --instances instances (default 4096) of a 65-joint humanoid-shaped skin of depth 10, two skeletons (primitives) per instance
+of --vertices vertices each (default 1000), one clip with translation, rotation and scale channels of 60 keys on every joint.  The
+instances share the two meshes' source attributes and each skeleton has its own skinned ranges, as SkeletonManager lays them out.
+
+Usage: python tools/bench_animation.py [--instances N] [--vertices V] [--iters K] [--warmup W]"""
+import argparse
+import json
+import math
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+f32 = np.float32
+
+
+def skinned_mesh(n_instances, n_vertices, seed=0):
+    """Mesh words + one r3_skinning_input per skeleton: 2 meshes' source attributes, then per skeleton its updated position / normal."""
+    from rend3_b200.layouts import ATTR_ABSENT, SKINNING_INPUT_DTYPE
+
+    rng = np.random.default_rng(seed)
+    parts, cursor = [], 0
+
+    def push(a):
+        nonlocal cursor
+        raw = np.ascontiguousarray(a).view(np.uint32).reshape(-1)
+        parts.append(raw)
+        cursor += len(raw)
+        return 4 * (cursor - len(raw))
+
+    meshes = []
+    for _ in range(2):
+        nrm = rng.standard_normal((n_vertices, 3)).astype(f32)
+        nrm /= np.linalg.norm(nrm, axis=1, keepdims=True).astype(f32)
+        w = rng.random((n_vertices, 4)).astype(f32)
+        meshes.append((push(rng.uniform(-1, 1, (n_vertices, 3)).astype(f32)), push(nrm), push(rng.integers(0, 65, (n_vertices, 4)).astype(np.uint16)),
+                       push((w / w.sum(axis=1, keepdims=True)).astype(f32))))
+    n_skel = 2 * n_instances
+    recs = np.zeros(n_skel, dtype=SKINNING_INPUT_DTYPE)
+    out_base = cursor
+    for s in range(n_skel):
+        p, n, j, w = meshes[s % 2]
+        recs[s] = (p, n, ATTR_ABSENT, j, w, 4 * (out_base + 6 * n_vertices * s), 4 * (out_base + 6 * n_vertices * s + 3 * n_vertices), ATTR_ABSENT,
+                   65 * s, n_vertices)
+    parts.append(np.zeros(6 * n_vertices * n_skel, dtype=np.uint32))
+    return np.concatenate(parts), recs
+
+
+def pose_bytes(jobs, targets, library, n_keys):
+    """Bytes pose_kernel requests per launch: job + targets, per joint its channel record (64 B), joint record (112 B), per track the
+    binary search (ceil(log2 K) + 2 key times) and two key values, and 64 B per matrix stored."""
+    joints = int(library.skins["joint_count"][0])
+    search = (math.ceil(math.log2(n_keys)) + 2) * 4
+    per_joint = 64 + 112 + 3 * search + 2 * (3 + 4 + 3) * 4
+    reads = len(jobs) * (16 + joints * per_joint) + 8 * len(targets)
+    writes = 64 * int(targets["joint_count"].sum())
+    unique = library.channels.nbytes + library.joints.nbytes + library.keys.nbytes + jobs.nbytes + targets.nbytes
+    return {"requested_read_bytes": reads, "written_bytes": writes, "distinct_read_bytes": unique}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--instances", type=int, default=4096)
+    ap.add_argument("--vertices", type=int, default=1000)
+    ap.add_argument("--iters", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=20)
+    args = ap.parse_args()
+
+    import torch
+
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_animation needs a CUDA device")
+    import animation_case
+    import oracle
+    from oracle.anim import load_anim_oracle_backend
+    from rend3_b200.backend import load_cuda_backend
+
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip().splitlines()
+    data, jobs, targets, buf = animation_case.crowd(args.instances)
+    words, recs = skinned_mesh(args.instances, args.vertices)
+    n_joints = int(targets["joint_count"].sum())
+
+    b = load_cuda_backend(0)
+    b.set_mesh_buffer(words)
+    b.set_animations(*data.library.arrays())
+    b.set_skeletons(recs, buf)
+    b.set_pose_jobs(jobs, targets)
+    stream = torch.cuda.ExternalStream(b.stream())
+
+    def device_ms(fn):
+        for _ in range(args.warmup):
+            fn()
+        b.sync()
+        start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        start.record(stream)
+        for _ in range(args.iters):
+            fn()
+        stop.record(stream)
+        stop.synchronize()
+        return start.elapsed_time(stop) / args.iters
+
+    # r3_set_pose_jobs is the per-frame host call of the new path (new times): host clock, the call ends in a stream synchronise
+    for _ in range(3):
+        b.set_pose_jobs(jobs, targets)
+    t0 = time.perf_counter()
+    for _ in range(50):
+        b.set_pose_jobs(jobs, targets)
+    set_jobs_ms = (time.perf_counter() - t0) * 1e3 / 50
+
+    pose_ms = device_ms(b.pose_skeletons)
+    skin_ms = device_ms(b.skin_posed)
+    posed = b.readback_joint_matrices(0, len(buf))
+
+    # frame-graph flushes per frame: posed path vs r3_skin with host matrices
+    def flushes(fn):
+        before = b.frame_graph_stats()["flushed"]
+        b.frame_begin()
+        fn()
+        b.frame_end()
+        b.sync()
+        return b.frame_graph_stats()["flushed"] - before
+
+    flush_posed = flushes(lambda: (b.pose_skeletons(), b.skin_posed()))
+    flush_skin = flushes(lambda: b.skin(recs, posed))
+
+    # r3_skin: per-frame upload of the joint matrices + launch + stream drain (host clock around a call that ends in a synchronise)
+    for _ in range(3):
+        b.skin(recs, posed)
+    t0 = time.perf_counter()
+    reps = 20
+    for _ in range(reps):
+        b.skin(recs, posed)
+    skin_host_ms = (time.perf_counter() - t0) * 1e3 / reps
+
+    # the host pose: the oracle (C, OpenMP over jobs) on this machine's cores
+    threads = oracle.set_threads(os.cpu_count() or 1)
+    orc = load_anim_oracle_backend()
+    orc.set_animations(*data.library.arrays())
+    orc.set_skeletons(recs[:0], buf)
+    orc.set_pose_jobs(jobs, targets)
+    orc.pose_skeletons()
+    t0 = time.perf_counter()
+    for _ in range(5):
+        orc.pose_skeletons()
+    host_pose_ms = (time.perf_counter() - t0) * 1e3 / 5
+    same = bool(np.array_equal(orc.readback_joint_matrices(0, len(buf)).view(np.uint32), posed.view(np.uint32)))
+    orc.close()
+    b.close()
+
+    model = pose_bytes(jobs, targets, data.library, 60)
+    joints_posed = len(jobs) * int(data.library.skins["joint_count"][0])
+    print(json.dumps({
+        "workload": {"instances": args.instances, "joints_per_skin": int(data.library.skins["joint_count"][0]), "skeletons": len(recs),
+                     "vertices_per_skeleton": args.vertices, "keys_per_track": 60, "joint_matrices_written": n_joints},
+        "gpu": smi[0] if smi else torch.cuda.get_device_name(0),
+        "pose_skeletons_ms": round(pose_ms, 4), "skin_posed_ms": round(skin_ms, 4), "set_pose_jobs_host_ms": round(set_jobs_ms, 4),
+        "set_pose_jobs_bytes": int(jobs.nbytes + targets.nbytes + 8 * len(jobs)),
+        "joints_posed_per_s": joints_posed / (pose_ms * 1e-3),
+        "pose_byte_model": model, "pose_requested_bytes_per_s": (model["requested_read_bytes"] + model["written_bytes"]) / (pose_ms * 1e-3),
+        "early_flushes_per_frame": {"posed": flush_posed, "r3_skin": flush_skin},
+        "host_alternative": {"oracle_pose_ms": round(host_pose_ms, 3), "oracle_threads": threads, "r3_skin_upload_and_sync_ms": round(skin_host_ms, 3),
+                             "joint_bytes_uploaded_per_frame": 64 * len(buf)},
+        "device_pose_equals_oracle": same,
+    }))
+
+
+if __name__ == "__main__":
+    main()
