@@ -1,5 +1,5 @@
-/* r3_anim_check.h — argument checks of r3_set_animations / r3_set_pose_jobs, shared by the library and its CPU oracle so that both
- * reject exactly the same inputs.  Plain C99 / C++, header only.
+/* r3_anim_check.h — argument checks of r3_set_animations / r3_set_pose_jobs and r3_set_object_animations / r3_set_object_pose_jobs,
+ * shared by the library and its CPU oracle so that both reject exactly the same inputs.  Plain C99 / C++, header only.
  *
  * The checks turn the reference's panic sites into errors (rend3-anim/src/lib.rs:166-175, 190; skeleton.rs:151-162):
  *   an empty key channel (`times.len() - 1` underflow), fewer values than key times, a NaN or negative duration (f32::clamp's assert),
@@ -116,6 +116,70 @@ static inline int r3_anim_check_jobs(const r3_anim_skin* skins, const r3_anim_cl
         if (r[2 * i] < r[2 * (i - 1) + 1]) { *msg = "set_pose_jobs: two targets write overlapping joint ranges"; rc = R3_E_INVALID; break; }
     free(r);
     return rc;
+}
+
+/* ---- object animation (r3_set_object_animations / r3_set_object_pose_jobs): the same track rules, the same duration rule */
+static inline int r3_anim_check_object_library(const r3_anim_object_library* L, const char** msg) {
+    *msg = "";
+    if (!L) { *msg = "set_object_animations: null library"; return R3_E_INVALID; }
+    if ((!L->nodes && L->n_nodes) || (!L->clips && L->n_clips) || (!L->channels && L->n_channels) || (!L->keys && L->n_keys)) {
+        *msg = "set_object_animations: null array"; return R3_E_INVALID;
+    }
+    for (uint32_t c = 0; c < L->n_clips; ++c) {
+        const r3_anim_node_clip cl = L->clips[c];
+        if (!(cl.duration >= 0.0f)) { *msg = "set_object_animations: clip duration is NaN or negative"; return R3_E_INVALID; }
+        if ((uint64_t)cl.first_channel + cl.channel_count > L->n_channels) { *msg = "set_object_animations: clip channel range out of range"; return R3_E_INVALID; }
+    }
+    for (uint32_t k = 0; k < L->n_channels; ++k) {
+        const r3_anim_node_channel* ch = &L->channels[k];
+        if (ch->node >= L->n_nodes) { *msg = "set_object_animations: channel node out of range"; return R3_E_INVALID; }
+        if (r3_anim_check_track(&ch->translation, 3, L->keys, L->n_keys, msg) != R3_OK) return R3_E_INVALID;
+        if (r3_anim_check_track(&ch->rotation, 4, L->keys, L->n_keys, msg) != R3_OK) return R3_E_INVALID;
+        if (r3_anim_check_track(&ch->scale, 3, L->keys, L->n_keys, msg) != R3_OK) return R3_E_INVALID;
+    }
+    return R3_OK;
+}
+
+static inline int r3_anim_slot_cmp(const void* a, const void* b) {
+    const uint32_t x = *(const uint32_t*)a, y = *(const uint32_t*)b;
+    return x < y ? -1 : x > y ? 1 : 0;
+}
+
+/* jobs against the clips of the object library that is set and an object buffer of n_slots slots.  On success, when `slots_out` is
+ * not null, *slots_out is a malloc'd list of the slot of every (job, target) pair in job order (*n_out entries; the caller frees it). */
+static inline int r3_anim_check_object_jobs(const r3_anim_node_clip* clips, uint32_t n_clips, uint32_t n_slots, const r3_pose_job* jobs,
+                                            uint32_t n_jobs, const r3_object_pose_target* targets, uint32_t n_targets,
+                                            uint32_t** slots_out, uint64_t* n_out, const char** msg) {
+    *msg = "";
+    if ((!jobs && n_jobs) || (!targets && n_targets)) { *msg = "set_object_pose_jobs: null array"; return R3_E_INVALID; }
+    uint64_t n = 0;
+    for (uint32_t i = 0; i < n_jobs; ++i) {
+        const r3_pose_job j = jobs[i];
+        if (j.clip >= n_clips) { *msg = "set_object_pose_jobs: clip out of range"; return R3_E_INVALID; }
+        if ((uint64_t)j.first_target + j.target_count > n_targets) { *msg = "set_object_pose_jobs: target range out of range"; return R3_E_INVALID; }
+        for (uint32_t t = 0; t < j.target_count; ++t) {
+            const r3_object_pose_target tg = targets[j.first_target + t];
+            if (tg.channel >= clips[j.clip].channel_count) { *msg = "set_object_pose_jobs: target channel out of the clip's range"; return R3_E_INVALID; }
+            if (tg.slot >= n_slots) { *msg = "set_object_pose_jobs: target slot beyond the object buffer"; return R3_E_INVALID; }
+        }
+        n += j.target_count;
+    }
+    uint32_t* s = (uint32_t*)malloc(n ? n * sizeof(uint32_t) : 4);
+    uint32_t* sorted = (uint32_t*)malloc(n ? n * sizeof(uint32_t) : 4);
+    if (!s || !sorted) { free(s); free(sorted); *msg = "set_object_pose_jobs: out of host memory"; return R3_E_INVALID; }
+    uint64_t k = 0;
+    for (uint32_t i = 0; i < n_jobs; ++i)
+        for (uint32_t t = 0; t < jobs[i].target_count; ++t) s[k++] = targets[jobs[i].first_target + t].slot;
+    if (n) memcpy(sorted, s, n * sizeof(uint32_t));
+    qsort(sorted, n, sizeof(uint32_t), r3_anim_slot_cmp);
+    int rc = R3_OK;
+    for (uint64_t i = 1; i < n; ++i)
+        if (sorted[i] == sorted[i - 1]) { *msg = "set_object_pose_jobs: two targets name the same slot"; rc = R3_E_INVALID; break; }
+    free(sorted);
+    if (rc != R3_OK || !slots_out) { free(s); return rc; }
+    *slots_out = s;
+    *n_out = n;
+    return R3_OK;
 }
 
 #endif /* R3_ANIM_CHECK_H */

@@ -358,4 +358,55 @@ typedef struct r3_pose_target {
 } r3_pose_target;
 R3_STATIC_ASSERT(sizeof(r3_pose_target) == 8, "r3_pose_target");
 
+/* ---- object animation: the object-transform half of pose_animation_frame (rend3-anim/src/lib.rs:192-212, posed on the device by
+ * r3_pose_objects).  Tracks are r3_anim_track over the key blob of r3_anim_object_library. */
+
+/* A scene node that carries an object: its bind pose, local_transform.to_scale_rotation_translation() (lib.rs:194), decomposed on the
+ * host.  A property without a track takes its bind value (lib.rs:196-199), not IDENTITY's. */
+typedef struct r3_anim_node {
+    float bind_translation[3];    /* @0 */
+    uint32_t _pad0;
+    float bind_rotation[4];       /* @16 quaternion x, y, z, w */
+    float bind_scale[3];          /* @32 */
+    uint32_t _pad1;
+} r3_anim_node;
+R3_STATIC_ASSERT(sizeof(r3_anim_node) == 48, "r3_anim_node");
+R3_STATIC_ASSERT(offsetof(r3_anim_node, bind_rotation) == 16, "bind_rotation");
+R3_STATIC_ASSERT(offsetof(r3_anim_node, bind_scale) == 32, "bind_scale");
+
+/* One (node, AnimationChannels) entry of Animation::channels (lib.rs:192): the node's translation / rotation / scale tracks, each
+ * possibly absent (times == R3_ANIM_ABSENT), and the node index into r3_anim_object_library.nodes. */
+typedef struct r3_anim_node_channel {
+    r3_anim_track translation;    /* @0 */
+    r3_anim_track rotation;       /* @16 */
+    r3_anim_track scale;          /* @32 */
+    uint32_t node;                /* @48 */
+    uint32_t _pad[3];
+} r3_anim_node_channel;
+R3_STATIC_ASSERT(sizeof(r3_anim_node_channel) == 64, "r3_anim_node_channel");
+R3_STATIC_ASSERT(offsetof(r3_anim_node_channel, node) == 48, "node");
+
+/* One Animation, with only the channels of nodes that carry objects: r3_anim_object_library.channels[first_channel,
+ * first_channel + channel_count). */
+typedef struct r3_anim_node_clip {
+    uint32_t first_channel;
+    uint32_t channel_count;
+    float duration;               /* Animation::duration: time is clamped to [0, duration] (lib.rs:190) */
+    uint32_t _pad;
+} r3_anim_node_clip;
+R3_STATIC_ASSERT(sizeof(r3_anim_node_clip) == 16, "r3_anim_node_clip");
+
+/* One primitive of a posed node's object (object.inner.primitives, lib.rs:208-210): its object slot, the channel of the job's clip
+ * that poses it (an index within the clip), and InternalObject::mesh_bounding_sphere (object.rs:268-270), which set_object_transform
+ * moves to world space (object.rs:313).  Jobs are r3_pose_job records whose targets index these. */
+typedef struct r3_object_pose_target {
+    uint32_t slot;                /* @0 */
+    uint32_t channel;             /* @4 */
+    uint32_t _pad[2];
+    float mesh_sphere_center[3];  /* @16 */
+    float mesh_sphere_radius;     /* @28 */
+} r3_object_pose_target;
+R3_STATIC_ASSERT(sizeof(r3_object_pose_target) == 32, "r3_object_pose_target");
+R3_STATIC_ASSERT(offsetof(r3_object_pose_target, mesh_sphere_center) == 16, "mesh_sphere_center");
+
 #endif /* R3_LAYOUTS_H */

@@ -20,12 +20,14 @@
  *   - one context per GPU; calls on a context must be externally serialised (this is the
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
- *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_exchange_merge, r3_peer_*) only enqueue work on the context's stream and return.
+ *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_exchange_merge, r3_peer_*) only enqueue work on the
+ *     context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
  *     r3_batch_counts / r3_batching_info / r3_forward_stats / r3_stage_times (small device-to-host reads), and the
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
  *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
- *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices —
+ *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices, r3_set_object_animations,
+ *     r3_set_object_pose_jobs —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
  *     has to grow (first frame, larger world, new resolution) is reallocated with a stream synchronisation as well.
@@ -148,8 +150,8 @@ int r3_readback_mesh_buffer(r3_ctx*, void* bytes, uint64_t capacity_bytes);
 
 /* ------------------------------------------------------------------ skeletal animation on the device
  * The joint half of rend3-anim's pose_animation_frame (rend3-anim/src/lib.rs:165-176, 190, 214-262) with the arithmetic of rule R12
- * (DESIGN.md §2), and skinning from joint matrices that stay in device memory.  The object-transform half (lib.rs:192-212) stays on the
- * host (r3_update_objects).
+ * (DESIGN.md §2), and skinning from joint matrices that stay in device memory.  The object-transform half (lib.rs:192-212) is the next
+ * block (r3_pose_objects).
  *   r3_set_animations  the skins, their joints, the clips and their key channels (blocking upload).
  *   r3_set_skeletons   r3_skin's arguments, kept resident: the skinning records and the joint buffer, which starts with the given
  *                      matrices (Skeleton::joint_matrices at creation).  Blocking.
@@ -179,6 +181,37 @@ int r3_set_pose_jobs(r3_ctx*, const r3_pose_job* jobs, uint32_t n_jobs, const r3
 int r3_pose_skeletons(r3_ctx*);
 int r3_skin_posed(r3_ctx*);
 int r3_readback_joint_matrices(r3_ctx*, float* out /* n x 16 */, uint32_t first, uint32_t n);
+
+/* ------------------------------------------------------------------ object animation on the device
+ * The object-transform half of rend3-anim's pose_animation_frame (rend3-anim/src/lib.rs:181-212): every posed node's TRS matrix becomes
+ * its objects' transform, as Renderer::set_object_transform sets it (object.rs:302-316): transform, world bounding sphere
+ * (mesh_bounding_sphere.apply_transform, util/frustum.rs:22-32) and sort location (transform_point3a(ZERO)).  Arithmetic: rule R12
+ * (DESIGN.md §2).  Independent of the skeletal block: each set_* call drops only its own jobs.
+ *   r3_set_object_animations  the nodes' bind poses, the clips, their channels and keys, and the renderer's handedness (blocking).
+ *   r3_set_object_pose_jobs   r3_pose_job records (clip, time, targets) over r3_object_pose_target records.  Blocking; call it before
+ *                             r3_frame_begin.  Its buffers only grow.
+ *   r3_pose_objects           enqueue only: each target's record (transform and sphere, float4 #0-4; enabled and the cold fields are
+ *                             untouched) and, when sort info is set, its sort location; then the cull + bake's dense copies of those
+ *                             slots and a new frame epoch.  Targets whose slot is at or past the current slot count are skipped.
+ *   r3_readback_objects       blocking: records [first, first + n) and, unless null, their sort locations (3 floats each).
+ * Validation (include/r3_anim_check.h): R3_E_INVALID for an index out of range, a NaN or negative duration, a track as
+ * r3_set_animations checks it, a target channel >= its clip's channel_count, a slot >= the current slot count, one slot named by two
+ * targets of the jobs (their stores would land in an unspecified order); R3_E_STATE for jobs before the library, r3_pose_objects before
+ * r3_set_objects or before the jobs, and any of these calls while the object buffer is borrowed (r3_set_objects_device).  A rejected
+ * call leaves the context as it was.
+ * A later r3_update_objects / r3_update_object_sort_info of a posed slot writes the bytes it is given over the pose until the next
+ * r3_pose_objects, which runs at the skinning node of every frame, before any camera culls (INTEGRATION.md). */
+typedef struct r3_anim_object_library {
+    const r3_anim_node* nodes; uint32_t n_nodes;
+    const r3_anim_node_clip* clips; uint32_t n_clips;
+    const r3_anim_node_channel* channels; uint32_t n_channels;
+    const float* keys; uint64_t n_keys;   /* key times and values of every track */
+    uint32_t left_handed;                 /* renderer.handedness == Handedness::Left: scale.z = -scale.z (lib.rs:201-203) */
+} r3_anim_object_library;
+int r3_set_object_animations(r3_ctx*, const r3_anim_object_library* library);
+int r3_set_object_pose_jobs(r3_ctx*, const r3_pose_job* jobs, uint32_t n_jobs, const r3_object_pose_target* targets, uint32_t n_targets);
+int r3_pose_objects(r3_ctx*);
+int r3_readback_objects(r3_ctx*, r3_object* out, float* locations_or_null /* n x 3 */, uint32_t first, uint32_t n);
 
 /* ------------------------------------------------------------------ per-object cull + uniform bake
  * GpuCuller::object_uniform_upload (culler.rs:427-529) fused with the sphere-frustum test of

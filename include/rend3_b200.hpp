@@ -69,6 +69,9 @@ struct EvalOutput {
     // instead: pose on the device and skin from the resident records and joint buffer (r3_set_animations / r3_set_skeletons /
     // r3_set_pose_jobs made before the frame); only enqueues work, so the frame stays one graph
     bool posed_skinning = false;
+    // pose the animated nodes' objects on the device (r3_set_object_animations / r3_set_object_pose_jobs made before the frame):
+    // transforms, world spheres and sort locations, written at the skinning node before any camera culls; only enqueues work
+    bool posed_objects = false;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -123,6 +126,7 @@ class GpuSkinner {   // skinning.rs:54-199: add_skinning_to_graph — skinned po
 public:
     void add_skinning_to_graph(Renderer& r, const EvalOutput& ev) const {
         if (ev.n_skeletons) r.check(r3_skin(r.raw(), ev.skinning_inputs, ev.n_skeletons, ev.joint_matrices, ev.n_joints));
+        if (ev.posed_objects) r.check(r3_pose_objects(r.raw()));
         if (ev.posed_skinning) {
             r.check(r3_pose_skeletons(r.raw()));
             r.check(r3_skin_posed(r.raw()));

@@ -7,6 +7,9 @@ scene's topological order filtered to the skin's joint nodes, and every animatio
 every skin of the scene, lib.rs:214; a skin the animation does not touch has no animated joint and comes out as IDENTITY * inverse
 bind).  Channels of nodes that are not joints of a skin are left out of that skin's clip: the reference indexes node_to_joint_idx with
 them (lib.rs:236) and would panic.
+
+ObjectAnimationData is the object-transform half (lib.rs:192-212): the channels of nodes that carry objects, for
+r3_set_object_animations, and r3_set_object_pose_jobs records.
 """
 from __future__ import annotations
 
@@ -15,8 +18,9 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .layouts import (ANIM_ABSENT, ANIM_CHANNEL_DTYPE, ANIM_CLIP_DTYPE, ANIM_JOINT_DTYPE, ANIM_NO_PARENT, ANIM_PARENT_NOT_JOINT,
-                      ANIM_SKIN_DTYPE, POSE_JOB_DTYPE, POSE_TARGET_DTYPE)
+from .layouts import (ANIM_ABSENT, ANIM_CHANNEL_DTYPE, ANIM_CLIP_DTYPE, ANIM_JOINT_DTYPE, ANIM_NO_PARENT, ANIM_NODE_CHANNEL_DTYPE,
+                      ANIM_NODE_CLIP_DTYPE, ANIM_NODE_DTYPE, ANIM_PARENT_NOT_JOINT, ANIM_SKIN_DTYPE, OBJECT_POSE_TARGET_DTYPE, POSE_JOB_DTYPE,
+                      POSE_TARGET_DTYPE)
 
 f32 = np.float32
 
@@ -37,11 +41,13 @@ class NodeChannels:
 
 @dataclass
 class Node:
-    """A scene node: its parent node and local_transform.to_scale_rotation_translation()."""
+    """A scene node: its parent node and local_transform.to_scale_rotation_translation(); `objects` are the primitives of the node's
+    object, each (object slot, mesh bounding-sphere centre, radius) — InternalObject::mesh_bounding_sphere."""
     parent: Optional[int] = None
     translation: Sequence[float] = (0.0, 0.0, 0.0)
     rotation: Sequence[float] = (0.0, 0.0, 0.0, 1.0)
     scale: Sequence[float] = (1.0, 1.0, 1.0)
+    objects: List[Tuple[int, Sequence[float], float]] = field(default_factory=list)
 
 
 @dataclass
@@ -158,3 +164,81 @@ class AnimationData:
                 jobs.append((self.clip_of[(animation, s)], time, len(targets), len(sk)))
                 targets += sk
         return np.array(jobs, dtype=POSE_JOB_DTYPE), np.array(targets, dtype=POSE_TARGET_DTYPE)
+
+
+@dataclass
+class ObjectLibrary:
+    """The arrays of r3_anim_object_library."""
+    nodes: np.ndarray
+    clips: np.ndarray
+    channels: np.ndarray
+    keys: np.ndarray
+    left_handed: bool
+
+    def arrays(self):
+        return self.nodes, self.clips, self.channels, self.keys, self.left_handed
+
+
+class ObjectAnimationData:
+    """The object-transform half of pose_animation_frame (lib.rs:192-212) over a synthetic scene: every animation becomes one clip with
+    the channels of the nodes that carry objects (a channel of a node without an object sets nothing), every node its bind pose.
+    `library` holds what r3_set_object_animations takes; `pose_jobs` turns pose_animation_frame calls into r3_set_object_pose_jobs
+    records.  `left_handed` is renderer.handedness == Handedness::Left."""
+
+    def __init__(self, nodes: Sequence[Node], animations: Sequence[Animation], left_handed: bool = False):
+        keys: List[np.ndarray] = []
+        n_keys = 0
+
+        def track(t: Optional[Track]):
+            nonlocal n_keys
+            r = np.zeros((), dtype=ANIM_NODE_CHANNEL_DTYPE["translation"])
+            if t is None:
+                r["times"] = ANIM_ABSENT
+                return r
+            for name, a in (("times", t.times), ("values", t.values)):
+                a = np.ascontiguousarray(a, dtype=f32).reshape(-1)
+                r[name] = n_keys
+                keys.append(a)
+                n_keys += len(a)
+            r["count"], r["value_count"] = len(t.times), len(t.values)
+            return r
+
+        node_recs = np.zeros(len(nodes), dtype=ANIM_NODE_DTYPE)
+        for i, node in enumerate(nodes):
+            node_recs[i]["bind_translation"], node_recs[i]["bind_rotation"], node_recs[i]["bind_scale"] = node.translation, node.rotation, node.scale
+        clips, channels = [], []
+        self.channel_of: Dict[Tuple[int, int], int] = {}   # (animation, node) -> channel within the clip
+        for a, anim in enumerate(animations):
+            first = len(channels)
+            for n in sorted(anim.channels):
+                if not nodes[n].objects:
+                    continue
+                nc = anim.channels[n]
+                ch = np.zeros((), dtype=ANIM_NODE_CHANNEL_DTYPE)
+                ch["translation"], ch["rotation"], ch["scale"] = track(nc.translation), track(nc.rotation), track(nc.scale)
+                ch["node"] = n
+                self.channel_of[(a, n)] = len(channels) - first
+                channels.append(ch)
+            clips.append((first, len(channels) - first, anim.duration))
+        self.library = ObjectLibrary(node_recs, np.array(clips, dtype=ANIM_NODE_CLIP_DTYPE), np.array(channels, dtype=ANIM_NODE_CHANNEL_DTYPE),
+                                     np.concatenate(keys) if keys else np.zeros(0, dtype=f32), left_handed)
+        self.nodes = list(nodes)
+
+    def upload(self, backend):
+        backend.set_object_animations(*self.library.arrays())
+
+    def pose_jobs(self, frames: Sequence[Tuple[int, float, int]]):
+        """pose_animation_frame(scene, animation, time) for each (animation, time, slot_offset) of `frames` — one scene instance each,
+        whose objects are the nodes' objects with their slots moved by slot_offset — as r3_set_object_pose_jobs records."""
+        jobs, targets = [], []
+        for animation, time, offset in frames:
+            first = len(targets)
+            for (a, n), ch in sorted(self.channel_of.items(), key=lambda kv: kv[1]):
+                if a != animation:
+                    continue
+                targets += [(slot + offset, ch, center, radius) for slot, center, radius in self.nodes[n].objects]
+            jobs.append((animation, time, first, len(targets) - first))
+        out = np.zeros(len(targets), dtype=OBJECT_POSE_TARGET_DTYPE)
+        for i, (slot, ch, center, radius) in enumerate(targets):
+            out[i]["slot"], out[i]["channel"], out[i]["mesh_sphere_center"], out[i]["mesh_sphere_radius"] = slot, ch, center, radius
+        return np.array(jobs, dtype=POSE_JOB_DTYPE), out

@@ -42,6 +42,7 @@ ENTRY_POINTS = [
     "peer_create", "peer_connect", "peer_send_atlas_rect", "peer_send_rows", "peer_signal", "peer_wait", "peer_destroy", "clear_shadow_rect", "set_cull_shard",
     "update_object_sort_info", "resize_objects", "update_mesh_buffer", "update_textures",
     "set_animations", "set_skeletons", "set_pose_jobs", "pose_skeletons", "skin_posed", "readback_joint_matrices",
+    "set_object_animations", "set_object_pose_jobs", "pose_objects", "readback_objects",
 ]
 
 
@@ -50,6 +51,12 @@ class _AnimLibrary(C.Structure):
     _fields_ = [("skins", C.c_void_p), ("n_skins", C.c_uint32), ("joints", C.c_void_p), ("n_joints", C.c_uint32), ("order", C.c_void_p),
                 ("clips", C.c_void_p), ("n_clips", C.c_uint32), ("channels", C.c_void_p), ("n_channels", C.c_uint32),
                 ("keys", C.c_void_p), ("n_keys", C.c_uint64)]
+
+
+class _AnimObjectLibrary(C.Structure):
+    """r3_anim_object_library (include/rend3_b200.h)"""
+    _fields_ = [("nodes", C.c_void_p), ("n_nodes", C.c_uint32), ("clips", C.c_void_p), ("n_clips", C.c_uint32), ("channels", C.c_void_p),
+                ("n_channels", C.c_uint32), ("keys", C.c_void_p), ("n_keys", C.c_uint64), ("left_handed", C.c_uint32)]
 
 
 class R3Error(RuntimeError):
@@ -248,6 +255,33 @@ class Backend:
         out = np.empty((max(n, 1), 16), dtype=np.float32)
         self._call("readback_joint_matrices", _ptr(out), C.c_uint32(first), C.c_uint32(n))
         return out[:n]
+
+    # ---- object animation (the object-transform half of pose_animation_frame, posed on the device)
+    def set_object_animations(self, nodes: np.ndarray, clips: np.ndarray, channels: np.ndarray, keys: np.ndarray, left_handed: bool):
+        n, c, ch = np.ascontiguousarray(nodes), np.ascontiguousarray(clips), np.ascontiguousarray(channels)
+        k = np.ascontiguousarray(keys, dtype=np.float32)
+        assert (n.dtype.itemsize, c.dtype.itemsize, ch.dtype.itemsize) == (48, 16, 64)
+        lib = _AnimObjectLibrary(_ptr(n) if len(n) else None, len(n), _ptr(c) if len(c) else None, len(c), _ptr(ch) if len(ch) else None, len(ch),
+                                 _ptr(k) if len(k) else None, len(k), 1 if left_handed else 0)
+        self._call("set_object_animations", C.byref(lib))
+
+    def set_object_pose_jobs(self, jobs: np.ndarray, targets: np.ndarray):
+        jobs, targets = np.ascontiguousarray(jobs), np.ascontiguousarray(targets)
+        assert jobs.dtype.itemsize == 16 and targets.dtype.itemsize == 32
+        self._call("set_object_pose_jobs", _ptr(jobs) if len(jobs) else None, C.c_uint32(len(jobs)), _ptr(targets) if len(targets) else None,
+                   C.c_uint32(len(targets)))
+
+    def pose_objects(self):
+        self._call("pose_objects")
+
+    def readback_objects(self, first: int, n: int, locations: bool = True):
+        """(records, (n, 3) sort locations or None)"""
+        from .layouts import OBJECT_DTYPE
+
+        out = np.zeros(max(n, 1), dtype=OBJECT_DTYPE)
+        loc = np.zeros((max(n, 1), 3), dtype=np.float32) if locations else None
+        self._call("readback_objects", _ptr(out), _ptr(loc), C.c_uint32(first), C.c_uint32(n))
+        return out[:n], (loc[:n] if locations else None)
 
     # ---- object cull + bake
     def object_uniform_upload(self, camera: int, header: np.ndarray, mode: int = CB_BAKE | CB_CULL):

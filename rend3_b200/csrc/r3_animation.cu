@@ -9,7 +9,12 @@
 // gives the same bits; the levels let the threads of a CTA compute all joints of a level at once.  pose_kernel: one CTA per job —
 // every joint's local matrix, then the globals level by level (in place over the locals, in shared memory, or in a global scratch for
 // skins above R3_ANIM_SMEM_JOINTS joints), then global * inverse_bind stored into each target's range of the joint buffer.
+//
+// The object-transform half (lib.rs:192-212, set_object_transform of object.rs:302-316) is pose_objects_kernel: one thread per posed
+// object samples its node's channel, builds the TRS matrix and writes the record's transform and world sphere and the slot's sort
+// location.  The work is small and latency-bound; the cull + bake's dense copies of those slots are then refreshed by r3_split_slots.
 #include <algorithm>
+#include <cstring>
 #include <vector>
 
 #include "../../include/r3_anim_check.h"
@@ -197,6 +202,66 @@ __global__ void __launch_bounds__(R3_ANIM_THREADS) pose_kernel(const r3_pose_job
     }
 }
 
+constexpr uint32_t R3_OBJ_POSE_THREADS = 128;
+
+// The object-transform half of pose_animation_frame (lib.rs:190-212) + set_object_transform (object.rs:302-316), one thread per
+// (job, target) item.  Rule R12: bind pose for an absent track, scale.z negated for a left-handed renderer, from_srt, then the record's
+// transform and world sphere (float4 #0-4) and the sort location.  Slots at or past n_slots are skipped (ScatterCopy drops them).
+__global__ void __launch_bounds__(R3_OBJ_POSE_THREADS) pose_objects_kernel(const uint2* __restrict__ items, uint32_t n_items, const r3_pose_job* __restrict__ jobs,
+                                                                            const r3_object_pose_target* __restrict__ targets, const r3_anim_node_clip* __restrict__ clips,
+                                                                            const r3_anim_node_channel* __restrict__ channels, const r3_anim_node* __restrict__ nodes,
+                                                                            const float* __restrict__ keys, uint32_t left_handed, float4* __restrict__ objects,
+                                                                            uint32_t n_slots, float* __restrict__ sort_loc, uint32_t sort_n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_items) return;
+    const uint2 it = items[i];
+    const r3_object_pose_target tg = targets[it.y];
+    if (tg.slot >= n_slots) return;
+    const r3_pose_job job = jobs[it.x];
+    const r3_anim_node_clip clip = clips[job.clip];
+    float t = job.time;                                                  // time.clamp(0.0, duration) (lib.rs:190)
+    if (t < 0.0f) t = 0.0f;
+    if (t > clip.duration) t = clip.duration;
+    const r3_anim_node_channel* ch = channels + clip.first_channel + tg.channel;
+    const r3_anim_node* nd = nodes + ch->node;
+    // a missing property takes the node's bind pose (lib.rs:194-199)
+    const r3_anim_track tt = ch->translation, rt = ch->rotation, st = ch->scale;
+    const float3 tr = tt.times == R3_ANIM_ABSENT ? make_float3(nd->bind_translation[0], nd->bind_translation[1], nd->bind_translation[2]) : sample3(keys, tt, t);
+    const float4 q = rt.times == R3_ANIM_ABSENT ? make_float4(nd->bind_rotation[0], nd->bind_rotation[1], nd->bind_rotation[2], nd->bind_rotation[3])
+                                                : sample_quat(keys, rt, t);
+    float3 sc = st.times == R3_ANIM_ABSENT ? make_float3(nd->bind_scale[0], nd->bind_scale[1], nd->bind_scale[2]) : sample3(keys, st, t);
+    if (left_handed) sc.z = __uint_as_float(__float_as_uint(sc.z) ^ 0x80000000u);   // scale.z = -scale.z (lib.rs:201-203): a sign flip
+    float m[16];
+    from_srt(sc, q, tr, m);
+    // BoundingSphere::apply_transform (util/frustum.rs:22-32): Vec3::length_squared of each axis, f32::max (a NaN operand is ignored,
+    // as fmaxf ignores it), sqrt; centre = matrix * (c, 1) in mul_vec4's order; radius = max_scale * r
+    float ls[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) ls[a] = add_rn(add_rn(mul_rn(m[4 * a], m[4 * a]), mul_rn(m[4 * a + 1], m[4 * a + 1])), mul_rn(m[4 * a + 2], m[4 * a + 2]));
+    const float max_scale = sqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
+    const float4 c = mat_vec_rn(m, tg.mesh_sphere_center[0], tg.mesh_sphere_center[1], tg.mesh_sphere_center[2], 1.0f);
+    float4* rec = objects + (size_t)tg.slot * 8;
+    rec[0] = make_float4(m[0], m[1], m[2], m[3]); rec[1] = make_float4(m[4], m[5], m[6], m[7]);
+    rec[2] = make_float4(m[8], m[9], m[10], m[11]); rec[3] = make_float4(m[12], m[13], m[14], m[15]);
+    rec[4] = make_float4(c.x, c.y, c.z, mul_rn(max_scale, tg.mesh_sphere_radius));
+    // location = transform_point3a(Vec3A::ZERO): w + ((x * 0 + y * 0) + z * 0) per component — the translation for finite axes
+    if (sort_loc && tg.slot < sort_n) {
+        float* l = sort_loc + 3 * (size_t)tg.slot;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) l[k] = add_rn(m[12 + k], add_rn(add_rn(mul_rn(m[k], 0.0f), mul_rn(m[4 + k], 0.0f)), mul_rn(m[8 + k], 0.0f)));
+    }
+}
+
+// the sort locations of the posed slots, for the host mirror the host batching sorts by
+__global__ void gather_locations_kernel(const uint32_t* __restrict__ slots, uint32_t n, const float* __restrict__ sort_loc, uint32_t sort_n, float* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t s = slots[i];
+    if (s >= sort_n) return;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) out[3 * (size_t)i + k] = sort_loc[3 * (size_t)s + k];
+}
+
 // a device array of n elements, a copy of src unless src is null (allocated even when empty, so that kernels always get a valid pointer)
 template <typename T>
 int upload_array(r3_ctx* c, T** out, const T* src, uint64_t n, std::vector<void*>& made) {
@@ -241,6 +306,18 @@ struct r3_anim_state {
     r3_pose_job* d_jobs = nullptr; r3_pose_target* d_targets = nullptr; uint32_t n_jobs = 0;
     uint64_t* d_spill_offset = nullptr; float* d_spill = nullptr; uint32_t smem_bytes = 0;
     uint64_t jobs_cap = 0, targets_cap = 0, spill_offset_cap = 0, spill_cap = 0;   // grow-only (r3_set_pose_jobs runs every frame)
+    // r3_set_object_animations (independent of the skeletal state above)
+    bool has_obj_library = false; uint32_t left_handed = 0;
+    std::vector<r3_anim_node_clip> obj_clips;
+    r3_anim_node* d_nodes = nullptr; r3_anim_node_clip* d_node_clips = nullptr; r3_anim_node_channel* d_node_channels = nullptr; float* d_obj_keys = nullptr;
+    // r3_set_object_pose_jobs: the jobs and targets, and one item (job, target) per posed target with its slot
+    bool has_obj_jobs = false; uint32_t n_obj_items = 0;
+    r3_pose_job* d_obj_jobs = nullptr; r3_object_pose_target* d_obj_targets = nullptr; uint2* d_obj_items = nullptr; uint32_t* d_obj_slots = nullptr;
+    float* d_loc_stage = nullptr;
+    uint64_t obj_jobs_cap = 0, obj_targets_cap = 0, obj_items_cap = 0, obj_slots_cap = 0, loc_stage_cap = 0;   // grow-only
+    std::vector<uint32_t> obj_slots;          // host copy of d_obj_slots
+    std::vector<float> loc_stage;             // the posed slots' locations on their way to c->sort_loc
+    bool locations_pending = false;           // r3_pose_objects ran since c->sort_loc last took the posed locations
 
     void free_library() { for (void* p : {(void*)d_skins, (void*)d_joints, (void*)d_sched, (void*)d_levels, (void*)d_clips, (void*)d_channels, (void*)d_keys}) cudaFree(p);
                           d_skins = nullptr; d_joints = nullptr; d_sched = nullptr; d_levels = nullptr; d_clips = nullptr; d_channels = nullptr; d_keys = nullptr;
@@ -251,10 +328,18 @@ struct r3_anim_state {
     void free_jobs() { for (void* p : {(void*)d_jobs, (void*)d_targets, (void*)d_spill_offset, (void*)d_spill}) cudaFree(p);
                        d_jobs = nullptr; d_targets = nullptr; d_spill_offset = nullptr; d_spill = nullptr;
                        jobs_cap = targets_cap = spill_offset_cap = spill_cap = 0; drop_jobs(); }
+    void free_obj_library() { for (void* p : {(void*)d_nodes, (void*)d_node_clips, (void*)d_node_channels, (void*)d_obj_keys}) cudaFree(p);
+                              d_nodes = nullptr; d_node_clips = nullptr; d_node_channels = nullptr; d_obj_keys = nullptr;
+                              has_obj_library = false; left_handed = 0; obj_clips.clear(); }
+    void drop_obj_jobs() { has_obj_jobs = false; n_obj_items = 0; obj_slots.clear(); }   // the buffers stay for the next r3_set_object_pose_jobs
+    void free_obj_jobs() { for (void* p : {(void*)d_obj_jobs, (void*)d_obj_targets, (void*)d_obj_items, (void*)d_obj_slots, (void*)d_loc_stage}) cudaFree(p);
+                           d_obj_jobs = nullptr; d_obj_targets = nullptr; d_obj_items = nullptr; d_obj_slots = nullptr; d_loc_stage = nullptr;
+                           obj_jobs_cap = obj_targets_cap = obj_items_cap = obj_slots_cap = loc_stage_cap = 0; drop_obj_jobs(); }
 };
 
 void r3_anim_destroy(r3_ctx* c) {
     if (!c->anim) return;
+    c->anim->free_obj_jobs(); c->anim->free_obj_library();
     c->anim->free_jobs(); c->anim->free_skeletons(); c->anim->free_library();
     delete c->anim;
     c->anim = nullptr;
@@ -405,5 +490,137 @@ R3_EXPORT int r3_readback_joint_matrices(r3_ctx* c, float* out, uint32_t first, 
     cudaSetDevice(c->device);
     R3_CUDA(c, r3_stream_sync(c));
     R3_CUDA(c, cudaMemcpy(out, a->d_joint_buf + (size_t)first * 16, (size_t)n * 64, cudaMemcpyDeviceToHost));
+    return R3_OK;
+}
+
+// ------------------------------------------------------------------ object animation (the object-transform half of pose_animation_frame)
+// Host batching sorts by the host mirror c->sort_loc: after r3_pose_objects it takes the posed slots' locations from the device.  The
+// stage half enqueues a gather and its copy to the host (the caller drains the stream, which the host batching does anyway for the
+// visible list); the apply half writes them into the mirror.
+int r3_anim_stage_posed_locations(r3_ctx* c, bool* staged) {
+    *staged = false;
+    r3_anim_state* a = c->anim;
+    if (!a || !a->locations_pending) return R3_OK;
+    const uint32_t n = a->n_obj_items, sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    if (n == 0 || sort_n == 0 || !c->d_sort_loc) { a->locations_pending = false; return R3_OK; }
+    gather_locations_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(a->d_obj_slots, n, c->d_sort_loc, sort_n, a->d_loc_stage);
+    R3_CHECK_LAUNCH(c, "gather_locations_kernel");
+    a->loc_stage.resize(3 * (size_t)n);
+    R3_CUDA(c, cudaMemcpyAsync(a->loc_stage.data(), a->d_loc_stage, (size_t)n * 12, cudaMemcpyDeviceToHost, c->stream));
+    *staged = true;
+    return R3_OK;
+}
+void r3_anim_apply_posed_locations(r3_ctx* c) {
+    r3_anim_state* a = c->anim;
+    const size_t sort_n = c->sort_key.size();
+    for (size_t i = 0; i < a->obj_slots.size(); ++i)
+        if (a->obj_slots[i] < sort_n) memcpy(&c->sort_loc[3 * (size_t)a->obj_slots[i]], &a->loc_stage[3 * i], 12);
+    a->locations_pending = false;
+}
+// the same, blocking: before the posed slots' list is replaced
+static int refresh_posed_locations(r3_ctx* c) {
+    bool staged = false;
+    R3_TRY(r3_anim_stage_posed_locations(c, &staged));
+    if (!staged) return R3_OK;
+    R3_CUDA(c, r3_stream_sync(c));
+    r3_anim_apply_posed_locations(c);
+    return R3_OK;
+}
+
+R3_EXPORT int r3_set_object_animations(r3_ctx* c, const r3_anim_object_library* L) {
+    if (!c) return R3_E_INVALID;
+    const char* msg = "";
+    if (r3_anim_check_object_library(L, &msg) != R3_OK) return r3_fail(c, R3_E_INVALID, msg);
+    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_object_animations: the object buffer is borrowed (r3_set_objects_device)");
+    cudaSetDevice(c->device);
+    R3_TRY(anim_state(c));
+    r3_anim_state* a = c->anim;
+    r3_anim_state n;
+    const int rc = transactional(c, [&](std::vector<void*>& made) {
+        R3_TRY(upload_array(c, &n.d_nodes, L->nodes, L->n_nodes, made));
+        R3_TRY(upload_array(c, &n.d_node_clips, L->clips, L->n_clips, made));
+        R3_TRY(upload_array(c, &n.d_node_channels, L->channels, L->n_channels, made));
+        return upload_array(c, &n.d_obj_keys, L->keys, L->n_keys, made);
+    });
+    if (rc != R3_OK) return rc;
+    R3_TRY(refresh_posed_locations(c));
+    a->drop_obj_jobs();
+    a->free_obj_library();
+    a->d_nodes = n.d_nodes; a->d_node_clips = n.d_node_clips; a->d_node_channels = n.d_node_channels; a->d_obj_keys = n.d_obj_keys;
+    n.d_nodes = nullptr; n.d_node_clips = nullptr; n.d_node_channels = nullptr; n.d_obj_keys = nullptr;
+    a->obj_clips.assign(L->clips, L->clips + L->n_clips);
+    a->left_handed = L->left_handed ? 1u : 0u;
+    a->has_obj_library = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_set_object_pose_jobs(r3_ctx* c, const r3_pose_job* jobs, uint32_t n_jobs, const r3_object_pose_target* targets, uint32_t n_targets) {
+    if (!c) return R3_E_INVALID;
+    r3_anim_state* a = c->anim;
+    if (!a || !a->has_obj_library) return r3_fail(c, R3_E_STATE, "set_object_pose_jobs before set_object_animations");
+    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_object_pose_jobs: the object buffer is borrowed (r3_set_objects_device)");
+    const char* msg = "";
+    uint32_t* listed = nullptr;
+    uint64_t n_items = 0;
+    if (r3_anim_check_object_jobs(a->obj_clips.data(), (uint32_t)a->obj_clips.size(), c->n_slots, jobs, n_jobs, targets, n_targets, &listed, &n_items, &msg) != R3_OK)
+        return r3_fail(c, R3_E_INVALID, msg);
+    std::vector<uint32_t> slots(listed, listed + n_items);
+    free(listed);
+    std::vector<uint2> items;
+    items.reserve(n_items);
+    for (uint32_t i = 0; i < n_jobs; ++i)
+        for (uint32_t t = 0; t < jobs[i].target_count; ++t) items.push_back(make_uint2(i, jobs[i].first_target + t));
+    const uint32_t n = (uint32_t)n_items;   // distinct slots below n_slots
+    cudaSetDevice(c->device);
+    R3_TRY(refresh_posed_locations(c));
+    // the call is made every simulation frame: the buffers only grow, and a growth keeps the current jobs (a failed one leaves them)
+    R3_TRY(r3_reserve_t(c, &a->d_obj_jobs, &a->obj_jobs_cap, std::max(n_jobs, 1u), true));
+    R3_TRY(r3_reserve_t(c, &a->d_obj_targets, &a->obj_targets_cap, std::max(n_targets, 1u), true));
+    R3_TRY(r3_reserve_t(c, &a->d_obj_items, &a->obj_items_cap, std::max(n, 1u), true));
+    R3_TRY(r3_reserve_t(c, &a->d_obj_slots, &a->obj_slots_cap, std::max(n, 1u), true));
+    R3_TRY(r3_reserve_t(c, &a->d_loc_stage, &a->loc_stage_cap, 3 * (uint64_t)std::max(n, 1u), false));
+    if (n_jobs) R3_CUDA(c, cudaMemcpyAsync(a->d_obj_jobs, jobs, (size_t)n_jobs * sizeof(r3_pose_job), cudaMemcpyHostToDevice, c->stream));
+    if (n_targets) R3_CUDA(c, cudaMemcpyAsync(a->d_obj_targets, targets, (size_t)n_targets * sizeof(r3_object_pose_target), cudaMemcpyHostToDevice, c->stream));
+    if (n) {
+        R3_CUDA(c, cudaMemcpyAsync(a->d_obj_items, items.data(), (size_t)n * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
+        R3_CUDA(c, cudaMemcpyAsync(a->d_obj_slots, slots.data(), (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
+    }
+    R3_CUDA(c, r3_stream_sync(c));                                    // host pointers are only borrowed for the call
+    a->n_obj_items = n;
+    a->obj_slots.swap(slots);
+    a->has_obj_jobs = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_pose_objects(r3_ctx* c) {
+    if (!c) return R3_E_INVALID;
+    r3_anim_state* a = c->anim;
+    if (!a || !a->has_obj_jobs) return r3_fail(c, R3_E_STATE, "pose_objects before set_object_animations + set_object_pose_jobs");
+    if (!c->d_objects) return r3_fail(c, R3_E_STATE, "pose_objects before set_objects");
+    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "pose_objects: the object buffer is borrowed (r3_set_objects_device)");
+    if (a->n_obj_items == 0) return R3_OK;
+    cudaSetDevice(c->device);
+    const uint32_t n = a->n_obj_items, sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    pose_objects_kernel<<<(n + R3_OBJ_POSE_THREADS - 1) / R3_OBJ_POSE_THREADS, R3_OBJ_POSE_THREADS, 0, c->stream>>>(
+        a->d_obj_items, n, a->d_obj_jobs, a->d_obj_targets, a->d_node_clips, a->d_node_channels, a->d_nodes, a->d_obj_keys, a->left_handed,
+        reinterpret_cast<float4*>(c->d_objects), c->n_slots, c->d_sort_loc, sort_n);
+    R3_CHECK_LAUNCH(c, "pose_objects_kernel");
+    R3_TRY(r3_split_slots(c, a->d_obj_slots, n));                     // rows_xyz / rows_w / spheres and the affine bit of the posed slots
+    r3_new_frame_epoch(c);                                            // a frame-wide sort made before the pose is stale
+    a->locations_pending = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_readback_objects(r3_ctx* c, r3_object* out, float* locations, uint32_t first, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (!out && n) return r3_fail(c, R3_E_INVALID, "readback_objects: null");
+    if ((uint64_t)first + n > c->n_slots) return r3_fail(c, R3_E_INVALID, "readback_objects: range outside the object buffer");
+    if (locations && (uint64_t)first + n > (c->have_live ? c->sort_key.size() : 0u))
+        return r3_fail(c, R3_E_INVALID, "readback_objects: range outside the sort info");
+    if (n == 0) return R3_OK;
+    cudaSetDevice(c->device);
+    R3_CUDA(c, r3_stream_sync(c));
+    R3_CUDA(c, cudaMemcpy(out, c->d_objects + first, (size_t)n * sizeof(r3_object), cudaMemcpyDeviceToHost));
+    if (locations) R3_CUDA(c, cudaMemcpy(locations, c->d_sort_loc + 3 * (size_t)first, (size_t)n * 12, cudaMemcpyDeviceToHost));
     return R3_OK;
 }

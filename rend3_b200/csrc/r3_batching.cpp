@@ -44,12 +44,16 @@ int r3_host_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], uint
     if (!cam->header_set) return r3_fail(c, R3_E_STATE, "batch_objects before object_uniform_upload");
     const uint32_t cap = cam->header.object_count;
     if (c->sort_key.size() < cap) return r3_fail(c, R3_E_STATE, "batch_objects needs r3_set_object_sort_info");
-    // visible list: the only device->host transfer of the frame (4 B per visible object)
+    // visible list: the only device->host transfer of the frame (4 B per visible object), and with it the locations of the objects
+    // r3_pose_objects posed since the host mirror last took them (12 B per posed object), so that no extra drain is needed
     uint32_t nv = 0;
-    if (cam->d_visible_count) {
-        R3_CUDA(c, cudaMemcpyAsync(&nv, cam->d_visible_count, 4, cudaMemcpyDeviceToHost, c->stream));
+    bool staged = false;
+    R3_TRY(r3_anim_stage_posed_locations(c, &staged));
+    if (cam->d_visible_count || staged) {
+        if (cam->d_visible_count) R3_CUDA(c, cudaMemcpyAsync(&nv, cam->d_visible_count, 4, cudaMemcpyDeviceToHost, c->stream));
         R3_CUDA(c, r3_stream_sync(c));
     }
+    if (staged) r3_anim_apply_posed_locations(c);
     cam->visible_count_host = (int)nv;
     std::vector<uint32_t> visible(nv), index_count(nv);
     if (nv) {

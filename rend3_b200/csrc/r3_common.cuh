@@ -222,6 +222,10 @@ int r3_iobuf_swap(r3_ctx* c, r3_iobuf* b, uint64_t new_elems);
 int r3_launch_skinning(r3_ctx* c, const r3_skinning_input* d_inputs, const uint32_t* d_chunk_prefix, uint32_t n_skeletons, uint32_t total_chunks,
                        const float* d_joints, uint32_t n_joints);
 void r3_anim_destroy(r3_ctx* c);             // r3_animation.cu: frees c->anim (r3_ctx_destroy)
+// r3_animation.cu: after r3_pose_objects the host mirror c->sort_loc is behind the device's.  stage enqueues a copy of the posed slots'
+// locations to the host (*staged = true when it did); once the caller has drained the stream, apply writes them into c->sort_loc.
+int r3_anim_stage_posed_locations(r3_ctx* c, bool* staged);
+void r3_anim_apply_posed_locations(r3_ctx* c);
 
 #ifdef __CUDACC__
 // IEEE, never-contracted arithmetic for the bit-exact stages (SURVEY D7)

@@ -127,7 +127,7 @@ class BaseRenderGraph:
                      settings: BaseRenderGraphSettings = BaseRenderGraphSettings(), srgb_target: bool = True,
                      upload: bool = True, scissor_rows: Optional[Tuple[int, int]] = None, shadow_filter=None, after_shadows=None,
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
-                     posed_skinning: bool = False):
+                     posed_skinning: bool = False, posed_objects: bool = False):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -139,7 +139,9 @@ class BaseRenderGraph:
         environment variable.  `skinning` = (records, joint matrices) skins with r3_skin, which uploads the matrices and waits for the
         stream (a recorded frame flushes there); `posed_skinning` instead poses the skeletons on the device and skins from the resident
         records and joint buffer (r3_pose_skeletons + r3_skin_posed after r3_set_animations / r3_set_skeletons / r3_set_pose_jobs):
-        only enqueued work, so the frame stays one graph."""
+        only enqueued work, so the frame stays one graph.  `posed_objects` poses the animated nodes' objects on the device first
+        (r3_pose_objects after r3_set_object_animations / r3_set_object_pose_jobs): their transforms, world spheres and sort locations
+        are written before any camera culls, also enqueue only."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -164,6 +166,8 @@ class BaseRenderGraph:
         b.set_frame_uniforms(frame_uniforms(ev.camera, settings.ambient_color, resolution))  # :142
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
+        if posed_objects:                                                         # :145 pose_animation_frame's set_object_transform half
+            b.pose_objects()
         if posed_skinning:                                                        # :145 from resident data (r3_set_skeletons / r3_set_pose_jobs)
             b.pose_skeletons()
             b.skin_posed()

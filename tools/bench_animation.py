@@ -1,11 +1,15 @@
 """Crowd animation benchmark: device posing (r3_pose_skeletons) and skinning from resident joint matrices (r3_skin_posed) against the
 host path they replace (the oracle's pose on the CPU + r3_skin's per-frame upload and stream drain).  Prints one JSON line.
 
+With --objects K > 0 each instance also carries K posed objects (one per animated node, translation / rotation / scale tracks of 60
+keys), and the line gains "objects": the device time of r3_pose_objects (pose + the cull's dense copies) against the host path it
+replaces — the oracle's object pose, then r3_update_objects and r3_update_object_sort_info of the posed slots, each ending in a drain.
+
 Workload: --instances instances (default 4096) of a 65-joint humanoid-shaped skin of depth 10, two skeletons (primitives) per instance
 of --vertices vertices each (default 1000), one clip with translation, rotation and scale channels of 60 keys on every joint.  The
 instances share the two meshes' source attributes and each skeleton has its own skinned ranges, as SkeletonManager lays them out.
 
-Usage: python tools/bench_animation.py [--instances N] [--vertices V] [--iters K] [--warmup W]"""
+Usage: python tools/bench_animation.py [--instances N] [--vertices V] [--objects K] [--iters I] [--warmup W]"""
 import argparse
 import json
 import math
@@ -67,12 +71,70 @@ def pose_bytes(jobs, targets, library, n_keys):
     return {"requested_read_bytes": reads, "written_bytes": writes, "distinct_read_bytes": unique}
 
 
+def object_bench(args, b, device_ms):
+    """r3_pose_objects over instances x objects posed objects against the host pose + r3_update_objects + r3_update_object_sort_info."""
+    import animation_case
+    import object_animation_case
+    from oracle.objanim import load_objanim_oracle_backend
+    from rend3_b200.animation import Animation, Node, NodeChannels, ObjectAnimationData
+
+    rng = np.random.default_rng(1)
+    k, duration = args.objects, 2.0
+    nodes = [Node(None, rng.uniform(-3, 3, 3).astype(f32), animation_case._unit_quat(rng), (1.0, 1.0, 1.0),
+                  [(i, rng.uniform(-1, 1, 3).astype(f32), f32(1.5))]) for i in range(k)]
+    channels = {i: NodeChannels(animation_case._track(rng, 60, 3, duration), animation_case._track(rng, 60, 4, duration),
+                                animation_case._track(rng, 60, 3, duration)) for i in range(k)}
+    data = ObjectAnimationData(nodes, [Animation(channels, duration)], left_handed=True)
+    jobs, targets = data.pose_jobs([(0, float(rng.uniform(0, duration)), i * k) for i in range(args.instances)])
+    n = args.instances * k
+    records = object_animation_case._records(n, rng)
+    key, flags, loc = np.zeros(n, np.uint64), np.ones(n, np.uint8), rng.uniform(-9, 9, (n, 3)).astype(f32)
+    b.set_objects(records)
+    b.set_object_sort_info(key, flags, loc)
+    data.upload(b)
+    b.set_object_pose_jobs(jobs, targets)
+    pose_ms = device_ms(b.pose_objects)
+    got_r, got_l = b.readback_objects(0, n)
+
+    orc = load_objanim_oracle_backend()
+    orc.set_objects(records)
+    orc.set_object_sort_info(key, flags, loc)
+    data.upload(orc)
+    orc.set_object_pose_jobs(jobs, targets)
+    orc.pose_objects()
+    t0 = time.perf_counter()
+    for _ in range(5):
+        orc.pose_objects()
+    host_pose_ms = (time.perf_counter() - t0) * 1e3 / 5
+    want_r, want_l = orc.readback_objects(0, n)
+    orc.close()
+    same = bool(np.array_equal(got_r.view(np.uint32).reshape(n, 32)[:, :30], want_r.view(np.uint32).reshape(n, 32)[:, :30])
+                and np.array_equal(got_l.view(np.uint32), want_l.view(np.uint32)))
+
+    slots = np.arange(n, dtype=np.uint32)
+    def upload():
+        b.update_objects(slots, want_r)
+        b.update_object_sort_info(slots, key, flags, want_l)
+    for _ in range(3):
+        upload()
+    t0 = time.perf_counter()
+    reps = 20
+    for _ in range(reps):
+        upload()
+    upload_ms = (time.perf_counter() - t0) * 1e3 / reps
+    return {"instances": args.instances, "objects_per_instance": k, "objects_posed": n, "pose_objects_ms": round(pose_ms, 4),
+            "host_alternative": {"oracle_object_pose_ms": round(host_pose_ms, 3),
+                                 "update_objects_and_sort_info_ms": round(upload_ms, 3), "bytes_uploaded_per_frame": n * (128 + 4 + 4 + 8 + 1 + 12)},
+            "device_pose_equals_oracle": same}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--instances", type=int, default=4096)
     ap.add_argument("--vertices", type=int, default=1000)
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--objects", type=int, default=0, help="posed objects per instance (0: skeletons only)")
     args = ap.parse_args()
 
     import torch
@@ -154,6 +216,7 @@ def main():
     host_pose_ms = (time.perf_counter() - t0) * 1e3 / 5
     same = bool(np.array_equal(orc.readback_joint_matrices(0, len(buf)).view(np.uint32), posed.view(np.uint32)))
     orc.close()
+    objects = object_bench(args, b, device_ms) if args.objects > 0 else None
     b.close()
 
     model = pose_bytes(jobs, targets, data.library, 60)
@@ -170,6 +233,7 @@ def main():
         "host_alternative": {"oracle_pose_ms": round(host_pose_ms, 3), "oracle_threads": threads, "r3_skin_upload_and_sync_ms": round(skin_host_ms, 3),
                              "joint_bytes_uploaded_per_frame": 64 * len(buf)},
         "device_pose_equals_oracle": same,
+        **({"objects": objects} if objects is not None else {}),
     }))
 
 
