@@ -165,6 +165,20 @@ typedef struct r3_directional_light {
 R3_STATIC_ASSERT(sizeof(r3_directional_light) == 128, "DirectionalLight");
 R3_STATIC_ASSERT(offsetof(r3_directional_light, atlas_offset) == 104, "atlas_offset");
 
+/* One directional light as the caller keeps it — rend3-types DirectionalLight (colour, intensity, direction, distance, resolution) —
+ * plus its placement in the shadow atlas (directional/shadow_alloc.rs), in texels.  r3_set_directional_light_sources; host only. */
+typedef struct r3_directional_light_source {
+    float color[3];               /* @0 */
+    float intensity;              /* @12 */
+    float direction[3];           /* @16 un-normalised, as given */
+    float distance;               /* @28 side of the shadow camera's box */
+    uint32_t resolution;          /* @32 shadow map texels along a side (texel = distance / resolution) */
+    uint32_t offset[2];           /* @36 atlas placement, texels */
+    uint32_t size;                /* @44 */
+} r3_directional_light_source;
+R3_STATIC_ASSERT(sizeof(r3_directional_light_source) == 48, "DirectionalLight source");
+R3_STATIC_ASSERT(offsetof(r3_directional_light_source, resolution) == 32, "resolution");
+
 /* ShaderPointLight — rend3/src/managers/point.rs:21-26; buffer = u32 count @0, array @16 */
 typedef struct r3_point_light {
     float position[4];

@@ -20,14 +20,15 @@
  *   - one context per GPU; calls on a context must be externally serialised (this is the
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
- *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_exchange_merge, r3_peer_*) only enqueue work on the
+ *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_evaluate_shadow_cameras, r3_shadow_uniform_upload,
+ *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
  *     r3_batch_counts / r3_batching_info / r3_forward_stats / r3_stage_times (small device-to-host reads), and the
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
  *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices, r3_set_object_animations,
- *     r3_set_object_pose_jobs —
+ *     r3_set_object_pose_jobs, r3_set_directional_light_sources, r3_readback_shadow_cameras —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
  *     has to grow (first frame, larger world, new resolution) is reallocated with a stream synchronisation as well.
@@ -139,6 +140,26 @@ int r3_set_skybox(r3_ctx*, const r3_texture_desc* desc, const void* texels, uint
 int r3_set_directional_lights(r3_ctx*, const void* bytes, uint64_t nbytes,
                               uint32_t atlas_width, uint32_t atlas_height);         /* directional.rs:135-156 */
 int r3_set_point_lights(r3_ctx*, const void* bytes, uint64_t nbytes);              /* point.rs:58-74 */
+/* DirectionalLightManager::evaluate (directional.rs:99-157) on the device, with the shadow camera arithmetic of rule R13 (DESIGN.md §2).
+ *   r3_set_directional_light_sources  blocking: the lights and their atlas placements.  Fills the light buffer's static fields
+ *                                     (colour * intensity, direction, 1 / atlas size, offset / atlas size, size / atlas size) and
+ *                                     allocates the atlas as r3_set_directional_lights does.  Checked first: n <= R3_MAX_SHADOWS, every
+ *                                     size > 0 and every placement inside the atlas; a rejected call (R3_E_INVALID) leaves the context as
+ *                                     it was.  This call and r3_set_directional_lights each replace what the other set.
+ *   r3_evaluate_shadow_cameras        enqueue only: one kernel writes every light's view_proj into the light buffer and its shadow camera
+ *                                     (view, view_proj, frustum) into a device-resident block, around viewport_location.  Call it once
+ *                                     per frame after r3_set_frame_uniforms; in a frame graph the kernel's arguments are updated in place.
+ *   r3_shadow_uniform_upload          enqueue only: r3_object_uniform_upload for camera shadow_index, with view, view_proj and frustum
+ *                                     read on the device from that block.  resolution = (size, size), flags from the handedness
+ *                                     (single-sampled; shadow cameras cull front faces).  R3_E_STATE before sources are set or before an
+ *                                     evaluation since they were set; R3_E_INVALID for shadow_index >= n or object_count > the slots.
+ *   r3_readback_shadow_cameras        blocking: the first n evaluated headers (object_count 0: it is given per upload) and, unless null,
+ *                                     the light records. */
+int r3_set_directional_light_sources(r3_ctx*, const r3_directional_light_source* lights, uint32_t n, uint32_t atlas_width,
+                                     uint32_t atlas_height, uint32_t left_handed);
+int r3_evaluate_shadow_cameras(r3_ctx*, const float viewport_location[3]);
+int r3_shadow_uniform_upload(r3_ctx*, uint32_t shadow_index, uint32_t object_count, uint32_t mode);
+int r3_readback_shadow_cameras(r3_ctx*, r3_camera_header* out, r3_directional_light* lights_or_null, uint32_t n);
 int r3_set_frame_uniforms(r3_ctx*, const r3_frame_uniforms* uniforms);             /* uniforms.rs:94-106 */
 
 /* ------------------------------------------------------------------ GPU skinning

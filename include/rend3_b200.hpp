@@ -59,6 +59,9 @@ struct EvalOutput {
     const r3_texture_desc* textures = nullptr; uint32_t n_textures = 0; const void* texels = nullptr; uint64_t texel_bytes = 0;
     const r3_texture_desc* skybox = nullptr; const void* skybox_texels = nullptr; uint64_t skybox_bytes = 0;     // SkyboxRoutine's cube map (null = none)
     const void* directional_lights = nullptr; uint64_t directional_bytes = 0; uint32_t shadow_target_size[2] = {0, 0};
+    // the same lights as sources + atlas placements, in the light buffer's order, and the handedness: what
+    // r3_set_directional_light_sources takes when the shadow cameras are evaluated on the device
+    const r3_directional_light_source* directional_sources = nullptr; uint32_t n_directional_sources = 0; bool left_handed = true;
     const void* point_lights = nullptr; uint64_t point_bytes = 0;
     std::vector<ShadowMap> shadows;
     r3_camera_header viewport{};              // PerCameraUniform header of the viewport camera for this target
@@ -93,14 +96,19 @@ public:
     void check(int rc) const { if (rc != R3_OK) throw Error(rc, r3_last_error(ctx_)); }
 
     // renderer/eval.rs:157-181 — the buffers evaluate_instructions (re)uploads
-    void upload_world(const EvalOutput& ev) {
+    // device_shadow_cameras: the lights go up as sources (the frame evaluates their shadow cameras) instead of the light buffer
+    void upload_world(const EvalOutput& ev, bool device_shadow_cameras = false) {
         check(r3_set_objects(ctx_, ev.objects, ev.n_slots));
         if (ev.material_key) check(r3_set_object_sort_info(ctx_, ev.material_key, ev.sort_flags, ev.location, ev.n_slots));
         check(r3_set_mesh_buffer(ctx_, ev.mesh_buffer, ev.mesh_bytes));
         check(r3_set_textures(ctx_, ev.textures, ev.n_textures, ev.texels, ev.texel_bytes));
         check(r3_set_skybox(ctx_, ev.skybox, ev.skybox_texels, ev.skybox_bytes));
         check(r3_set_materials(ctx_, ev.materials, ev.n_materials));
-        check(r3_set_directional_lights(ctx_, ev.directional_lights, ev.directional_bytes, ev.shadow_target_size[0], ev.shadow_target_size[1]));
+        if (device_shadow_cameras)
+            check(r3_set_directional_light_sources(ctx_, ev.directional_sources, ev.n_directional_sources, ev.shadow_target_size[0], ev.shadow_target_size[1],
+                                                   ev.left_handed ? 1u : 0u));
+        else
+            check(r3_set_directional_lights(ctx_, ev.directional_lights, ev.directional_bytes, ev.shadow_target_size[0], ev.shadow_target_size[1]));
         check(r3_set_point_lights(ctx_, ev.point_lights, ev.point_bytes));
     }
     void sync() { check(r3_sync(ctx_)); }
@@ -163,6 +171,9 @@ public:
     HiZRoutine hi_z;
     TonemappingRoutine tonemapping;
     bool submit_as_graph = false;             // record the frame and submit it as one CUDA graph launch (graph.rs:510: one submit per frame)
+    // DirectionalLightManager::evaluate on the device (after Renderer::upload_world(ev, true)): the shadow cameras are evaluated around
+    // this frame's viewport_location and culled from device memory; ev.shadows' headers are not read, only their atlas viewports
+    bool device_shadow_cameras = false;
 
     void add_to_graph(Renderer& r, const EvalOutput& ev, uint32_t width, uint32_t height, SampleCount samples, const BaseRenderGraphSettings& settings,
                       bool target_is_srgb = true) {
@@ -170,8 +181,12 @@ public:
         if (submit_as_graph) r.check(r3_frame_begin(r.raw()));
         r.check(r3_clear_shadow_atlas(r.raw()));                                                     // base.rs:139
         r.check(r3_set_frame_uniforms(r.raw(), &ev.uniforms));                                       // :142
+        if (device_shadow_cameras) r.check(r3_evaluate_shadow_cameras(r.raw(), ev.viewport_location));
         gpu_skinner.add_skinning_to_graph(r, ev);                                                    // :145 state.skinning — before any camera culls
-        for (uint32_t i = 0; i < ev.shadows.size(); ++i) gpu_culler.object_uniform_upload(r, CameraSpecifier::Shadow(i), ev.shadows[i].header);   // :148
+        for (uint32_t i = 0; i < ev.shadows.size(); ++i) {                                          // :148
+            if (device_shadow_cameras) r.check(r3_shadow_uniform_upload(r.raw(), i, ev.n_slots, R3_CB_BAKE | R3_CB_CULL));
+            else gpu_culler.object_uniform_upload(r, CameraSpecifier::Shadow(i), ev.shadows[i].header);
+        }
         for (uint32_t i = 0; i < ev.shadows.size(); ++i) gpu_culler.add_culling_to_graph(r, CameraSpecifier::Shadow(i), ev.viewport_location);     // :150
         for (uint32_t i = 0; i < ev.shadows.size(); ++i) forward.add_shadow_to_graph(r, i, ev.shadows[i]);                                         // :153
         gpu_culler.object_uniform_upload(r, CameraSpecifier::Viewport(), ev.viewport);               // :156

@@ -204,6 +204,30 @@ class Backend:
     def set_directional_lights(self, data: bytes, atlas_w: int, atlas_h: int):
         self._call("set_directional_lights", C.c_char_p(data), C.c_uint64(len(data)), C.c_uint32(atlas_w), C.c_uint32(atlas_h))
 
+    # ---- directional lights evaluated on the device (rule R13)
+    def set_directional_light_sources(self, sources: np.ndarray, atlas_w: int, atlas_h: int, left_handed: bool):
+        from .layouts import LIGHT_SOURCE_DTYPE
+
+        src = np.ascontiguousarray(sources, dtype=LIGHT_SOURCE_DTYPE).reshape(-1)
+        self._call("set_directional_light_sources", _ptr(src) if len(src) else None, C.c_uint32(len(src)), C.c_uint32(atlas_w),
+                   C.c_uint32(atlas_h), C.c_uint32(1 if left_handed else 0))
+
+    def evaluate_shadow_cameras(self, viewport_location):
+        loc = np.ascontiguousarray(viewport_location, dtype=np.float32).reshape(3)
+        self._call("evaluate_shadow_cameras", _ptr(loc))
+
+    def shadow_uniform_upload(self, shadow_index: int, object_count: int, mode: int = CB_BAKE | CB_CULL):
+        self._call("shadow_uniform_upload", C.c_uint32(shadow_index), C.c_uint32(object_count), C.c_uint32(mode))
+
+    def readback_shadow_cameras(self, n: int):
+        """(CAMERA_HEADER_DTYPE[n], DIRECTIONAL_LIGHT_DTYPE[n])"""
+        from .layouts import DIRECTIONAL_LIGHT_DTYPE
+
+        heads = np.zeros(max(n, 1), dtype=CAMERA_HEADER_DTYPE)
+        lights = np.zeros(max(n, 1), dtype=DIRECTIONAL_LIGHT_DTYPE)
+        self._call("readback_shadow_cameras", _ptr(heads), _ptr(lights), C.c_uint32(n))
+        return heads[:n], lights[:n]
+
     def set_point_lights(self, data: bytes):
         self._call("set_point_lights", C.c_char_p(data), C.c_uint64(len(data)))
 

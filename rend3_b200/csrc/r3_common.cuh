@@ -123,6 +123,11 @@ struct r3_ctx {
     bool has_skybox = false; r3_texture_desc sky_desc{}; uint8_t* d_sky_texels = nullptr; uint64_t sky_cap = 0;   // cube map of the skybox routine
     r3_texture_desc* d_tex_descs = nullptr; uint32_t n_textures = 0, tex_descs_cap = 0; uint8_t* d_texels = nullptr; uint64_t texels_cap = 0, texel_bytes = 0;
     r3_directional_light* d_dir = nullptr; uint32_t n_dir = 0, dir_cap = 0;
+    // shadow cameras evaluated on the device (r3_lights.cu): the sources of r3_set_directional_light_sources and one camera header per
+    // light (view, view_proj, frustum written by the evaluation), both sized R3_MAX_SHADOWS; host copies of the placements
+    r3_directional_light_source* d_light_src = nullptr; r3_camera_header* d_shadow_cams = nullptr;
+    std::vector<r3_directional_light_source> light_src;
+    bool light_src_set = false, shadow_cams_evaluated = false; uint32_t light_src_left_handed = 0;
     r3_point_light* d_point = nullptr; uint32_t n_point = 0, point_cap = 0;
     float* d_light_mats = nullptr; uint64_t light_mats_cap = 0;   // view-space light tables built by light_prep_kernel
     r3_frame_uniforms uniforms{}; bool uniforms_set = false;
@@ -203,6 +208,9 @@ int r3_reserve_t(r3_ctx* c, T** ptr, C* cap, uint64_t need, bool keep = false, b
 
 // stages implemented in the other translation units
 int r3_launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode);
+// the same with view, view_proj and frustum read on the device from d_header (r3_shadow_uniform_upload); the rest from cam->header
+int r3_launch_cull_bake_device_camera(r3_ctx* c, r3_camera* cam, uint32_t mode, const r3_camera_header* d_header);
+int r3_camera_buffers(r3_ctx* c, r3_camera* cam, uint32_t mode);   // r3_object_uniform_upload's per-camera allocations
 int r3_split_objects(r3_ctx* c);
 int r3_split_slots(r3_ctx* c, const uint32_t* d_slots, uint32_t n);
 int r3_grow_hot(r3_ctx* c, uint32_t old_n, uint32_t n);   // r3_resize_objects: keep the hot copies of slots < old_n, zero slots [old_n, n)

@@ -80,7 +80,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
     cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc); cudaFree(c->d_gsort_keys[0]); cudaFree(c->d_gsort_keys[1]); cudaFree(c->d_gsort_hist); cudaFree(c->d_gsort_header);
     cudaFree(c->d_live_bits); cudaFree(c->d_mesh); cudaFree(c->d_materials); cudaFree(c->d_dir); cudaFree(c->d_point);
-    cudaFree(c->d_light_mats); cudaFree(c->d_atlas);
+    cudaFree(c->d_light_mats); cudaFree(c->d_atlas); cudaFree(c->d_light_src); cudaFree(c->d_shadow_cams);
     for (auto& k : c->cams) {
         cudaFree(k.d_matrices); cudaFree(k.d_visible); cudaFree(k.d_visible_count); cudaFree(k.d_tile_state);
         if (k.d_gathered) {   // visible-set exchange: unmap the peers' buffers, free ours
@@ -579,6 +579,7 @@ R3_EXPORT int r3_set_directional_lights(r3_ctx* c, const void* bytes, uint64_t n
     R3_TRY(r3_reserve_t(c, &c->d_dir, &c->dir_cap, n));
     if (n) R3_CUDA(c, cudaMemcpyAsync(c->d_dir, (const uint8_t*)bytes + 16, (size_t)n * sizeof(r3_directional_light), cudaMemcpyHostToDevice, c->stream));
     c->n_dir = n;
+    c->light_src_set = false;   // replaces r3_set_directional_light_sources
     if (aw != c->atlas_w || ah != c->atlas_h || !c->d_atlas) {
         R3_CUDA(c, r3_stream_sync(c));
         cudaFree(c->d_atlas);
@@ -623,7 +624,11 @@ R3_EXPORT int r3_object_uniform_upload(r3_ctx* c, uint32_t camera, const r3_came
     if (h->object_count > c->n_slots) return r3_fail(c, R3_E_INVALID, "object_count exceeds the object buffer");
     cam->header = *h;
     cam->header_set = true;
-    const uint32_t n = h->object_count;
+    R3_TRY(r3_camera_buffers(c, cam, mode));
+    return r3_launch_cull_bake(c, cam, mode);
+}
+int r3_camera_buffers(r3_ctx* c, r3_camera* cam, uint32_t mode) {
+    const uint32_t n = cam->header.object_count;
     if (mode & R3_CB_BAKE) {
         // a resized per-camera buffer starts zeroed (culler.rs:459-476: new buffer when the size changes)
         if (cam->matrices_cap < n || !cam->d_matrices) {
@@ -641,7 +646,7 @@ R3_EXPORT int r3_object_uniform_upload(r3_ctx* c, uint32_t camera, const r3_came
     }
     if (mode & R3_CB_CULL) R3_TRY(r3_reserve_t(c, &cam->d_visible, &cam->visible_cap, (uint64_t)n + 1));
     cam->visible_count_host = -1;
-    return r3_launch_cull_bake(c, cam, mode);
+    return R3_OK;
 }
 R3_EXPORT int r3_visible_count(r3_ctx* c, uint32_t camera, uint32_t* count) {
     R3_CAM_OR_FAIL(c, camera);

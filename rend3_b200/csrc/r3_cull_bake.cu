@@ -34,6 +34,7 @@
 // (History: a single-pass kernel with a decoupled look-back lost time to look-back stalls; the
 //  two-kernel AoS version ran at the copy bandwidth but moved 256 B per object.)
 #include <cstdlib>
+#include <type_traits>
 
 #include "r3_common.cuh"
 #include "r3_scan.cuh"
@@ -54,6 +55,12 @@ struct CullBakeParams {
     float frustum[5][4];
     uint32_t object_count;
 };
+// r3_shadow_uniform_upload: the camera lives in device memory (written by r3_evaluate_shadow_cameras in the same stream)
+struct DeviceCameraParams {
+    const r3_camera_header* cam;
+    uint32_t object_count;
+};
+constexpr int CAM_FLOATS = 52;   // view[16] | view_proj[16] | frustum[5][4], staged in shared memory by DeviceCameraParams launches
 
 // Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine
 // (a product with -0.0 can carry its sign into MV / MVP).
@@ -115,14 +122,27 @@ __global__ void __launch_bounds__(256) split_slots_kernel(const float4* __restri
     }
 }
 
-template <bool BAKE, bool CULL, bool LIVE>
+template <bool BAKE, bool CULL, bool LIVE, typename Params = CullBakeParams>
 __global__ void __launch_bounds__(CB_THREADS)
 cull_bake_kernel(const float4* __restrict__ rows_xyz, const float* __restrict__ rows_w, const uint32_t* __restrict__ affine_bits, const float4* __restrict__ spheres,
                  const uint32_t* __restrict__ enabled_bits, const uint32_t* __restrict__ live_bits, float4* __restrict__ matrices, uint32_t* __restrict__ words,
-                 uint32_t* __restrict__ cta_counts, const __grid_constant__ CullBakeParams p) {
+                 uint32_t* __restrict__ cta_counts, const __grid_constant__ Params p) {
     __shared__ uint32_t s_count[CB_WARPS];
     __shared__ float4 s_rows[BAKE ? CB_WARPS : 1][96];   // per warp: rows 0-2 of its 32 slots
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const float* view;
+    const float* view_proj;
+    const float* frustum;   // [5][4]
+    if constexpr (std::is_same<Params, DeviceCameraParams>::value) {
+        // one copy per CTA: the operands the constant bank holds for the other instantiations
+        __shared__ float s_cam[CAM_FLOATS];
+        const float* src = reinterpret_cast<const float*>(p.cam);
+        if (threadIdx.x < CAM_FLOATS) s_cam[threadIdx.x] = __ldg(src + (threadIdx.x < 32 ? threadIdx.x : threadIdx.x + 4));   // frustum at float 36
+        __syncthreads();
+        view = s_cam; view_proj = s_cam + 16; frustum = s_cam + 32;
+    } else {
+        view = p.view; view_proj = p.view_proj; frustum = &p.frustum[0][0];
+    }
     const int col = lane & 3, sub = lane >> 2;   // transform column / slot within an 8-slot group
     uint32_t count = 0;
 #pragma unroll 2
@@ -160,8 +180,8 @@ cull_bake_kernel(const float4* __restrict__ rows_xyz, const float* __restrict__ 
                     // affine slot: row 3 is bit for bit (+0, +0, +0, 1), so the constant is the element it would have read
                     const float w = ((affine >> slot) & 1u) ? (col == 3 ? 1.0f : 0.0f) : __ldcs(&rows_w[(size_t)obj * 4 + col]);
                     float4* dst = &matrices[(size_t)obj * 8 + col];
-                    __stcs(dst, mat_vec_rn(p.view, c[0], c[4], c[8], w));
-                    __stcs(dst + 4, mat_vec_rn(p.view_proj, c[0], c[4], c[8], w));
+                    __stcs(dst, mat_vec_rn(view, c[0], c[4], c[8], w));
+                    __stcs(dst + 4, mat_vec_rn(view_proj, c[0], c[4], c[8], w));
                 }
             }
         }
@@ -172,7 +192,8 @@ cull_bake_kernel(const float4* __restrict__ rows_xyz, const float* __restrict__ 
             bool inside = true;
 #pragma unroll
             for (int pl = 0; pl < 5; ++pl) {
-                const float d = add_rn(add_rn(add_rn(mul_rn(p.frustum[pl][0], sp.x), mul_rn(p.frustum[pl][1], sp.y)), mul_rn(p.frustum[pl][2], sp.z)), p.frustum[pl][3]);
+                const float* f = frustum + 4 * pl;
+                const float d = add_rn(add_rn(add_rn(mul_rn(f[0], sp.x), mul_rn(f[1], sp.y)), mul_rn(f[2], sp.z)), f[3]);
                 inside = inside && (d >= neg_radius);
             }
             const uint32_t word = __ballot_sync(0xFFFFFFFFu, base + lane < p.object_count && ((live >> lane) & 1u) && inside);
@@ -335,7 +356,7 @@ __global__ void __launch_bounds__(CP_THREADS) exchange_expand_kernel(const __gri
 
 }  // namespace
 
-int r3_launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode) {
+static int launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode, const r3_camera_header* d_header) {
     const uint32_t n = cam->header.object_count;
     const bool bake = mode & R3_CB_BAKE, cull = mode & R3_CB_CULL;
     if (n == 0 || (!bake && !cull)) {
@@ -367,7 +388,19 @@ int r3_launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode) {
     cull_bake_kernel<B, C, L><<<n_ctas, CB_THREADS, 0, c->stream>>>(c->d_hot_xyz, reinterpret_cast<const float*>(c->d_hot_w), c->d_affine_bits, c->d_hot_sphere, \
                                                                     c->d_enabled_bits, c->d_live_bits, mats, words, cta_counts, p)
     r3_stage_begin(c, R3_STAGE_CULL_BAKE);
-    if (bake && cull) { if (live) R3_CB_LAUNCH(true, true, true); else R3_CB_LAUNCH(true, true, false); }
+    if (d_header) {
+        // without a live mask the kernel's `live` word is the enabled word, so the LIVE instantiations read the enabled bits instead
+        const DeviceCameraParams dp{d_header, n};
+        const uint32_t* live_bits = live ? c->d_live_bits : c->d_enabled_bits;
+#define R3_CB_DEV_LAUNCH(B, C)                                                                                                                       \
+    cull_bake_kernel<B, C, C, DeviceCameraParams><<<n_ctas, CB_THREADS, 0, c->stream>>>(c->d_hot_xyz, reinterpret_cast<const float*>(c->d_hot_w),     \
+                                                                                      c->d_affine_bits, c->d_hot_sphere, c->d_enabled_bits, live_bits, \
+                                                                                      mats, words, cta_counts, dp)
+        if (bake && cull) R3_CB_DEV_LAUNCH(true, true);
+        else if (bake) R3_CB_DEV_LAUNCH(true, false);
+        else R3_CB_DEV_LAUNCH(false, true);
+#undef R3_CB_DEV_LAUNCH
+    } else if (bake && cull) { if (live) R3_CB_LAUNCH(true, true, true); else R3_CB_LAUNCH(true, true, false); }
     else if (bake) R3_CB_LAUNCH(true, false, false);
     else { if (live) R3_CB_LAUNCH(false, true, true); else R3_CB_LAUNCH(false, true, false); }
 #undef R3_CB_LAUNCH
@@ -401,6 +434,11 @@ int r3_launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode) {
         R3_CHECK_LAUNCH(c, "compact_visible_kernel");
     }
     return R3_OK;
+}
+
+int r3_launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode) { return launch_cull_bake(c, cam, mode, nullptr); }
+int r3_launch_cull_bake_device_camera(r3_ctx* c, r3_camera* cam, uint32_t mode, const r3_camera_header* d_header) {
+    return launch_cull_bake(c, cam, mode, d_header);
 }
 
 uint64_t r3_hot_capacity(uint64_t want) {

@@ -1,0 +1,229 @@
+// r3_lights.cu — DirectionalLightManager::evaluate (rend3/src/managers/directional.rs:99-157) on the device: every directional light's
+// texel-snapped orthographic shadow camera around the viewer (directional/shadow_camera.rs:6-33), so that a frame whose camera moves needs
+// no light upload.  The arithmetic is rule R13 (DESIGN.md §2): one IEEE f32 operation at a time in the order written, never contracted
+// (this unit is compiled with -fmad=false and every operation is an explicit _rn intrinsic).
+//
+//   r3_set_directional_light_sources  blocking: static light fields into the light buffer (through r3_set_directional_lights, which also
+//                                     allocates the atlas), the sources into device memory
+//   r3_evaluate_shadow_cameras        one thread per light writes the light's view_proj and its camera header (view, view_proj, frustum)
+//   r3_shadow_uniform_upload          the cull + bake of Shadow(i) reading that header on the device
+//   r3_readback_shadow_cameras        blocking readback of the headers and light records
+#include <cmath>
+#include <cstring>
+
+#include "r3_common.cuh"
+
+namespace {
+
+struct v3 { float x, y, z; };
+
+__device__ __forceinline__ v3 sub3(v3 a, v3 b) { return {sub_rn(a.x, b.x), sub_rn(a.y, b.y), sub_rn(a.z, b.z)}; }
+__device__ __forceinline__ v3 add3(v3 a, v3 b) { return {add_rn(a.x, b.x), add_rn(a.y, b.y), add_rn(a.z, b.z)}; }
+// glam's scalar dot: (x x' + y y') + z z'
+__device__ __forceinline__ float dot3(v3 a, v3 b) { return add_rn(add_rn(mul_rn(a.x, b.x), mul_rn(a.y, b.y)), mul_rn(a.z, b.z)); }
+// glam.py::cross: (a.y b.z - b.y a.z, a.z b.x - b.z a.x, a.x b.y - b.x a.y)
+__device__ __forceinline__ v3 cross3(v3 a, v3 b) {
+    return {sub_rn(mul_rn(a.y, b.z), mul_rn(b.y, a.z)), sub_rn(mul_rn(a.z, b.x), mul_rn(b.z, a.x)), sub_rn(mul_rn(a.x, b.y), mul_rn(b.x, a.y))};
+}
+// normalize = v * (1 / sqrt(dot3))
+__device__ __forceinline__ v3 normalize3(v3 a) {
+    const float r = div_rn(1.0f, __fsqrt_rn(dot3(a, a)));
+    return {mul_rn(a.x, r), mul_rn(a.y, r), mul_rn(a.z, r)};
+}
+
+// glam.py::look_to_lh into m[16] (column-major)
+__device__ void look_to_lh(v3 eye, v3 dir, float* m) {
+    const v3 up = {0.0f, 1.0f, 0.0f};
+    const v3 f = normalize3(dir);
+    const v3 s = normalize3(cross3(up, f));
+    const v3 u = cross3(f, s);
+    m[0] = s.x; m[1] = u.x; m[2] = f.x; m[3] = 0.0f;
+    m[4] = s.y; m[5] = u.y; m[6] = f.y; m[7] = 0.0f;
+    m[8] = s.z; m[9] = u.z; m[10] = f.z; m[11] = 0.0f;
+    m[12] = -dot3(eye, s); m[13] = -dot3(eye, u); m[14] = -dot3(eye, f); m[15] = 1.0f;
+}
+// look_at_lh(eye, center) = look_to_lh(eye, center - eye); look_at_rh(eye, center) = look_to_lh(eye, eye - center)
+__device__ void look_at(v3 eye, v3 center, bool lh, float* m) { look_to_lh(eye, lh ? sub3(center, eye) : sub3(eye, center), m); }
+
+// transform_point3: ((x_axis px + y_axis py) + z_axis pz) + w_axis
+__device__ __forceinline__ v3 transform_point3(const float* m, v3 p) {
+    float r[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) r[k] = add_rn(add_rn(add_rn(mul_rn(m[k], p.x), mul_rn(m[4 + k], p.y)), mul_rn(m[8 + k], p.z)), m[12 + k]);
+    return {r[0], r[1], r[2]};
+}
+
+// Mat4::inverse: the GLM cofactor expansion glam's SSE2 build uses.  m[4 c + r] = column c, row r.  Coefficients a*b - c*d; the
+// cofactor columns ((v1 f0 - v2 f1) + v3 f2) times the sign vectors; det = SSE2 dot4 of column 0 with the first cofactor row,
+// (d.x + d.z) + (d.y + d.w); every element times (1 / det).
+__device__ void inverse4(const float* m, float* out) {
+#define M(c, r) m[4 * (c) + (r)]
+#define COEF(a, b, c, d) sub_rn(mul_rn(a, b), mul_rn(c, d))
+    float fac[6][4];
+    const int rr[6][2] = {{2, 3}, {1, 3}, {1, 2}, {0, 3}, {0, 2}, {0, 1}};   // (row i, row j) of Fac0..Fac5
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+        const int i = rr[k][0], j = rr[k][1];
+        const float c0 = COEF(M(2, i), M(3, j), M(3, i), M(2, j));
+        const float c2 = COEF(M(1, i), M(3, j), M(3, i), M(1, j));
+        const float c3 = COEF(M(1, i), M(2, j), M(2, i), M(1, j));
+        fac[k][0] = c0; fac[k][1] = c0; fac[k][2] = c2; fac[k][3] = c3;
+    }
+    float vec[4][4];   // vec[r] = (m[1][r], m[0][r], m[0][r], m[0][r])
+#pragma unroll
+    for (int r = 0; r < 4; ++r) { vec[r][0] = M(1, r); vec[r][1] = M(0, r); vec[r][2] = M(0, r); vec[r][3] = M(0, r); }
+    // inv_c = (vec[a] fac[p] - vec[b] fac[q]) + vec[e] fac[t]
+    const int terms[4][6] = {{1, 0, 2, 1, 3, 2}, {0, 0, 2, 3, 3, 4}, {0, 1, 1, 3, 3, 5}, {0, 2, 1, 4, 2, 5}};
+    const float sign_a[4] = {1.0f, -1.0f, 1.0f, -1.0f}, sign_b[4] = {-1.0f, 1.0f, -1.0f, 1.0f};
+    float inv[16];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const int* t = terms[c];
+        const float* sg = (c & 1) ? sign_b : sign_a;
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            inv[4 * c + k] = mul_rn(add_rn(sub_rn(mul_rn(vec[t[0]][k], fac[t[1]][k]), mul_rn(vec[t[2]][k], fac[t[3]][k])), mul_rn(vec[t[4]][k], fac[t[5]][k])), sg[k]);
+    }
+    const float d0 = mul_rn(M(0, 0), inv[0]), d1 = mul_rn(M(0, 1), inv[4]), d2 = mul_rn(M(0, 2), inv[8]), d3 = mul_rn(M(0, 3), inv[12]);
+    const float rcp = div_rn(1.0f, add_rn(add_rn(d0, d2), add_rn(d1, d3)));
+#pragma unroll
+    for (int k = 0; k < 16; ++k) out[k] = mul_rn(inv[k], rcp);
+#undef COEF
+#undef M
+}
+
+// one thread per light: R13
+__global__ void __launch_bounds__(64) shadow_camera_kernel(const r3_directional_light_source* __restrict__ src, uint32_t n, uint32_t left_handed,
+                                                            float lx, float ly, float lz, r3_directional_light* __restrict__ lights,
+                                                            r3_camera_header* __restrict__ cams) {
+    const uint32_t i = threadIdx.x;
+    if (i >= n) return;
+    const r3_directional_light_source s = src[i];
+    const bool lh = left_handed != 0;
+    const v3 dir = {s.direction[0], s.direction[1], s.direction[2]}, zero = {0.0f, 0.0f, 0.0f}, loc = {lx, ly, lz};
+    const float texel = div_rn(s.distance, (float)s.resolution);
+    float origin_view[16], inv[16], view[16], vp[16];
+    look_at(zero, dir, lh, origin_view);
+    const v3 cov = transform_point3(origin_view, loc);
+    // Rust's f32 % (fmodf): exact, with the sign of the dividend
+    const v3 shadow_loc = {sub_rn(cov.x, fmodf(cov.x, texel)), sub_rn(cov.y, fmodf(cov.y, texel)), sub_rn(cov.z, 0.0f)};
+    inverse4(origin_view, inv);
+    const v3 new_loc = transform_point3(inv, shadow_loc);
+    look_at(new_loc, add3(new_loc, dir), lh, view);
+    // orthographic_{lh,rh}(-h, h, -h, h, h, -h), h = distance * 0.5 (camera.rs:90-96)
+    const float half = mul_rn(s.distance, 0.5f), left = -half, right = half, bottom = -half, top = half, near = half, far = -half;
+    const float rcp_w = div_rn(1.0f, sub_rn(right, left)), rcp_h = div_rn(1.0f, sub_rn(top, bottom));
+    const float r = div_rn(1.0f, lh ? sub_rn(far, near) : sub_rn(near, far));
+    float proj[16] = {add_rn(rcp_w, rcp_w), 0.0f, 0.0f, 0.0f, 0.0f, add_rn(rcp_h, rcp_h), 0.0f, 0.0f, 0.0f, 0.0f, r, 0.0f,
+                      mul_rn(-add_rn(left, right), rcp_w), mul_rn(-add_rn(top, bottom), rcp_h), lh ? mul_rn(-r, near) : mul_rn(r, near), 1.0f};
+    // view_proj = proj * view: column j = ((p0 v.x + p1 v.y) + p2 v.z) + p3 v.w
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float4 col = mat_vec_rn(proj, view[4 * j], view[4 * j + 1], view[4 * j + 2], view[4 * j + 3]);
+        vp[4 * j] = col.x; vp[4 * j + 1] = col.y; vp[4 * j + 2] = col.z; vp[4 * j + 3] = col.w;
+    }
+    r3_camera_header h;
+    memset(&h, 0, sizeof h);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) { h.view[k] = view[k]; h.view_proj[k] = vp[k]; lights[i].view_proj[k] = vp[k]; }
+    // Frustum::from_matrix (util/frustum.rs:96-145): left = r3 + r0, right = r3 - r0, top = r3 - r1, bottom = r3 + r1, near = r3 - r2,
+    // each divided by |abc|
+    const int row[5] = {0, 0, 1, 1, 2};
+    const bool plus[5] = {true, false, false, true, false};
+#pragma unroll
+    for (int pl = 0; pl < 5; ++pl) {
+        float q[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) q[c] = plus[pl] ? add_rn(vp[4 * c + 3], vp[4 * c + row[pl]]) : sub_rn(vp[4 * c + 3], vp[4 * c + row[pl]]);
+        const float mag = __fsqrt_rn(dot3({q[0], q[1], q[2]}, {q[0], q[1], q[2]}));
+#pragma unroll
+        for (int c = 0; c < 4; ++c) h.frustum[pl][c] = div_rn(q[c], mag);
+    }
+    h.shadow_index = i;
+    h.resolution[0] = (float)s.size; h.resolution[1] = (float)s.size;
+    h.flags = lh ? R3_PCU_POSITIVE_AREA_VISIBLE : 0u;   // TriangleVisibility::from_winding_and_face: Cw (Left) + Front culled
+    cams[i] = h;
+}
+
+}  // namespace
+
+R3_EXPORT int r3_set_directional_light_sources(r3_ctx* c, const r3_directional_light_source* lights, uint32_t n, uint32_t aw, uint32_t ah,
+                                               uint32_t left_handed) {
+    if (!c) return R3_E_INVALID;
+    if (!lights && n) return r3_fail(c, R3_E_INVALID, "set_directional_light_sources: null lights");
+    if (n > R3_MAX_SHADOWS) return r3_fail(c, R3_E_INVALID, "set_directional_light_sources: more lights than R3_MAX_SHADOWS");
+    for (uint32_t i = 0; i < n; ++i) {
+        const r3_directional_light_source& s = lights[i];
+        if (s.size == 0 || (uint64_t)s.offset[0] + s.size > aw || (uint64_t)s.offset[1] + s.size > ah)
+            return r3_fail(c, R3_E_INVALID, "set_directional_light_sources: empty map or placement outside the atlas");
+    }
+    cudaSetDevice(c->device);
+    if (!c->d_light_src) R3_CUDA(c, cudaMalloc((void**)&c->d_light_src, R3_MAX_SHADOWS * sizeof(r3_directional_light_source)));
+    if (!c->d_shadow_cams) R3_CUDA(c, cudaMalloc((void**)&c->d_shadow_cams, R3_MAX_SHADOWS * sizeof(r3_camera_header)));
+    // the static fields as directional.rs:135-156 writes them; view_proj stays 0 until the first evaluation
+    std::vector<uint8_t> bytes(16 + (size_t)n * sizeof(r3_directional_light), 0);
+    *reinterpret_cast<uint32_t*>(bytes.data()) = n;
+    r3_directional_light* dl = reinterpret_cast<r3_directional_light*>(bytes.data() + 16);
+    const float w = (float)aw, h = (float)ah;
+    for (uint32_t i = 0; i < n; ++i) {
+        const r3_directional_light_source& s = lights[i];
+        for (int k = 0; k < 3; ++k) { dl[i].color[k] = s.color[k] * s.intensity; dl[i].direction[k] = s.direction[k]; }
+        dl[i].inv_resolution[0] = 1.0f / w; dl[i].inv_resolution[1] = 1.0f / h;
+        dl[i].atlas_offset[0] = (float)s.offset[0] / w; dl[i].atlas_offset[1] = (float)s.offset[1] / h;
+        dl[i].atlas_size[0] = (float)s.size / w; dl[i].atlas_size[1] = (float)s.size / h;
+    }
+    if (n) R3_CUDA(c, cudaMemcpyAsync(c->d_light_src, lights, (size_t)n * sizeof(r3_directional_light_source), cudaMemcpyHostToDevice, c->stream));
+    R3_TRY(r3_set_directional_lights(c, bytes.data(), bytes.size(), aw, ah));   // drains the stream: `lights` is only borrowed
+    c->light_src.assign(lights, lights + n);
+    c->light_src_left_handed = left_handed ? 1u : 0u;
+    c->light_src_set = true;
+    c->shadow_cams_evaluated = false;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_evaluate_shadow_cameras(r3_ctx* c, const float loc[3]) {
+    if (!c) return R3_E_INVALID;
+    if (!loc) return r3_fail(c, R3_E_INVALID, "evaluate_shadow_cameras: null location");
+    if (!c->light_src_set) return r3_fail(c, R3_E_STATE, "evaluate_shadow_cameras before set_directional_light_sources");
+    cudaSetDevice(c->device);
+    const uint32_t n = (uint32_t)c->light_src.size();
+    if (n) {
+        shadow_camera_kernel<<<1, 64, 0, c->stream>>>(c->d_light_src, n, c->light_src_left_handed, loc[0], loc[1], loc[2], c->d_dir, c->d_shadow_cams);
+        R3_CHECK_LAUNCH(c, "shadow_camera_kernel");
+    }
+    c->shadow_cams_evaluated = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_shadow_uniform_upload(r3_ctx* c, uint32_t shadow_index, uint32_t object_count, uint32_t mode) {
+    if (!c) return R3_E_INVALID;
+    if (!c->light_src_set || !c->shadow_cams_evaluated) return r3_fail(c, R3_E_STATE, "shadow_uniform_upload before set_directional_light_sources + evaluate_shadow_cameras");
+    if (shadow_index >= c->light_src.size()) return r3_fail(c, R3_E_INVALID, "shadow_uniform_upload: no such light");
+    if (object_count > c->n_slots) return r3_fail(c, R3_E_INVALID, "object_count exceeds the object buffer");
+    cudaSetDevice(c->device);
+    r3_camera* cam = &c->cams[r3_cam_slot(shadow_index)];
+    // the fields the host knows; view, view_proj and frustum stay on the device (the triangle cull reads none of them)
+    r3_camera_header h;
+    memset(&h, 0, sizeof h);
+    const float size = (float)c->light_src[shadow_index].size;
+    h.shadow_index = shadow_index;
+    h.resolution[0] = size; h.resolution[1] = size;
+    h.flags = c->light_src_left_handed ? R3_PCU_POSITIVE_AREA_VISIBLE : 0u;
+    h.object_count = object_count;
+    cam->header = h;
+    cam->header_set = true;
+    R3_TRY(r3_camera_buffers(c, cam, mode));
+    return r3_launch_cull_bake_device_camera(c, cam, mode, c->d_shadow_cams + shadow_index);
+}
+
+R3_EXPORT int r3_readback_shadow_cameras(r3_ctx* c, r3_camera_header* out, r3_directional_light* lights, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (!out && n) return r3_fail(c, R3_E_INVALID, "readback_shadow_cameras: null");
+    if (!c->light_src_set || !c->shadow_cams_evaluated) return r3_fail(c, R3_E_STATE, "readback_shadow_cameras before evaluate_shadow_cameras");
+    if (n > c->light_src.size()) return r3_fail(c, R3_E_INVALID, "readback_shadow_cameras: more cameras than lights");
+    cudaSetDevice(c->device);
+    if (n) R3_CUDA(c, cudaMemcpyAsync(out, c->d_shadow_cams, (size_t)n * sizeof *out, cudaMemcpyDeviceToHost, c->stream));
+    if (n && lights) R3_CUDA(c, cudaMemcpyAsync(lights, c->d_dir, (size_t)n * sizeof *lights, cudaMemcpyDeviceToHost, c->stream));
+    R3_CUDA(c, r3_stream_sync(c));
+    return R3_OK;
+}

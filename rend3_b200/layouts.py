@@ -135,6 +135,20 @@ DIRECTIONAL_LIGHT_DTYPE = _dt(
 
 POINT_LIGHT_DTYPE = _dt([("position", (f4, 4), 0), ("color", (f4, 3), 16), ("radius", f4, 28)], 32)
 
+# r3_directional_light_source: a DirectionalLight plus its atlas placement (r3_set_directional_light_sources)
+LIGHT_SOURCE_DTYPE = _dt(
+    [
+        ("color", (f4, 3), 0),
+        ("intensity", f4, 12),
+        ("direction", (f4, 3), 16),
+        ("distance", f4, 28),
+        ("resolution", u4, 32),
+        ("offset", (u4, 2), 36),
+        ("size", u4, 44),
+    ],
+    48,
+)
+
 MATERIAL_DTYPE = _dt(
     [
         ("textures", (u4, 10), 0),

@@ -109,8 +109,9 @@ class BaseRenderGraph:
         self.gpu_culler = GpuCuller(backend, max_compute_workgroups_per_dimension)
         self._resolution: Optional[Tuple[int, int]] = None
 
-    def upload_world(self, ev: EvalOutput):
-        """What evaluate_instructions leaves in wgpu buffers (renderer/eval.rs:157-181)."""
+    def upload_world(self, ev: EvalOutput, device_shadow_cameras: bool = False):
+        """What evaluate_instructions leaves in wgpu buffers (renderer/eval.rs:157-181).  With `device_shadow_cameras` the lights go up
+        as sources and atlas placements; the frame evaluates their shadow cameras on the device."""
         b = self.backend
         b.set_objects(ev.object_buffer)
         flags = (ev.object_live & 1) | ((ev.object_atomic & 1) << 1) | ((ev.object_back_to_front & 1) << 2)
@@ -120,14 +121,17 @@ class BaseRenderGraph:
         b.set_textures(ev.texture_descs, ev.texture_texels)
         b.set_skybox(ev.skybox_desc, ev.skybox_texels)
         b.set_materials(ev.material_buffer)
-        b.set_directional_lights(ev.directional_buffer, ev.shadow_target_size[0], ev.shadow_target_size[1])
+        if device_shadow_cameras:
+            b.set_directional_light_sources(ev.directional_sources, ev.shadow_target_size[0], ev.shadow_target_size[1], ev.camera.handedness == LEFT)
+        else:
+            b.set_directional_lights(ev.directional_buffer, ev.shadow_target_size[0], ev.shadow_target_size[1])
         b.set_point_lights(ev.point_buffer)
 
     def add_to_graph(self, ev: EvalOutput, resolution: Tuple[int, int], samples: int = 1,
                      settings: BaseRenderGraphSettings = BaseRenderGraphSettings(), srgb_target: bool = True,
                      upload: bool = True, scissor_rows: Optional[Tuple[int, int]] = None, shadow_filter=None, after_shadows=None,
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
-                     posed_skinning: bool = False, posed_objects: bool = False):
+                     posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -141,13 +145,15 @@ class BaseRenderGraph:
         records and joint buffer (r3_pose_skeletons + r3_skin_posed after r3_set_animations / r3_set_skeletons / r3_set_pose_jobs):
         only enqueued work, so the frame stays one graph.  `posed_objects` poses the animated nodes' objects on the device first
         (r3_pose_objects after r3_set_object_animations / r3_set_object_pose_jobs): their transforms, world spheres and sort locations
-        are written before any camera culls, also enqueue only."""
+        are written before any camera culls, also enqueue only.  `device_shadow_cameras` uploads the lights as sources
+        (r3_set_directional_light_sources) and evaluates their shadow cameras on the device around this frame's camera
+        (r3_evaluate_shadow_cameras, r3_shadow_uniform_upload): a frame whose camera moves needs no light upload."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
         b, culler = self.backend, self.gpu_culler
         if upload:
-            self.upload_world(ev)
+            self.upload_world(ev, device_shadow_cameras)
         if self._resolution != (resolution, samples, tuple(settings.clear_color)):
             b.set_render_target(resolution[0], resolution[1], samples, settings.clear_color)
             self._resolution = (resolution, samples, tuple(settings.clear_color))
@@ -164,6 +170,8 @@ class BaseRenderGraph:
                 if shadow_filter(i):
                     b.clear_shadow_rect(s.offset[0], s.offset[1], s.size, s.size)
         b.set_frame_uniforms(frame_uniforms(ev.camera, settings.ambient_color, resolution))  # :142
+        if device_shadow_cameras:                                                 # DirectionalLightManager::evaluate around this camera
+            b.evaluate_shadow_cameras(ev.camera.location())
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
         if posed_objects:                                                         # :145 pose_animation_frame's set_object_transform half
@@ -173,7 +181,10 @@ class BaseRenderGraph:
             b.skin_posed()
         mine = [(i, s) for i, s in enumerate(ev.shadows) if shadow_filter is None or shadow_filter(i)]
         for i, s in mine:                                                         # :148
-            culler.object_uniform_upload(ev, s.camera, i, (s.size, s.size), 1)
+            if device_shadow_cameras:
+                b.shadow_uniform_upload(i, len(ev.object_buffer))
+            else:
+                culler.object_uniform_upload(ev, s.camera, i, (s.size, s.size), 1)
         for i, s in mine:                                                         # :150
             culler.cull(ev, i)
         for i, s in mine:                                                         # :153

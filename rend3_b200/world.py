@@ -52,6 +52,7 @@ from .layouts import (
     MATERIAL_DTYPE,
     OBJECT_DTYPE,
     DIRECTIONAL_LIGHT_DTYPE,
+    LIGHT_SOURCE_DTYPE,
     POINT_LIGHT_DTYPE,
 )
 
@@ -535,6 +536,9 @@ class EvalOutput:
     camera: CameraState
     skybox_desc: Optional[np.ndarray] = None    # TEXTURE_DESC_DTYPE scalar (width = face size), None = no skybox
     skybox_texels: Optional[np.ndarray] = None  # six faces (+X -X +Y -Y +Z -Z), each with its mip chain
+    # the lights behind directional_buffer, in its order, with their atlas placements (LIGHT_SOURCE_DTYPE): what
+    # r3_set_directional_light_sources takes so that the device evaluates the shadow cameras around each frame's camera
+    directional_sources: Optional[np.ndarray] = None
 
 
 class Renderer:
@@ -731,13 +735,16 @@ class Renderer:
         shadows: List[ShadowDesc] = []
         size = (MINIMUM_SHADOW_MAP_SIZE, MINIMUM_SHADOW_MAP_SIZE)
         dl = np.zeros(0, dtype=DIRECTIONAL_LIGHT_DTYPE)
+        src = np.zeros(0, dtype=LIGHT_SOURCE_DTYPE)
         if atlas is not None:
             dims, maps = atlas
             size = (max(dims[0], MINIMUM_SHADOW_MAP_SIZE), max(dims[1], MINIMUM_SHADOW_MAP_SIZE))
             size_f = np.array(size, dtype=f32)
             dl = np.zeros(len(maps), dtype=DIRECTIONAL_LIGHT_DTYPE)
+            src = np.zeros(len(maps), dtype=LIGHT_SOURCE_DTYPE)
             for k, (ox, oy, sz, handle) in enumerate(maps):
                 light = self.dir_lights[handle]
+                src[k] = (light.color, light.intensity, light.direction, light.distance, light.resolution, (ox, oy), sz)
                 cam = shadow_camera(light, self.camera)
                 shadows.append(ShadowDesc((ox, oy), sz, handle, cam))
                 dl[k]["view_proj"] = cam.view_proj.reshape(16)
@@ -772,6 +779,7 @@ class Renderer:
             skybox_desc=sky_desc,
             skybox_texels=sky_blob,
             directional_buffer=dbytes,
+            directional_sources=src,
             point_buffer=pbytes,
             shadows=shadows,
             shadow_target_size=size,
