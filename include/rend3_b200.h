@@ -20,7 +20,8 @@
  *   - one context per GPU; calls on a context must be externally serialised (this is the
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
- *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_evaluate_shadow_cameras, r3_shadow_uniform_upload,
+ *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_evaluate_shadow_cameras,
+ *     r3_shadow_uniform_upload,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
@@ -28,7 +29,8 @@
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
  *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices, r3_set_object_animations,
- *     r3_set_object_pose_jobs, r3_set_directional_light_sources, r3_readback_shadow_cameras —
+ *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_directional_light_sources,
+ *     r3_readback_shadow_cameras —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
  *     has to grow (first frame, larger world, new resolution) is reallocated with a stream synchronisation as well.
@@ -118,6 +120,34 @@ int r3_update_object_sort_info(r3_ctx*, const uint32_t* slots, const uint64_t* m
  * r3_set_objects + r3_set_object_sort_info of the old contents followed by zeros.  R3_E_STATE while the records are borrowed
  * (r3_set_objects_device) or a visible-set exchange / peer plumbing is connected (their buffers are sized at creation). */
 int r3_resize_objects(r3_ctx*, uint32_t n_slots);
+/* Objects that move: Renderer::set_object_transform (object.rs:302-316) for n objects in one kernel, from host or device memory.
+ *   r3_set_object_mesh_spheres       InternalObject::mesh_bounding_sphere (object.rs:268-270) per slot, (centre, radius): what
+ *                                    set_object_transform moves to world space.  slots == NULL: spheres for slots 0 .. n-1 (replaces the
+ *                                    array); otherwise entry i sets slot slots[i], each below the current sphere count and named once
+ *                                    (R3_E_INVALID otherwise, nothing written).  Blocking.  The spheres belong to the mesh, not the record:
+ *                                    r3_set_objects keeps them, r3_resize_objects grows them with zero spheres like the sort info.
+ *   r3_set_object_transforms         transform = mat4s[i] (column-major), bounding sphere = mesh sphere.apply_transform
+ *                                    (util/frustum.rs:22-32), sort location = transform_point3a(ZERO).  Arithmetic: rule R12 (DESIGN.md §2).
+ *                                    slots == NULL: slots 0 .. n-1 (the dense form, n <= the slot count).  Host pointers, blocking: they are
+ *                                    copied to the device, one kernel runs and the stream is drained once.
+ *   r3_set_object_transforms_device  the same from DEVICE memory, enqueue only: the pointers (matrices 16-byte aligned) are read by the
+ *                                    kernel when it runs on the context's stream.  Legal between r3_frame_begin and r3_frame_end; in a
+ *                                    frame graph the kernel's arguments are updated in place.  Whatever produces the buffers must be
+ *                                    ordered before the call on that stream (r3_get_stream: enqueue the producer there, or make the
+ *                                    stream wait on an event before r3_frame_begin), and they must stay valid until the frame has run.
+ * Only float4 #0-4 of the record change (transform, sphere); `enabled`, the cold fields, key and flags are untouched, exactly as in
+ * r3_pose_objects.  The same kernel writes the cull + bake's dense copies of those slots (rows, row 3, spheres, the affine bit) and, when
+ * sort info is set, their sort locations; a new frame epoch starts, as after a pose.  The host batching's mirror of the locations is
+ * refreshed in the drain it makes anyway for the visible list; the device batching path gets no new drain.
+ * Slots must be distinct (two entries' stores would land in an unspecified order).  The host form checks this, and that every slot is
+ * below the current slot count, before anything is written: R3_E_INVALID, context unchanged.  The device form cannot look: out-of-range
+ * slots are dropped (ScatterCopy's robust access, as in r3_update_objects), distinctness is a precondition.
+ * R3_E_STATE: before r3_set_objects; while the mesh spheres cover fewer slots than the object buffer (never set, or r3_set_objects made
+ * the world larger than they are); while the object buffer is borrowed (r3_set_objects_device).  n == 0 is R3_OK and enqueues nothing.
+ * A slot that r3_pose_objects also poses takes whichever of the two calls is enqueued later. */
+int r3_set_object_mesh_spheres(r3_ctx*, const uint32_t* slots_or_null, const float* center_radius /* n x 4 */, uint32_t n);
+int r3_set_object_transforms(r3_ctx*, const uint32_t* slots_or_null, const float* mat4s /* n x 16, column-major */, uint32_t n);
+int r3_set_object_transforms_device(r3_ctx*, const uint32_t* d_slots_or_null, const float* d_mat4s, uint32_t n);
 int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);               /* eval_output.mesh_buffer (mesh.rs:99) */
 /* MeshManager::add (mesh.rs:123-184): write nbytes at byte_offset of the megabuffer (both multiples of 4).  A write past the end extends it;
  * words between the old end and byte_offset read 0.  The allocation grows to the next power of two, keeping its contents (also what

@@ -75,6 +75,11 @@ struct EvalOutput {
     // pose the animated nodes' objects on the device (r3_set_object_animations / r3_set_object_pose_jobs made before the frame):
     // transforms, world spheres and sort locations, written at the skinning node before any camera culls; only enqueues work
     bool posed_objects = false;
+    // InternalObject::mesh_bounding_sphere per slot, (centre, radius) x n_slots (null = not uploaded: no object can be moved)
+    const float* mesh_spheres = nullptr;
+    // objects the application moved this frame (Renderer::set_object_transform in bulk): matrices (and slots, null = slots 0 .. n-1)
+    // in DEVICE memory, their producer ordered on the context's stream; applied at the skinning node before posed_objects, enqueue only
+    const uint32_t* d_moved_slots = nullptr; const float* d_moved_transforms = nullptr; uint32_t n_moved = 0;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -100,6 +105,7 @@ public:
     void upload_world(const EvalOutput& ev, bool device_shadow_cameras = false) {
         check(r3_set_objects(ctx_, ev.objects, ev.n_slots));
         if (ev.material_key) check(r3_set_object_sort_info(ctx_, ev.material_key, ev.sort_flags, ev.location, ev.n_slots));
+        if (ev.mesh_spheres) check(r3_set_object_mesh_spheres(ctx_, nullptr, ev.mesh_spheres, ev.n_slots));
         check(r3_set_mesh_buffer(ctx_, ev.mesh_buffer, ev.mesh_bytes));
         check(r3_set_textures(ctx_, ev.textures, ev.n_textures, ev.texels, ev.texel_bytes));
         check(r3_set_skybox(ctx_, ev.skybox, ev.skybox_texels, ev.skybox_bytes));
@@ -111,6 +117,8 @@ public:
             check(r3_set_directional_lights(ctx_, ev.directional_lights, ev.directional_bytes, ev.shadow_target_size[0], ev.shadow_target_size[1]));
         check(r3_set_point_lights(ctx_, ev.point_lights, ev.point_bytes));
     }
+    // Renderer::set_object_transform (object.rs:302-316) for n objects from host memory (slots == nullptr: slots 0 .. n-1); blocking
+    void set_object_transforms(const uint32_t* slots, const float* mat4s, uint32_t n) { check(r3_set_object_transforms(ctx_, slots, mat4s, n)); }
     void sync() { check(r3_sync(ctx_)); }
 
 private:
@@ -134,6 +142,7 @@ class GpuSkinner {   // skinning.rs:54-199: add_skinning_to_graph — skinned po
 public:
     void add_skinning_to_graph(Renderer& r, const EvalOutput& ev) const {
         if (ev.n_skeletons) r.check(r3_skin(r.raw(), ev.skinning_inputs, ev.n_skeletons, ev.joint_matrices, ev.n_joints));
+        if (ev.n_moved) r.check(r3_set_object_transforms_device(r.raw(), ev.d_moved_slots, ev.d_moved_transforms, ev.n_moved));
         if (ev.posed_objects) r.check(r3_pose_objects(r.raw()));
         if (ev.posed_skinning) {
             r.check(r3_pose_skeletons(r.raw()));

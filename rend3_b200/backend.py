@@ -43,6 +43,7 @@ ENTRY_POINTS = [
     "update_object_sort_info", "resize_objects", "update_mesh_buffer", "update_textures",
     "set_animations", "set_skeletons", "set_pose_jobs", "pose_skeletons", "skin_posed", "readback_joint_matrices",
     "set_object_animations", "set_object_pose_jobs", "pose_objects", "readback_objects",
+    "set_object_mesh_spheres", "set_object_transforms", "set_object_transforms_device",
 ]
 
 
@@ -166,6 +167,35 @@ class Backend:
 
     def resize_objects(self, n_slots: int):
         self._call("resize_objects", C.c_uint32(n_slots))
+
+    # ---- objects that move (Renderer::set_object_transform in bulk)
+    def set_object_mesh_spheres(self, spheres, slots=None):
+        """(n, 4) mesh spheres (centre, radius) for slots 0 .. n-1, or for the listed slots."""
+        sp = np.ascontiguousarray(spheres, dtype=np.float32).reshape(-1, 4)
+        s = None if slots is None else np.ascontiguousarray(slots, dtype=np.uint32)
+        assert s is None or len(s) == len(sp)
+        self._call("set_object_mesh_spheres", _ptr(s), _ptr(sp) if len(sp) else None, C.c_uint32(len(sp)))
+
+    def set_object_transforms(self, matrices, slots=None):
+        """(n, 16) column-major matrices from host memory for slots 0 .. n-1, or for the listed slots.  Blocking."""
+        m = np.ascontiguousarray(matrices, dtype=np.float32).reshape(-1, 16)
+        s = None if slots is None else np.ascontiguousarray(slots, dtype=np.uint32)
+        assert s is None or len(s) == len(m)
+        self._call("set_object_transforms", _ptr(s), _ptr(m) if len(m) else None, C.c_uint32(len(m)))
+
+    def set_object_transforms_device(self, matrices, slots=None, n: Optional[int] = None):
+        """The same from device memory, enqueue only.  `matrices` / `slots` are CUDA tensors (contiguous float32 (n, 16) / int32 or uint32
+        (n,)) or raw device pointers with `n` given; the caller keeps them alive and orders their producer on stream()."""
+        def pointer(x, width):
+            if x is None or isinstance(x, int):
+                return x, None
+            assert x.is_cuda and x.is_contiguous() and x.element_size() == 4, "a contiguous CUDA tensor of 4-byte elements"
+            return x.data_ptr(), x.numel() // width
+        mp, mn = pointer(matrices, 16)
+        sp, sn = pointer(slots, 1)
+        n = mn if n is None else n
+        assert n is not None and (sn is None or sn == n)
+        self._call("set_object_transforms_device", C.c_void_p(sp), C.c_void_p(mp), C.c_uint32(n))
 
     def set_mesh_buffer(self, words: np.ndarray):
         words = np.ascontiguousarray(words, dtype=np.uint32)

@@ -45,11 +45,13 @@ int r3_host_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], uint
     const uint32_t cap = cam->header.object_count;
     if (c->sort_key.size() < cap) return r3_fail(c, R3_E_STATE, "batch_objects needs r3_set_object_sort_info");
     // visible list: the only device->host transfer of the frame (4 B per visible object), and with it the locations of the objects
-    // r3_pose_objects posed since the host mirror last took them (12 B per posed object), so that no extra drain is needed
+    // r3_pose_objects posed since the host mirror last took them (12 B per posed object) and, after r3_set_object_transforms / _device,
+    // every location (12 B per slot: the host does not know which slots a device list named), so that no extra drain is needed
     uint32_t nv = 0;
-    bool staged = false;
+    bool staged = false, moved = false;
+    R3_TRY(r3_stage_moved_locations(c, &moved));
     R3_TRY(r3_anim_stage_posed_locations(c, &staged));
-    if (cam->d_visible_count || staged) {
+    if (cam->d_visible_count || staged || moved) {
         if (cam->d_visible_count) R3_CUDA(c, cudaMemcpyAsync(&nv, cam->d_visible_count, 4, cudaMemcpyDeviceToHost, c->stream));
         R3_CUDA(c, r3_stream_sync(c));
     }

@@ -112,6 +112,9 @@ struct r3_ctx {
     std::vector<uint64_t> sort_key; std::vector<uint8_t> sort_flags; std::vector<float> sort_loc;
     uint32_t* d_live_bits = nullptr; uint32_t live_bits_cap = 0; bool have_live = false;
     uint8_t* d_sort_key8 = nullptr; float* d_sort_loc = nullptr; uint32_t sort_dev_cap = 0; bool gpu_batching_ok = false;
+    // InternalObject::mesh_bounding_sphere per slot (r3_set_object_mesh_spheres): what r3_set_object_transforms moves to world space
+    float4* d_mesh_spheres = nullptr; uint32_t n_mesh_spheres = 0, mesh_spheres_cap = 0;
+    bool locations_moved = false;             // r3_set_object_transforms* ran since c->sort_loc last took the device's locations
     uint32_t sort_live_blend = 0, sort_wide_keys = 0;   // live slots with material key 2 (any_blend), slots with a key >= 64 (host batching)
     // frame-wide sort shared by the cameras of one frame (r3_gpu_batching.cu)
     unsigned long long* d_gsort_keys[2] = {nullptr, nullptr}; uint64_t gsort_cap[2] = {0, 0}; uint32_t* d_gsort_hist = nullptr; uint64_t gsort_hist_cap = 0;
@@ -234,8 +237,15 @@ void r3_anim_destroy(r3_ctx* c);             // r3_animation.cu: frees c->anim (
 // locations to the host (*staged = true when it did); once the caller has drained the stream, apply writes them into c->sort_loc.
 int r3_anim_stage_posed_locations(r3_ctx* c, bool* staged);
 void r3_anim_apply_posed_locations(r3_ctx* c);
+// r3_object_transforms.cu: the same after r3_set_object_transforms / _device, whose moved slots the host may not know: stage enqueues a
+// copy of every location into c->sort_loc, complete once the caller has drained the stream
+int r3_stage_moved_locations(r3_ctx* c, bool* staged);
+int r3_grow_mesh_spheres(r3_ctx* c, uint32_t n);   // r3_resize_objects: zero spheres for the new slots, once spheres are set
 
 #ifdef __CUDACC__
+// Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine
+// (a product with -0.0 can carry its sign into MV / MVP).
+__device__ __forceinline__ uint32_t affine_w_bits(uint32_t j) { return j == 3 ? 0x3f800000u : 0u; }
 // IEEE, never-contracted arithmetic for the bit-exact stages (SURVEY D7)
 __device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }

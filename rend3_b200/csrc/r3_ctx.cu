@@ -79,7 +79,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     if (!c->objects_borrowed) cudaFree(c->d_objects);
     cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
     cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc); cudaFree(c->d_gsort_keys[0]); cudaFree(c->d_gsort_keys[1]); cudaFree(c->d_gsort_hist); cudaFree(c->d_gsort_header);
-    cudaFree(c->d_live_bits); cudaFree(c->d_mesh); cudaFree(c->d_materials); cudaFree(c->d_dir); cudaFree(c->d_point);
+    cudaFree(c->d_mesh_spheres); cudaFree(c->d_live_bits); cudaFree(c->d_mesh); cudaFree(c->d_materials); cudaFree(c->d_dir); cudaFree(c->d_point);
     cudaFree(c->d_light_mats); cudaFree(c->d_atlas); cudaFree(c->d_light_src); cudaFree(c->d_shadow_cams);
     for (auto& k : c->cams) {
         cudaFree(k.d_matrices); cudaFree(k.d_visible); cudaFree(k.d_visible_count); cudaFree(k.d_tile_state);
@@ -524,6 +524,7 @@ R3_EXPORT int r3_resize_objects(r3_ctx* c, uint32_t n) {
     if (n > c->objects_cap || !c->d_objects) R3_TRY(r3_reserve_t(c, &c->d_objects, &c->objects_cap, r3_hot_capacity(n), true));
     R3_CUDA(c, cudaMemsetAsync(c->d_objects + old_n, 0, (size_t)(n - old_n) * sizeof(r3_object), c->stream));
     R3_TRY(r3_grow_hot(c, old_n, n));
+    R3_TRY(r3_grow_mesh_spheres(c, n));
     c->n_slots = n;   // zero records have no triangles: the cached invocation bounds stay valid
     const size_t sorted = c->sort_key.size();
     if (c->have_live && sorted < n) {

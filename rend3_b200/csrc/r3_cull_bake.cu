@@ -62,10 +62,6 @@ struct DeviceCameraParams {
 };
 constexpr int CAM_FLOATS = 52;   // view[16] | view_proj[16] | frustum[5][4], staged in shared memory by DeviceCameraParams launches
 
-// Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine
-// (a product with -0.0 can carry its sign into MV / MVP).
-__device__ __forceinline__ uint32_t affine_w_bits(uint32_t j) { return j == 3 ? 0x3f800000u : 0u; }
-
 // AoS Object records -> the dense hot arrays.  8 lanes per 128-byte record (coalesced 512-byte loads); float4 #0-3 =
 // transform columns, #4 = bounding sphere, #7.y = `enabled` (byte 116).  Lane k < 4 holds column k and scatters it into
 // element k of rows 0-2 (rows_xyz) and of row 3 (rows_w).

@@ -54,6 +54,7 @@ int main(int argc, char** argv) {
         uint64_t n = 0;
         ev.objects = as<r3_object>(s, "objects", &n); ev.n_slots = (uint32_t)n;
         ev.material_key = as<uint64_t>(s, "material_key"); ev.sort_flags = as<uint8_t>(s, "sort_flags"); ev.location = as<float>(s, "location");
+        if (s.count("mesh_spheres")) ev.mesh_spheres = as<float>(s, "mesh_spheres");
         ev.mesh_buffer = as<uint8_t>(s, "mesh", &n); ev.mesh_bytes = n;
         ev.materials = as<r3_material>(s, "materials", &n); ev.n_materials = (uint32_t)n;
         ev.textures = as<r3_texture_desc>(s, "tex_descs", &n); ev.n_textures = (uint32_t)n;

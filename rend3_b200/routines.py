@@ -109,14 +109,18 @@ class BaseRenderGraph:
         self.gpu_culler = GpuCuller(backend, max_compute_workgroups_per_dimension)
         self._resolution: Optional[Tuple[int, int]] = None
 
-    def upload_world(self, ev: EvalOutput, device_shadow_cameras: bool = False):
+    def upload_world(self, ev: EvalOutput, device_shadow_cameras: bool = False, movable_objects: bool = False):
         """What evaluate_instructions leaves in wgpu buffers (renderer/eval.rs:157-181).  With `device_shadow_cameras` the lights go up
-        as sources and atlas placements; the frame evaluates their shadow cameras on the device."""
+        as sources and atlas placements; the frame evaluates their shadow cameras on the device.  With `movable_objects` the mesh
+        bounding spheres go up too (r3_set_object_mesh_spheres), so that r3_set_object_transforms can move the objects."""
         b = self.backend
         b.set_objects(ev.object_buffer)
         flags = (ev.object_live & 1) | ((ev.object_atomic & 1) << 1) | ((ev.object_back_to_front & 1) << 2)
         loc = np.ascontiguousarray(ev.object_location, dtype=f32)
         b.set_object_sort_info(ev.object_material_key, flags.astype(np.uint8), loc)
+        if movable_objects:
+            assert ev.object_mesh_sphere is not None, "this EvalOutput carries no mesh spheres"
+            b.set_object_mesh_spheres(ev.object_mesh_sphere)
         b.set_mesh_buffer(ev.mesh_buffer)
         b.set_textures(ev.texture_descs, ev.texture_texels)
         b.set_skybox(ev.skybox_desc, ev.skybox_texels)
@@ -131,7 +135,8 @@ class BaseRenderGraph:
                      settings: BaseRenderGraphSettings = BaseRenderGraphSettings(), srgb_target: bool = True,
                      upload: bool = True, scissor_rows: Optional[Tuple[int, int]] = None, shadow_filter=None, after_shadows=None,
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
-                     posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False):
+                     posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
+                     movable_objects: bool = False):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -147,13 +152,17 @@ class BaseRenderGraph:
         (r3_pose_objects after r3_set_object_animations / r3_set_object_pose_jobs): their transforms, world spheres and sort locations
         are written before any camera culls, also enqueue only.  `device_shadow_cameras` uploads the lights as sources
         (r3_set_directional_light_sources) and evaluates their shadow cameras on the device around this frame's camera
-        (r3_evaluate_shadow_cameras, r3_shadow_uniform_upload): a frame whose camera moves needs no light upload."""
+        (r3_evaluate_shadow_cameras, r3_shadow_uniform_upload): a frame whose camera moves needs no light upload.
+        `object_transforms` = (slots or None, matrices) moves objects at the skinning node, before `posed_objects`
+        (Renderer::set_object_transform in bulk): CUDA tensors go through r3_set_object_transforms_device — enqueue only, their producer
+        ordered on the context's stream — and host arrays through r3_set_object_transforms, which waits for the stream.  It needs the mesh
+        spheres: an uploading frame with `movable_objects` (or `object_transforms`) sends them."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
         b, culler = self.backend, self.gpu_culler
         if upload:
-            self.upload_world(ev, device_shadow_cameras)
+            self.upload_world(ev, device_shadow_cameras, movable_objects or object_transforms is not None)
         if self._resolution != (resolution, samples, tuple(settings.clear_color)):
             b.set_render_target(resolution[0], resolution[1], samples, settings.clear_color)
             self._resolution = (resolution, samples, tuple(settings.clear_color))
@@ -174,6 +183,12 @@ class BaseRenderGraph:
             b.evaluate_shadow_cameras(ev.camera.location())
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
+        if object_transforms is not None:                                         # :145 objects the application moved this frame
+            slots, matrices = object_transforms
+            if getattr(matrices, "is_cuda", False):
+                b.set_object_transforms_device(matrices, slots)
+            else:
+                b.set_object_transforms(matrices, slots)
         if posed_objects:                                                         # :145 pose_animation_frame's set_object_transform half
             b.pose_objects()
         if posed_skinning:                                                        # :145 from resident data (r3_set_skeletons / r3_set_pose_jobs)

@@ -29,6 +29,8 @@ def dump_scene(path: str, ev: EvalOutput, resolution: Tuple[int, int], samples: 
         _section(f, "material_key", np.ascontiguousarray(ev.object_material_key, dtype=np.uint64).tobytes())
         _section(f, "sort_flags", flags.tobytes())
         _section(f, "location", np.ascontiguousarray(ev.object_location, dtype=np.float32).tobytes())
+        if ev.object_mesh_sphere is not None:
+            _section(f, "mesh_spheres", np.ascontiguousarray(ev.object_mesh_sphere, dtype=np.float32).tobytes())
         _section(f, "mesh", np.ascontiguousarray(ev.mesh_buffer).tobytes())
         _section(f, "materials", np.ascontiguousarray(ev.material_buffer).tobytes())
         _section(f, "tex_descs", np.ascontiguousarray(ev.texture_descs).tobytes())

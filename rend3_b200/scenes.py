@@ -76,7 +76,8 @@ def bulk_object_records(renderer: Renderer, transforms: np.ndarray, mesh_ids: np
     return rec, loc
 
 
-def eval_with_bulk_objects(renderer: Renderer, rec: np.ndarray, loc: np.ndarray, n_live: int) -> EvalOutput:
+def eval_with_bulk_objects(renderer: Renderer, rec: np.ndarray, loc: np.ndarray, n_live: int, mesh_ids: Optional[np.ndarray] = None) -> EvalOutput:
+    """`mesh_ids` (the objects' meshes, as given to bulk_object_records) also fills the mesh spheres r3_set_object_mesh_spheres takes."""
     ev = renderer.evaluate()
     cap = len(rec)
     mats = renderer.materials
@@ -90,6 +91,11 @@ def eval_with_bulk_objects(renderer: Renderer, rec: np.ndarray, loc: np.ndarray,
     ev.object_back_to_front = np.zeros(cap, dtype=np.uint8); ev.object_back_to_front[:n_live] = b2f_of[mi]
     ev.object_live = np.zeros(cap, dtype=np.uint8); ev.object_live[:n_live] = 1
     ev.object_location = loc
+    ev.object_mesh_sphere = None
+    if mesh_ids is not None:
+        ev.object_mesh_sphere = np.zeros((cap, 4), dtype=f32)
+        ev.object_mesh_sphere[:n_live, :3] = np.array([m["center"] for m in renderer.meshes], dtype=f32)[mesh_ids]
+        ev.object_mesh_sphere[:n_live, 3] = np.array([m["radius"] for m in renderer.meshes], dtype=f32)[mesh_ids]
     return ev
 
 
@@ -256,7 +262,7 @@ def cube_field_scene(n_objects: int = 10_000, seed: int = 1, resolution: Tuple[i
         material_ids = np.concatenate([material_ids, np.zeros(3, dtype=np.uint32)])
         n_objects += 3
     rec, loc = bulk_object_records(r, transforms, mesh_ids, material_ids)
-    return eval_with_bulk_objects(r, rec, loc, n_objects)
+    return eval_with_bulk_objects(r, rec, loc, n_objects, mesh_ids)
 
 
 def object_cloud_records(n: int, seed: int = 2, extent: float = 1000.0, disabled_fraction: float = 0.01) -> np.ndarray:

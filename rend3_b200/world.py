@@ -539,6 +539,9 @@ class EvalOutput:
     # the lights behind directional_buffer, in its order, with their atlas placements (LIGHT_SOURCE_DTYPE): what
     # r3_set_directional_light_sources takes so that the device evaluates the shadow cameras around each frame's camera
     directional_sources: Optional[np.ndarray] = None
+    # (capacity, 4) f32  InternalObject::mesh_bounding_sphere (object.rs:268-270) as (centre, radius), zeros for empty slots: what
+    # r3_set_object_mesh_spheres takes so that r3_set_object_transforms can move the objects on the device
+    object_mesh_sphere: Optional[np.ndarray] = None
 
 
 class Renderer:
@@ -718,9 +721,11 @@ class Renderer:
         b2f = np.zeros(cap, dtype=np.uint8)
         live = np.zeros(cap, dtype=np.uint8)
         location = np.zeros((cap, 3), dtype=f32)
+        mesh_sphere = np.zeros((cap, 4), dtype=f32)
         for i, e in enumerate(self.objects[:cap]):
             if e is None:
                 continue
+            mesh_sphere[i, :3], mesh_sphere[i, 3] = e["mesh_center"], e["mesh_radius"]
             m = self.materials[int(e["rec"]["material_index"])]
             key[i], atomic[i], b2f[i], live[i] = m.key(), m.atomic_capable(), m.back_to_front(), 1
             location[i] = e["location"]
@@ -784,4 +789,5 @@ class Renderer:
             shadows=shadows,
             shadow_target_size=size,
             camera=self.camera,
+            object_mesh_sphere=mesh_sphere,
         )
