@@ -187,6 +187,19 @@ typedef struct r3_point_light {
 } r3_point_light;
 R3_STATIC_ASSERT(sizeof(r3_point_light) == 32, "PointLight");
 
+/* One point light as the caller keeps it — rend3-types PointLight (rend3-types/src/lib.rs:1124-1136), in its field order: one entry of
+ * PointLightManager's handle table (r3_set_point_light_sources / r3_update_point_light_sources) */
+typedef struct r3_point_light_source {
+    float position[3];            /* @0 */
+    float color[3];               /* @12 */
+    float radius;                 /* @24 */
+    float intensity;              /* @28 */
+} r3_point_light_source;
+R3_STATIC_ASSERT(sizeof(r3_point_light_source) == 32, "PointLight source");
+R3_STATIC_ASSERT(offsetof(r3_point_light_source, color) == 12, "color");
+R3_STATIC_ASSERT(offsetof(r3_point_light_source, radius) == 24, "radius");
+R3_STATIC_ASSERT(offsetof(r3_point_light_source, intensity) == 28, "intensity");
+
 /* GpuPoweredShaderWrapper<PbrMaterial> — managers/material.rs:25-29 + pbr/material.rs:526-543,
  * material.wgsl:21-57 (208 bytes) */
 typedef struct r3_material {

@@ -21,7 +21,7 @@
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_evaluate_shadow_cameras,
- *     r3_shadow_uniform_upload,
+ *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
@@ -30,7 +30,7 @@
  *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices, r3_set_object_animations,
  *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_directional_light_sources,
- *     r3_readback_shadow_cameras —
+ *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
  *     has to grow (first frame, larger world, new resolution) is reallocated with a stream synchronisation as well.
@@ -170,6 +170,37 @@ int r3_set_skybox(r3_ctx*, const r3_texture_desc* desc, const void* texels, uint
 int r3_set_directional_lights(r3_ctx*, const void* bytes, uint64_t nbytes,
                               uint32_t atlas_width, uint32_t atlas_height);         /* directional.rs:135-156 */
 int r3_set_point_lights(r3_ctx*, const void* bytes, uint64_t nbytes);              /* point.rs:58-74 */
+/* PointLightManager (rend3/src/managers/point.rs) on the device: the handle table `data: Vec<Option<PointLight>>` lives in device memory
+ * and its evaluate (point.rs:58-74, called once per frame at renderer/eval.rs:180) runs as a kernel, so lights that move every frame —
+ * also lights whose positions a CUDA producer computes — need no upload and no stream drain.
+ *   r3_set_point_light_sources            blocking: replaces the whole table with n_handles entries (data after a run of add's);
+ *                                         live_or_null[h] == 0 marks handle h dead (None), live_or_null == NULL: every handle is live.
+ *   r3_update_point_light_sources         blocking: add / update / remove of n handles from HOST memory.  live[i] == 0 removes handles[i],
+ *                                         any other value adds or replaces it with lights[i].  A handle at or beyond the table's size grows
+ *                                         the table (add's resize); the handles between start dead.  A handle named twice, a null pointer
+ *                                         or the handle 0xFFFFFFFF (the table size would not fit 32 bits) is R3_E_INVALID and nothing is
+ *                                         written.  The arrays are copied, one kernel runs and the stream is drained once.
+ *   r3_update_point_light_sources_device  the same from DEVICE memory, enqueue only (legal between r3_frame_begin and r3_frame_end; in a
+ *                                         frame graph the kernel's arguments are updated in place).  d_live_or_null == NULL: every listed
+ *                                         handle is added or replaced.  Handles must be distinct (two entries' stores would land in an
+ *                                         unspecified order); handles at or beyond the table's size are dropped (the table cannot grow
+ *                                         without the host).  The producer of the arrays is ordered as for r3_set_object_transforms_device.
+ *   r3_evaluate_point_lights              enqueue only: ShaderPointLightBuffer (count @0, then {position.xyz 1, colour * intensity, radius}
+ *                                         per live handle in ascending handle order @16) into the buffer the shading reads.  Call it once
+ *                                         per frame after r3_set_frame_uniforms.  Arithmetic: DESIGN.md §2, R14 (exact).
+ *   r3_readback_point_lights              blocking: the buffer the shading reads, in the layout above, whichever call filled it: the first
+ *                                         min(capacity_bytes, 16 + 32 count) bytes (capacity_bytes >= 16; read the count at @0 and call
+ *                                         again with more room when the array did not fit).
+ * r3_set_point_lights and the source calls each replace what the other set: r3_set_point_lights empties the handle table, and an
+ * evaluation rewrites the buffer from the table.  After a set or update, r3_forward_resolve and r3_forward_blend return R3_E_STATE until
+ * r3_evaluate_point_lights has run.  The shading reads the light count from the device buffer; the host only knows a capacity (the
+ * table size, or r3_set_point_lights' count), so a frame graph keeps its topology while lights come and go. */
+int r3_set_point_light_sources(r3_ctx*, const r3_point_light_source* lights, const uint8_t* live_or_null, uint32_t n_handles);
+int r3_update_point_light_sources(r3_ctx*, const uint32_t* handles, const r3_point_light_source* lights, const uint8_t* live, uint32_t n);
+int r3_update_point_light_sources_device(r3_ctx*, const uint32_t* d_handles, const r3_point_light_source* d_lights,
+                                         const uint8_t* d_live_or_null, uint32_t n);
+int r3_evaluate_point_lights(r3_ctx*);
+int r3_readback_point_lights(r3_ctx*, void* bytes, uint64_t capacity_bytes);
 /* DirectionalLightManager::evaluate (directional.rs:99-157) on the device, with the shadow camera arithmetic of rule R13 (DESIGN.md §2).
  *   r3_set_directional_light_sources  blocking: the lights and their atlas placements.  Fills the light buffer's static fields
  *                                     (colour * intensity, direction, 1 / atlas size, offset / atlas size, size / atlas size) and

@@ -63,6 +63,9 @@ struct EvalOutput {
     // r3_set_directional_light_sources takes when the shadow cameras are evaluated on the device
     const r3_directional_light_source* directional_sources = nullptr; uint32_t n_directional_sources = 0; bool left_handed = true;
     const void* point_lights = nullptr; uint64_t point_bytes = 0;
+    // PointLightManager's handle table behind point_lights (records + live bytes, dead handles included): what
+    // r3_set_point_light_sources takes when the point lights are evaluated on the device
+    const r3_point_light_source* point_sources = nullptr; const uint8_t* point_live = nullptr; uint32_t n_point_handles = 0;
     std::vector<ShadowMap> shadows;
     r3_camera_header viewport{};              // PerCameraUniform header of the viewport camera for this target
     r3_frame_uniforms uniforms{};             // FrameUniforms::new
@@ -101,8 +104,9 @@ public:
     void check(int rc) const { if (rc != R3_OK) throw Error(rc, r3_last_error(ctx_)); }
 
     // renderer/eval.rs:157-181 — the buffers evaluate_instructions (re)uploads
-    // device_shadow_cameras: the lights go up as sources (the frame evaluates their shadow cameras) instead of the light buffer
-    void upload_world(const EvalOutput& ev, bool device_shadow_cameras = false) {
+    // device_shadow_cameras: the lights go up as sources (the frame evaluates their shadow cameras) instead of the light buffer;
+    // device_point_lights: the point lights go up as the handle table (the frame evaluates them) instead of the evaluated buffer
+    void upload_world(const EvalOutput& ev, bool device_shadow_cameras = false, bool device_point_lights = false) {
         check(r3_set_objects(ctx_, ev.objects, ev.n_slots));
         if (ev.material_key) check(r3_set_object_sort_info(ctx_, ev.material_key, ev.sort_flags, ev.location, ev.n_slots));
         if (ev.mesh_spheres) check(r3_set_object_mesh_spheres(ctx_, nullptr, ev.mesh_spheres, ev.n_slots));
@@ -115,7 +119,8 @@ public:
                                                    ev.left_handed ? 1u : 0u));
         else
             check(r3_set_directional_lights(ctx_, ev.directional_lights, ev.directional_bytes, ev.shadow_target_size[0], ev.shadow_target_size[1]));
-        check(r3_set_point_lights(ctx_, ev.point_lights, ev.point_bytes));
+        if (device_point_lights) check(r3_set_point_light_sources(ctx_, ev.point_sources, ev.point_live, ev.n_point_handles));
+        else check(r3_set_point_lights(ctx_, ev.point_lights, ev.point_bytes));
     }
     // Renderer::set_object_transform (object.rs:302-316) for n objects from host memory (slots == nullptr: slots 0 .. n-1); blocking
     void set_object_transforms(const uint32_t* slots, const float* mat4s, uint32_t n) { check(r3_set_object_transforms(ctx_, slots, mat4s, n)); }
@@ -183,6 +188,9 @@ public:
     // DirectionalLightManager::evaluate on the device (after Renderer::upload_world(ev, true)): the shadow cameras are evaluated around
     // this frame's viewport_location and culled from device memory; ev.shadows' headers are not read, only their atlas viewports
     bool device_shadow_cameras = false;
+    // PointLightManager::evaluate on the device (after Renderer::upload_world(ev, ..., true)), right after the frame uniforms; add / update /
+    // remove before it with r3_update_point_light_sources_device (enqueue only) or r3_update_point_light_sources
+    bool device_point_lights = false;
 
     void add_to_graph(Renderer& r, const EvalOutput& ev, uint32_t width, uint32_t height, SampleCount samples, const BaseRenderGraphSettings& settings,
                       bool target_is_srgb = true) {
@@ -191,6 +199,7 @@ public:
         r.check(r3_clear_shadow_atlas(r.raw()));                                                     // base.rs:139
         r.check(r3_set_frame_uniforms(r.raw(), &ev.uniforms));                                       // :142
         if (device_shadow_cameras) r.check(r3_evaluate_shadow_cameras(r.raw(), ev.viewport_location));
+        if (device_point_lights) r.check(r3_evaluate_point_lights(r.raw()));                       // renderer/eval.rs:180
         gpu_skinner.add_skinning_to_graph(r, ev);                                                    // :145 state.skinning — before any camera culls
         for (uint32_t i = 0; i < ev.shadows.size(); ++i) {                                          // :148
             if (device_shadow_cameras) r.check(r3_shadow_uniform_upload(r.raw(), i, ev.n_slots, R3_CB_BAKE | R3_CB_CULL));

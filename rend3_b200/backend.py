@@ -261,6 +261,53 @@ class Backend:
     def set_point_lights(self, data: bytes):
         self._call("set_point_lights", C.c_char_p(data), C.c_uint64(len(data)))
 
+    # ---- PointLightManager on the device (handle table, add / update / remove, evaluate)
+    def set_point_light_sources(self, sources: np.ndarray, live: Optional[np.ndarray] = None):
+        """The whole handle table: POINT_LIGHT_SOURCE_DTYPE[n] and live bytes (None: every handle live).  Blocking."""
+        from .layouts import POINT_LIGHT_SOURCE_DTYPE
+
+        src = np.ascontiguousarray(sources, dtype=POINT_LIGHT_SOURCE_DTYPE).reshape(-1)
+        lv = None if live is None else np.ascontiguousarray(live, dtype=np.uint8).reshape(-1)
+        assert lv is None or len(lv) == len(src)
+        self._call("set_point_light_sources", _ptr(src) if len(src) else None, _ptr(lv) if lv is not None and len(lv) else None, C.c_uint32(len(src)))
+
+    def update_point_light_sources(self, handles, sources: np.ndarray, live):
+        """add / update (live != 0) or remove (live == 0) of the listed handles, from host memory.  Blocking."""
+        from .layouts import POINT_LIGHT_SOURCE_DTYPE
+
+        h = np.ascontiguousarray(handles, dtype=np.uint32).reshape(-1)
+        src = np.ascontiguousarray(sources, dtype=POINT_LIGHT_SOURCE_DTYPE).reshape(-1)
+        lv = np.ascontiguousarray(live, dtype=np.uint8).reshape(-1)
+        assert len(src) == len(h) and len(lv) == len(h)
+        self._call("update_point_light_sources", _ptr(h), _ptr(src), _ptr(lv), C.c_uint32(len(h)))
+
+    def update_point_light_sources_device(self, handles, sources, live=None, n: Optional[int] = None):
+        """The same from device memory, enqueue only.  `handles` (int32 / uint32 (n,)), `sources` (float32 (n, 8): the 32-byte records)
+        and `live` (uint8 (n,), None: every handle live) are contiguous CUDA tensors, or raw device pointers with `n` given; the caller
+        keeps them alive and orders their producer on stream()."""
+        def pointer(x, elem, width):
+            if x is None or isinstance(x, int):
+                return x, None
+            assert x.is_cuda and x.is_contiguous() and x.element_size() == elem, "a contiguous CUDA tensor"
+            return x.data_ptr(), x.numel() // width
+        hp, hn = pointer(handles, 4, 1)
+        sp, sn = pointer(sources, 4, 8)
+        lp, ln = pointer(live, 1, 1)
+        n = hn if n is None else n
+        assert n is not None and (sn is None or sn == n) and (ln is None or ln == n)
+        self._call("update_point_light_sources_device", C.c_void_p(hp), C.c_void_p(sp), C.c_void_p(lp), C.c_uint32(n))
+
+    def evaluate_point_lights(self):
+        self._call("evaluate_point_lights")
+
+    def readback_point_lights(self) -> bytes:
+        """The buffer the shading reads: u32 count @0, POINT_LIGHT_DTYPE array @16 (as EvalOutput.point_buffer)."""
+        head = np.zeros(4, dtype=np.uint32)
+        self._call("readback_point_lights", _ptr(head), C.c_uint64(16))
+        out = np.zeros(16 + 32 * int(head[0]), dtype=np.uint8)
+        self._call("readback_point_lights", _ptr(out), C.c_uint64(len(out)))
+        return out.tobytes()
+
     def set_frame_uniforms(self, record: np.ndarray):
         b = record.tobytes()
         assert len(b) == 496

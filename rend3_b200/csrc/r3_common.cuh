@@ -131,7 +131,12 @@ struct r3_ctx {
     r3_directional_light_source* d_light_src = nullptr; r3_camera_header* d_shadow_cams = nullptr;
     std::vector<r3_directional_light_source> light_src;
     bool light_src_set = false, shadow_cams_evaluated = false; uint32_t light_src_left_handed = 0;
-    r3_point_light* d_point = nullptr; uint32_t n_point = 0, point_cap = 0;
+    // ShaderPointLightBuffer as the shading reads it: u32 count @0, r3_point_light array @16 (allocated at context creation, count 0).
+    // The count is only known on the device; point_capacity (r3_set_point_lights' count, or the handle table's size) bounds it and sizes
+    // the light prep.  point_handles: size of PointLightManager's handle table (r3_lights.cu), sources + live bytes on the device.
+    uint8_t* d_point = nullptr; uint64_t point_bytes_cap = 0; uint32_t point_capacity = 0;
+    r3_point_light_source* d_point_src = nullptr; uint8_t* d_point_live = nullptr; uint32_t point_handles = 0, point_src_cap = 0, point_live_cap = 0;
+    bool point_eval_pending = false;          // sources set or updated since the last r3_evaluate_point_lights: the buffer is stale
     float* d_light_mats = nullptr; uint64_t light_mats_cap = 0;   // view-space light tables built by light_prep_kernel
     r3_frame_uniforms uniforms{}; bool uniforms_set = false;
     float* d_atlas = nullptr; uint32_t atlas_w = 0, atlas_h = 0;
@@ -241,6 +246,7 @@ void r3_anim_apply_posed_locations(r3_ctx* c);
 // copy of every location into c->sort_loc, complete once the caller has drained the stream
 int r3_stage_moved_locations(r3_ctx* c, bool* staged);
 int r3_grow_mesh_spheres(r3_ctx* c, uint32_t n);   // r3_resize_objects: zero spheres for the new slots, once spheres are set
+int r3_reserve_point_buffer(r3_ctx* c, uint32_t n_lights);   // r3_lights.cu: room for n lights in c->d_point, contents kept
 
 #ifdef __CUDACC__
 // Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine

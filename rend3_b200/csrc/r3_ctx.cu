@@ -63,6 +63,10 @@ R3_EXPORT int r3_ctx_create(int device, r3_ctx** out) {
     if (cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || c->sm_count < 1) { cudaStreamDestroy(c->stream); delete c; cudaGetLastError(); return R3_E_CUDA; }
     if (cudaMalloc((void**)&c->d_stats, 8 * sizeof(unsigned long long)) != cudaSuccess) { delete c; return R3_E_OOM; }
     cudaMemsetAsync(c->d_stats, 0, 64, c->stream);
+    // the shading reads the point-light count from this buffer in every frame: it exists from the start, holding no light
+    c->point_bytes_cap = 16 + 16 * sizeof(r3_point_light);
+    if (cudaMalloc((void**)&c->d_point, c->point_bytes_cap) != cudaSuccess) { cudaFree(c->d_stats); delete c; return R3_E_OOM; }
+    cudaMemsetAsync(c->d_point, 0, c->point_bytes_cap, c->stream);
     *out = c;
     return R3_OK;
 }
@@ -80,7 +84,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
     cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc); cudaFree(c->d_gsort_keys[0]); cudaFree(c->d_gsort_keys[1]); cudaFree(c->d_gsort_hist); cudaFree(c->d_gsort_header);
     cudaFree(c->d_mesh_spheres); cudaFree(c->d_live_bits); cudaFree(c->d_mesh); cudaFree(c->d_materials); cudaFree(c->d_dir); cudaFree(c->d_point);
-    cudaFree(c->d_light_mats); cudaFree(c->d_atlas); cudaFree(c->d_light_src); cudaFree(c->d_shadow_cams);
+    cudaFree(c->d_light_mats); cudaFree(c->d_atlas); cudaFree(c->d_light_src); cudaFree(c->d_shadow_cams); cudaFree(c->d_point_src); cudaFree(c->d_point_live);
     for (auto& k : c->cams) {
         cudaFree(k.d_matrices); cudaFree(k.d_visible); cudaFree(k.d_visible_count); cudaFree(k.d_tile_state);
         if (k.d_gathered) {   // visible-set exchange: unmap the peers' buffers, free ours
@@ -597,10 +601,13 @@ R3_EXPORT int r3_set_point_lights(r3_ctx* c, const void* bytes, uint64_t nbytes)
     cudaSetDevice(c->device);
     const uint32_t n = *(const uint32_t*)bytes;
     if (nbytes < 16 + (uint64_t)n * sizeof(r3_point_light)) return r3_fail(c, R3_E_INVALID, "set_point_lights: short buffer");
-    R3_TRY(r3_reserve_t(c, &c->d_point, &c->point_cap, n));
-    if (n) R3_CUDA(c, cudaMemcpyAsync(c->d_point, (const uint8_t*)bytes + 16, (size_t)n * sizeof(r3_point_light), cudaMemcpyHostToDevice, c->stream));
+    R3_TRY(r3_reserve_point_buffer(c, n));
+    // header and array together: the shading reads the count from the device, whichever call filled the buffer
+    R3_CUDA(c, cudaMemcpyAsync(c->d_point, bytes, 16 + (size_t)n * sizeof(r3_point_light), cudaMemcpyHostToDevice, c->stream));
     R3_CUDA(c, r3_stream_sync(c));
-    c->n_point = n;
+    c->point_capacity = n;
+    c->point_handles = 0;             // replaces the handle table of r3_set_point_light_sources
+    c->point_eval_pending = false;
     return R3_OK;
 }
 void r3_new_frame_epoch(r3_ctx* c) {

@@ -8,10 +8,13 @@
 //   r3_evaluate_shadow_cameras        one thread per light writes the light's view_proj and its camera header (view, view_proj, frustum)
 //   r3_shadow_uniform_upload          the cull + bake of Shadow(i) reading that header on the device
 //   r3_readback_shadow_cameras        blocking readback of the headers and light records
+// and PointLightManager's handle table with its evaluate (second half of the file).
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 
 #include "r3_common.cuh"
+#include "r3_scan.cuh"
 
 namespace {
 
@@ -225,5 +228,154 @@ R3_EXPORT int r3_readback_shadow_cameras(r3_ctx* c, r3_camera_header* out, r3_di
     if (n) R3_CUDA(c, cudaMemcpyAsync(out, c->d_shadow_cams, (size_t)n * sizeof *out, cudaMemcpyDeviceToHost, c->stream));
     if (n && lights) R3_CUDA(c, cudaMemcpyAsync(lights, c->d_dir, (size_t)n * sizeof *lights, cudaMemcpyDeviceToHost, c->stream));
     R3_CUDA(c, r3_stream_sync(c));
+    return R3_OK;
+}
+
+// ------------------------------------------------------------------ point lights
+// PointLightManager (rend3/src/managers/point.rs) on the device: the handle table `data: Vec<Option<PointLight>>` as sources + live
+// bytes, add / update / remove as one scatter kernel (from host or device memory) and evaluate (point.rs:58-74) as one CTA that compacts
+// the live handles in ascending order into ShaderPointLightBuffer — rule R14 (DESIGN.md §2): position (x, y, z, 1), colour = three
+// __fmul_rn(c, intensity), radius copied; nothing is clamped, so NaN, inf, negative and zero values reach the shading unchanged.
+namespace {
+
+constexpr int POINT_EVAL_THREADS = 256;
+
+// one thread per listed handle; out-of-range handles are dropped (the device form cannot grow the table)
+__global__ void point_light_scatter_kernel(const uint32_t* __restrict__ handles, const r3_point_light_source* __restrict__ lights,
+                                           const uint8_t* __restrict__ live, uint32_t n, uint32_t n_handles,
+                                           r3_point_light_source* __restrict__ table, uint8_t* __restrict__ table_live) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t h = handles[i];
+    if (h >= n_handles) return;
+    const uint8_t l = live ? (live[i] != 0 ? 1 : 0) : 1;
+    if (l) table[h] = lights[i];   // a removed handle keeps its record: evaluate skips it, the next add overwrites it
+    table_live[h] = l;
+}
+
+// data.iter().flatten() in handle order: one CTA walks the table a block at a time, the running count carried across the chunks
+__global__ void __launch_bounds__(POINT_EVAL_THREADS) point_light_evaluate_kernel(const r3_point_light_source* __restrict__ table,
+                                                                                   const uint8_t* __restrict__ table_live, uint32_t n_handles,
+                                                                                   uint8_t* __restrict__ out) {
+    __shared__ uint32_t s_warp[POINT_EVAL_THREADS / 32 + 1];
+    float4* dst = reinterpret_cast<float4*>(out + 16);
+    const uint32_t count = block_scan_excl_chunked<POINT_EVAL_THREADS, uint32_t>(
+        n_handles, s_warp, [&](uint32_t h) { return table_live[h] ? 1u : 0u; },
+        [&](uint32_t h, uint32_t pos) {
+            if (!table_live[h]) return;
+            const r3_point_light_source s = table[h];
+            dst[2 * (size_t)pos] = make_float4(s.position[0], s.position[1], s.position[2], 1.0f);
+            dst[2 * (size_t)pos + 1] = make_float4(__fmul_rn(s.color[0], s.intensity), __fmul_rn(s.color[1], s.intensity),
+                                                   __fmul_rn(s.color[2], s.intensity), s.radius);
+        });
+    if (threadIdx.x == 0) *reinterpret_cast<uint4*>(out) = make_uint4(count, 0u, 0u, 0u);
+}
+
+// the table's device arrays hold at least n handles, contents kept; the handles in [c->point_handles, n) start dead
+int grow_point_table(r3_ctx* c, uint32_t n) {
+    if (n <= c->point_handles) return R3_OK;
+    R3_TRY(r3_reserve_t(c, &c->d_point_src, &c->point_src_cap, n, true));
+    R3_TRY(r3_reserve_t(c, &c->d_point_live, &c->point_live_cap, n, true));
+    R3_TRY(r3_reserve_point_buffer(c, n));
+    R3_CUDA(c, cudaMemsetAsync(c->d_point_live + c->point_handles, 0, n - c->point_handles, c->stream));
+    return R3_OK;
+}
+
+int launch_point_scatter(r3_ctx* c, const uint32_t* handles, const r3_point_light_source* lights, const uint8_t* live, uint32_t n) {
+    point_light_scatter_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(handles, lights, live, n, c->point_handles, c->d_point_src, c->d_point_live);
+    R3_CHECK_LAUNCH(c, "point_light_scatter_kernel");
+    return R3_OK;
+}
+
+}  // namespace
+
+int r3_reserve_point_buffer(r3_ctx* c, uint32_t n_lights) {
+    uint64_t cap = c->point_bytes_cap;
+    void* p = c->d_point;
+    const int rc = r3_reserve(c, &p, &cap, 16 + (uint64_t)n_lights * sizeof(r3_point_light), 1, true, false);
+    c->d_point = (uint8_t*)p; c->point_bytes_cap = cap;
+    return rc;
+}
+
+R3_EXPORT int r3_set_point_light_sources(r3_ctx* c, const r3_point_light_source* lights, const uint8_t* live, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (!lights && n) return r3_fail(c, R3_E_INVALID, "set_point_light_sources: null lights");
+    cudaSetDevice(c->device);
+    R3_TRY(r3_reserve_t(c, &c->d_point_src, &c->point_src_cap, n, true));   // kept: a failed allocation leaves the old table
+    R3_TRY(r3_reserve_t(c, &c->d_point_live, &c->point_live_cap, n, true));
+    R3_TRY(r3_reserve_point_buffer(c, n));
+    if (n) {
+        R3_CUDA(c, cudaMemcpyAsync(c->d_point_src, lights, (size_t)n * sizeof *lights, cudaMemcpyHostToDevice, c->stream));
+        if (live) R3_CUDA(c, cudaMemcpyAsync(c->d_point_live, live, n, cudaMemcpyHostToDevice, c->stream));
+        else R3_CUDA(c, cudaMemsetAsync(c->d_point_live, 1, n, c->stream));
+    }
+    R3_CUDA(c, r3_stream_sync(c));   // `lights` and `live` are only borrowed
+    c->point_handles = n;
+    c->point_capacity = n;
+    c->point_eval_pending = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_update_point_light_sources(r3_ctx* c, const uint32_t* handles, const r3_point_light_source* lights, const uint8_t* live, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (!handles || !lights || !live) return r3_fail(c, R3_E_INVALID, "update_point_light_sources: null");
+    if (n == 0) return R3_OK;
+    std::vector<uint32_t> sorted(handles, handles + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint32_t i = 1; i < n; ++i)
+        if (sorted[i] == sorted[i - 1]) return r3_fail(c, R3_E_INVALID, "update_point_light_sources: a handle is named twice");
+    if (sorted.back() == 0xFFFFFFFFu) return r3_fail(c, R3_E_INVALID, "update_point_light_sources: handle 0xFFFFFFFF (the table size would not fit 32 bits)");
+    cudaSetDevice(c->device);
+    const uint32_t size = std::max(c->point_handles, sorted.back() + 1u);
+    R3_TRY(grow_point_table(c, size));
+    const size_t bytes = (size_t)n * (sizeof(r3_point_light_source) + 4 + 1);
+    R3_TRY(r3_reserve(c, &c->d_scratch, &c->scratch_cap, bytes, 1, false, false));
+    r3_point_light_source* d_lights = (r3_point_light_source*)c->d_scratch;
+    uint32_t* d_handles = (uint32_t*)(d_lights + n);
+    uint8_t* d_live = (uint8_t*)(d_handles + n);
+    R3_CUDA(c, cudaMemcpyAsync(d_lights, lights, (size_t)n * sizeof *lights, cudaMemcpyHostToDevice, c->stream));
+    R3_CUDA(c, cudaMemcpyAsync(d_handles, handles, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
+    R3_CUDA(c, cudaMemcpyAsync(d_live, live, n, cudaMemcpyHostToDevice, c->stream));
+    c->point_handles = size;
+    c->point_capacity = size;
+    R3_TRY(launch_point_scatter(c, d_handles, d_lights, d_live, n));
+    R3_CUDA(c, r3_stream_sync(c));
+    c->point_eval_pending = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_update_point_light_sources_device(r3_ctx* c, const uint32_t* d_handles, const r3_point_light_source* d_lights, const uint8_t* d_live, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (n == 0) return R3_OK;
+    if (!d_handles || !d_lights) return r3_fail(c, R3_E_INVALID, "update_point_light_sources_device: null");
+    cudaSetDevice(c->device);
+    R3_TRY(launch_point_scatter(c, d_handles, d_lights, d_live, n));
+    c->point_eval_pending = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_evaluate_point_lights(r3_ctx* c) {
+    if (!c) return R3_E_INVALID;
+    cudaSetDevice(c->device);
+    point_light_evaluate_kernel<<<1, POINT_EVAL_THREADS, 0, c->stream>>>(c->d_point_src, c->d_point_live, c->point_handles, c->d_point);
+    R3_CHECK_LAUNCH(c, "point_light_evaluate_kernel");
+    c->point_capacity = c->point_handles;
+    c->point_eval_pending = false;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_readback_point_lights(r3_ctx* c, void* bytes, uint64_t capacity) {
+    if (!c) return R3_E_INVALID;
+    if (!bytes || capacity < 16) return r3_fail(c, R3_E_INVALID, "readback_point_lights: room for the 16-byte header needed");
+    cudaSetDevice(c->device);
+    R3_CUDA(c, cudaMemcpyAsync(bytes, c->d_point, 16, cudaMemcpyDeviceToHost, c->stream));
+    R3_CUDA(c, r3_stream_sync(c));
+    const uint64_t held = (c->point_bytes_cap - 16) / sizeof(r3_point_light);
+    const uint64_t count = std::min<uint64_t>(*(const uint32_t*)bytes, held);
+    const uint64_t n = std::min<uint64_t>(count * sizeof(r3_point_light), capacity - 16);
+    if (n) {
+        R3_CUDA(c, cudaMemcpyAsync((uint8_t*)bytes + 16, c->d_point + 16, n, cudaMemcpyDeviceToHost, c->stream));
+        R3_CUDA(c, r3_stream_sync(c));
+    }
     return R3_OK;
 }

@@ -34,7 +34,8 @@ struct ShadeParams {
     const r3_material* materials; uint32_t n_materials;
     TexTable tt;                                                          // bindless d2 texture table (r3_set_textures)
     TexTable sky; r3_texture_desc sky_desc; float inv_origin_view_proj[16];   // skybox routine (r3_set_skybox)
-    const DirPrep* dir; uint32_t n_dir; const PointPrep* point; uint32_t n_point;
+    const DirPrep* dir; uint32_t n_dir; const PointPrep* point;
+    const uint32_t* point_count;                                          // ShaderPointLightBuffer's count (@0), written on the device
     const float* atlas; uint32_t atlas_w, atlas_h;
     // blend routine (r3_forward_blend): triangle records of the key-2 regions + the per-sample fragment lists
     const r3_tri_record* tris2; unsigned long long n_tris2; const uint32_t* frag_heads; const uint4* frag_nodes;
@@ -446,10 +447,12 @@ __device__ __forceinline__ float4 shade_inputs(const ShadeParams& p, const DirPr
             color.x += s.x; color.y += s.y; color.z += s.z;
         }
         uint32_t n_eval = p.n_dir;
-        const uint32_t n_smem_point = min(p.n_point, (uint32_t)MAX_SMEM_POINT);
-        for (uint32_t base = 0; base < p.n_point; base += 32u) {                   // opaque.wgsl:524-546, ascending light order
+        // loaded here, where the loop starts, rather than kept live from the kernel's staging: the register budget stays as it was
+        const uint32_t n_point = *p.point_count;
+        const uint32_t n_smem_point = min(n_point, (uint32_t)MAX_SMEM_POINT);
+        for (uint32_t base = 0; base < n_point; base += 32u) {                     // opaque.wgsl:524-546, ascending light order
             uint32_t m = base < n_smem_point ? mask.w[base >> 5] : 0xFFFFFFFFu;
-            if (p.n_point - base < 32u) m &= (1u << (p.n_point - base)) - 1u;
+            if (n_point - base < 32u) m &= (1u << (n_point - base)) - 1u;
             while (m) {
                 const uint32_t i = base + (uint32_t)__ffs(m) - 1u;
                 m &= m - 1u;
@@ -488,8 +491,10 @@ template <int SAMPLES, bool TEX>
 __global__ void __launch_bounds__(256) resolve_kernel(const __grid_constant__ ShadeParams p) {
     __shared__ DirPrep s_dir[MAX_SMEM_DIR];
     __shared__ PointPrep s_point[MAX_SMEM_POINT];
+    // the point-light count, loaded once for the staging and the tile test (shade_inputs reads the same word for its loop)
+    const uint32_t n_point = *p.point_count;
     {
-        const uint32_t nd = min(p.n_dir, (uint32_t)MAX_SMEM_DIR) * 32u, np = min(p.n_point, (uint32_t)MAX_SMEM_POINT) * 8u;
+        const uint32_t nd = min(p.n_dir, (uint32_t)MAX_SMEM_DIR) * 32u, np = min(n_point, (uint32_t)MAX_SMEM_POINT) * 8u;
         const float* gd = reinterpret_cast<const float*>(p.dir); const float* gp = reinterpret_cast<const float*>(p.point);
         float* sd = reinterpret_cast<float*>(s_dir); float* sp = reinterpret_cast<float*>(s_point);
         for (uint32_t i = threadIdx.x; i < nd; i += blockDim.x) sd[i] = gd[i];
@@ -527,7 +532,7 @@ __global__ void __launch_bounds__(256) resolve_kernel(const __grid_constant__ Sh
             mirror = !(perceptual * perceptual > 1.0e-30f);
         }
         const bool no_cull = __syncthreads_or(mirror ? 1 : 0) != 0;
-        if (p.n_point != 0u && !no_cull) {
+        if (n_point != 0u && !no_cull) {
             const float big = 3.0e38f;
             float lo[3] = {covered ? f.vp.x : big, covered ? f.vp.y : big, covered ? f.vp.z : big};
             float hi[3] = {covered ? f.vp.x : -big, covered ? f.vp.y : -big, covered ? f.vp.z : -big};
@@ -540,7 +545,7 @@ __global__ void __launch_bounds__(256) resolve_kernel(const __grid_constant__ Sh
                 }
             if (lane == 0) { s_box[warp][0] = lo[0]; s_box[warp][1] = lo[1]; s_box[warp][2] = lo[2]; s_box[warp][3] = hi[0]; s_box[warp][4] = hi[1]; s_box[warp][5] = hi[2]; }
             __syncthreads();
-            const uint32_t n_smem_point = min(p.n_point, (uint32_t)MAX_SMEM_POINT);
+            const uint32_t n_smem_point = min(n_point, (uint32_t)MAX_SMEM_POINT);
             if (threadIdx.x < MAX_SMEM_POINT) {
                 bool reach = false;
                 if (threadIdx.x < n_smem_point) {
@@ -566,7 +571,7 @@ __global__ void __launch_bounds__(256) resolve_kernel(const __grid_constant__ Sh
         }
         LightMask mask;
 #pragma unroll
-        for (int k = 0; k < MAX_SMEM_POINT / 32; ++k) mask.w[k] = (p.n_point != 0u && !no_cull) ? s_mask[k] : 0xFFFFFFFFu;
+        for (int k = 0; k < MAX_SMEM_POINT / 32; ++k) mask.w[k] = (n_point != 0u && !no_cull) ? s_mask[k] : 0xFFFFFFFFu;
         if (!in_target) return;
         out = make_float4(p.clear[0], p.clear[1], p.clear[2], p.clear[3]);
         if (covered) { out = shade_inputs<TEX>(p, s_dir, s_point, f, mask, (pass ? p.tris1 : p.tris0) + (rec - 1u), px, py, &n_lights); n_shaded = 1; }
@@ -627,8 +632,9 @@ template <int SAMPLES, bool TEX>
 __global__ void __launch_bounds__(256) blend_apply_kernel(const __grid_constant__ ShadeParams p) {
     __shared__ DirPrep s_dir[MAX_SMEM_DIR];
     __shared__ PointPrep s_point[MAX_SMEM_POINT];
+    const uint32_t n_point = *p.point_count;   // for the staging (shade_inputs reads the same word for its loop)
     {
-        const uint32_t nd = min(p.n_dir, (uint32_t)MAX_SMEM_DIR) * 32u, np = min(p.n_point, (uint32_t)MAX_SMEM_POINT) * 8u;
+        const uint32_t nd = min(p.n_dir, (uint32_t)MAX_SMEM_DIR) * 32u, np = min(n_point, (uint32_t)MAX_SMEM_POINT) * 8u;
         const float* gd = reinterpret_cast<const float*>(p.dir); const float* gp = reinterpret_cast<const float*>(p.point);
         float* sd = reinterpret_cast<float*>(s_dir); float* sp = reinterpret_cast<float*>(s_point);
         for (uint32_t i = threadIdx.x; i < nd; i += blockDim.x) sd[i] = gd[i];
@@ -740,10 +746,13 @@ __global__ void __launch_bounds__(256) skybox_kernel(const __grid_constant__ Sha
     p.hdr16[pi] = make_uint2(*reinterpret_cast<const uint32_t*>(&h01), *reinterpret_cast<const uint32_t*>(&h23));
 }
 
-// light prep: one thread per light (opaque.wgsl:491,519,528 hoisted out of the fragment loop)
-__global__ void light_prep_kernel(const r3_directional_light* dir, uint32_t n_dir, const r3_point_light* point, uint32_t n_point,
+// light prep: one thread per light (opaque.wgsl:491,519,528 hoisted out of the fragment loop).  The grid covers the point lights'
+// capacity; the buffer's count (@0 of `point_buf`, at most that capacity) says how many exist this frame.
+__global__ void light_prep_kernel(const r3_directional_light* dir, uint32_t n_dir, const uint8_t* point_buf,
                                   const __grid_constant__ r3_frame_uniforms u, DirPrep* out_dir, PointPrep* out_point) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t n_point = *reinterpret_cast<const uint32_t*>(point_buf);
+    const r3_point_light* point = reinterpret_cast<const r3_point_light*>(point_buf + 16);
     if (i < n_dir) {
         const r3_directional_light L = dir[i];
         DirPrep o;
@@ -985,7 +994,7 @@ static void fill_shade_params(r3_ctx* c, ShadeParams* out) {
     p.tt.tex = c->d_tex_descs; p.tt.n_tex = c->n_textures; p.tt.texels = c->d_texels; p.tt.clamp_to_edge = 0u;
     p.sky.tex = nullptr; p.sky.n_tex = 0; p.sky.texels = c->has_skybox ? c->d_sky_texels : nullptr; p.sky.clamp_to_edge = 1u;
     p.sky_desc = c->sky_desc; memcpy(p.inv_origin_view_proj, c->uniforms.inv_origin_view_proj, 64);
-    p.dir = d_dir; p.n_dir = c->n_dir; p.point = d_point; p.n_point = c->n_point;
+    p.dir = d_dir; p.n_dir = c->n_dir; p.point = d_point; p.point_count = reinterpret_cast<const uint32_t*>(c->d_point);
     p.atlas = c->d_atlas; p.atlas_w = c->atlas_w; p.atlas_h = c->atlas_h;
     memcpy(p.ambient, c->uniforms.ambient, 16); memcpy(p.clear, c->clear_color, 16);
     p.width = c->width; p.height = c->height; p.row_begin = c->row_begin; p.row_end = c->row_end; p.samples = c->samples;
@@ -994,16 +1003,17 @@ static void fill_shade_params(r3_ctx* c, ShadeParams* out) {
 R3_EXPORT int r3_forward_resolve(r3_ctx* c) {
     if (!c || !c->d_vis) return r3_fail(c, R3_E_STATE, "forward_resolve before set_render_target");
     if (!c->uniforms_set) return r3_fail(c, R3_E_STATE, "forward_resolve before set_frame_uniforms");
+    if (c->point_eval_pending) return r3_fail(c, R3_E_STATE, "forward_resolve: point lights set or updated since the last evaluate_point_lights");
     cudaSetDevice(c->device);
-    const uint64_t need_floats = (uint64_t)c->n_dir * 32 + (uint64_t)c->n_point * 8 + 64;
+    const uint64_t need_floats = (uint64_t)c->n_dir * 32 + (uint64_t)c->point_capacity * 8 + 64;
     static_assert(sizeof(DirPrep) == 32 * 4 && sizeof(PointPrep) == 8 * 4, "prep sizes");
     R3_TRY(r3_reserve_t(c, &c->d_light_mats, &c->light_mats_cap, need_floats));
     float* prep = c->d_light_mats;
     DirPrep* d_dir = reinterpret_cast<DirPrep*>(prep);
     PointPrep* d_point = reinterpret_cast<PointPrep*>(prep + (size_t)c->n_dir * 32);
-    const uint32_t nl = c->n_dir > c->n_point ? c->n_dir : c->n_point;
+    const uint32_t nl = c->n_dir > c->point_capacity ? c->n_dir : c->point_capacity;
     if (nl) {
-        light_prep_kernel<<<(nl + 127) / 128, 128, 0, c->stream>>>(c->d_dir, c->n_dir, c->d_point, c->n_point, c->uniforms, d_dir, d_point);
+        light_prep_kernel<<<(nl + 127) / 128, 128, 0, c->stream>>>(c->d_dir, c->n_dir, c->d_point, c->uniforms, d_dir, d_point);
         R3_CHECK_LAUNCH(c, "light_prep_kernel");
     }
     ShadeParams p;
@@ -1027,6 +1037,7 @@ R3_EXPORT int r3_forward_resolve(r3_ctx* c) {
 R3_EXPORT int r3_forward_blend(r3_ctx* c) {
     if (!c || !c->d_vis) return r3_fail(c, R3_E_STATE, "forward_blend before set_render_target");
     if (!c->uniforms_set) return r3_fail(c, R3_E_STATE, "forward_blend before set_frame_uniforms");
+    if (c->point_eval_pending) return r3_fail(c, R3_E_STATE, "forward_blend: point lights set or updated since the last evaluate_point_lights");
     cudaSetDevice(c->device);
     bool ran = false;
     R3_TRY(r3_blend_collect(c, &ran));

@@ -135,6 +135,9 @@ DIRECTIONAL_LIGHT_DTYPE = _dt(
 
 POINT_LIGHT_DTYPE = _dt([("position", (f4, 4), 0), ("color", (f4, 3), 16), ("radius", f4, 28)], 32)
 
+# r3_point_light_source: rend3-types PointLight, one entry of PointLightManager's handle table (r3_set_point_light_sources)
+POINT_LIGHT_SOURCE_DTYPE = _dt([("position", (f4, 3), 0), ("color", (f4, 3), 12), ("radius", f4, 24), ("intensity", f4, 28)], 32)
+
 # r3_directional_light_source: a DirectionalLight plus its atlas placement (r3_set_directional_light_sources)
 LIGHT_SOURCE_DTYPE = _dt(
     [

@@ -109,10 +109,13 @@ class BaseRenderGraph:
         self.gpu_culler = GpuCuller(backend, max_compute_workgroups_per_dimension)
         self._resolution: Optional[Tuple[int, int]] = None
 
-    def upload_world(self, ev: EvalOutput, device_shadow_cameras: bool = False, movable_objects: bool = False):
+    def upload_world(self, ev: EvalOutput, device_shadow_cameras: bool = False, movable_objects: bool = False,
+                     device_point_lights: bool = False):
         """What evaluate_instructions leaves in wgpu buffers (renderer/eval.rs:157-181).  With `device_shadow_cameras` the lights go up
         as sources and atlas placements; the frame evaluates their shadow cameras on the device.  With `movable_objects` the mesh
-        bounding spheres go up too (r3_set_object_mesh_spheres), so that r3_set_object_transforms can move the objects."""
+        bounding spheres go up too (r3_set_object_mesh_spheres), so that r3_set_object_transforms can move the objects.  With
+        `device_point_lights` the point lights go up as PointLightManager's handle table (r3_set_point_light_sources); the frame
+        evaluates them on the device."""
         b = self.backend
         b.set_objects(ev.object_buffer)
         flags = (ev.object_live & 1) | ((ev.object_atomic & 1) << 1) | ((ev.object_back_to_front & 1) << 2)
@@ -129,14 +132,17 @@ class BaseRenderGraph:
             b.set_directional_light_sources(ev.directional_sources, ev.shadow_target_size[0], ev.shadow_target_size[1], ev.camera.handedness == LEFT)
         else:
             b.set_directional_lights(ev.directional_buffer, ev.shadow_target_size[0], ev.shadow_target_size[1])
-        b.set_point_lights(ev.point_buffer)
+        if device_point_lights:
+            b.set_point_light_sources(*ev.point_sources)
+        else:
+            b.set_point_lights(ev.point_buffer)
 
     def add_to_graph(self, ev: EvalOutput, resolution: Tuple[int, int], samples: int = 1,
                      settings: BaseRenderGraphSettings = BaseRenderGraphSettings(), srgb_target: bool = True,
                      upload: bool = True, scissor_rows: Optional[Tuple[int, int]] = None, shadow_filter=None, after_shadows=None,
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
-                     movable_objects: bool = False):
+                     movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -156,13 +162,18 @@ class BaseRenderGraph:
         `object_transforms` = (slots or None, matrices) moves objects at the skinning node, before `posed_objects`
         (Renderer::set_object_transform in bulk): CUDA tensors go through r3_set_object_transforms_device — enqueue only, their producer
         ordered on the context's stream — and host arrays through r3_set_object_transforms, which waits for the stream.  It needs the mesh
-        spheres: an uploading frame with `movable_objects` (or `object_transforms`) sends them."""
+        spheres: an uploading frame with `movable_objects` (or `object_transforms`) sends them.  `device_point_lights` uploads the point
+        lights as a handle table and evaluates them on the device right after the frame uniforms (r3_evaluate_point_lights, enqueue only);
+        `point_light_updates` = (handles, sources, live) adds, updates and removes handles first (PointLightManager::{add, update,
+        remove}): CUDA tensors through r3_update_point_light_sources_device — enqueue only, their producer ordered on the context's
+        stream — and host arrays through r3_update_point_light_sources, which waits for the stream."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
         b, culler = self.backend, self.gpu_culler
         if upload:
-            self.upload_world(ev, device_shadow_cameras, movable_objects or object_transforms is not None)
+            self.upload_world(ev, device_shadow_cameras, movable_objects or object_transforms is not None,
+                              device_point_lights or point_light_updates is not None)
         if self._resolution != (resolution, samples, tuple(settings.clear_color)):
             b.set_render_target(resolution[0], resolution[1], samples, settings.clear_color)
             self._resolution = (resolution, samples, tuple(settings.clear_color))
@@ -181,6 +192,14 @@ class BaseRenderGraph:
         b.set_frame_uniforms(frame_uniforms(ev.camera, settings.ambient_color, resolution))  # :142
         if device_shadow_cameras:                                                 # DirectionalLightManager::evaluate around this camera
             b.evaluate_shadow_cameras(ev.camera.location())
+        if point_light_updates is not None:                                       # PointLightManager::{add, update, remove}
+            handles, sources, live = point_light_updates
+            if getattr(handles, "is_cuda", False):
+                b.update_point_light_sources_device(handles, sources, live)
+            else:
+                b.update_point_light_sources(handles, sources, live)
+        if device_point_lights or point_light_updates is not None:                # PointLightManager::evaluate (renderer/eval.rs:180)
+            b.evaluate_point_lights()
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
         if object_transforms is not None:                                         # :145 objects the application moved this frame

@@ -54,6 +54,7 @@ from .layouts import (
     DIRECTIONAL_LIGHT_DTYPE,
     LIGHT_SOURCE_DTYPE,
     POINT_LIGHT_DTYPE,
+    POINT_LIGHT_SOURCE_DTYPE,
 )
 
 f32 = np.float32
@@ -542,6 +543,9 @@ class EvalOutput:
     # (capacity, 4) f32  InternalObject::mesh_bounding_sphere (object.rs:268-270) as (centre, radius), zeros for empty slots: what
     # r3_set_object_mesh_spheres takes so that r3_set_object_transforms can move the objects on the device
     object_mesh_sphere: Optional[np.ndarray] = None
+    # PointLightManager's handle table behind point_buffer: (POINT_LIGHT_SOURCE_DTYPE[n_handles], u8 live[n_handles]), dead handles
+    # zero records — what r3_set_point_light_sources takes so that the device evaluates the lights
+    point_sources: Optional[Tuple[np.ndarray, np.ndarray]] = None
 
 
 class Renderer:
@@ -683,6 +687,19 @@ class Renderer:
         self.point_lights.append(light)
         return len(self.point_lights) - 1
 
+    def update_point_light(self, handle: int, light: PointLight):
+        """data[handle] = Some(light) (PointLightManager::update, point.rs); a handle at or beyond the table's size grows it as add's
+        resize does, the handles between staying None."""
+        if handle >= len(self.point_lights):
+            self.point_lights.extend([None] * (handle + 1 - len(self.point_lights)))
+        self.point_lights[handle] = light
+
+    def remove_point_light(self, handle: int):
+        """data[handle] = None (PointLightManager::remove, point.rs), growing the table like update_point_light."""
+        if handle >= len(self.point_lights):
+            self.point_lights.extend([None] * (handle + 1 - len(self.point_lights)))
+        self.point_lights[handle] = None
+
     def set_camera_data(self, camera: Camera):
         self.camera = CameraState(camera, self.handedness, self.aspect_ratio)
 
@@ -767,6 +784,12 @@ class Renderer:
             pl[k]["color"] = np.asarray(l.color, dtype=f32) * f32(l.intensity)
             pl[k]["radius"] = l.radius
         pbytes = np.array([len(pl), 0, 0, 0], dtype=np.uint32).tobytes() + pl.tobytes()
+        psrc = np.zeros(len(self.point_lights), dtype=POINT_LIGHT_SOURCE_DTYPE)
+        plive = np.zeros(len(self.point_lights), dtype=np.uint8)
+        for h, l in enumerate(self.point_lights):
+            if l is not None:
+                psrc[h] = (l.position, l.color, l.radius, l.intensity)
+                plive[h] = 1
 
         tex_descs, tex_blob = self._texture_table()
         sky_desc, sky_blob = self._skybox_blob()
@@ -786,6 +809,7 @@ class Renderer:
             directional_buffer=dbytes,
             directional_sources=src,
             point_buffer=pbytes,
+            point_sources=(psrc, plive),
             shadows=shadows,
             shadow_target_size=size,
             camera=self.camera,
