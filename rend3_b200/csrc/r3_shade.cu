@@ -83,43 +83,76 @@ __device__ __forceinline__ float3 surface_shading(const float3 l, const float3 i
 }
 
 // shadow_sample_pcf5 (shadow/pcf.wgsl:1-9): five textureSampleCompareLevel taps (centre, +-1 texel in x and y) with the
-// linear, GreaterEqual, Repeat-addressed comparison sampler (common/samplers.rs:24,42-56).  All taps share the same
-// bilinear fractions, so the 20 texel compares collapse to the 12 distinct texels of a 4x4 neighbourhood without corners.
+// linear, GreaterEqual, Repeat-addressed comparison sampler (common/samplers.rs:24,42-56), in the oracle's rounding: each tap
+// takes its own coordinate (u * W + offset) - 0.5, bilinear weights lerp the 0/1 compares, and the taps are summed in source order.
+// One footprint shared by the five taps is not the same: next to a power of two u * W + 1 or u * W - 1 rounds where u * W does not,
+// and that tap's fraction moves by an ulp.  So each axis keeps the three coordinates of its offsets -1, 0, +1.
 __device__ __forceinline__ int wrap_texel(int i, int n) {
     if ((unsigned)i < (unsigned)n) return i;   // common case: no division
     const int m = i % n;
     return m < 0 ? m + n : m;
 }
+struct TapAxis { int i[3]; float f[3]; };   // floor and fraction of (u * n + o) - 0.5 for the offsets o = -1, 0, +1
+__device__ __forceinline__ TapAxis tap_axis(float u, uint32_t n) {
+    const float un = mul_rn(u, (float)n);
+    TapAxis a;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float x = sub_rn(add_rn(un, (float)(k - 1)), 0.5f), fl = floorf(x);
+        a.f[k] = sub_rn(x, fl);
+        // clamp before the int conversion: coordinates far outside the atlas only arise for fragments outside the light volume
+        a.i[k] = (int)fminf(fmaxf(fl, -1.0e9f), 1.0e9f);
+    }
+    return a;
+}
+// one tap: (c00 * (1 - fx) + c10 * fx) * (1 - fy) + (c01 * (1 - fx) + c11 * fx) * fy
+__device__ __forceinline__ float bilinear_rn(float c00, float c10, float c01, float c11, float fx, float fy) {
+    const float gx = sub_rn(1.0f, fx);
+    return add_rn(mul_rn(add_rn(mul_rn(c00, gx), mul_rn(c10, fx)), sub_rn(1.0f, fy)), mul_rn(add_rn(mul_rn(c01, gx), mul_rn(c11, fx)), fy));
+}
+__device__ __forceinline__ float texel_ge(const ShadeParams& p, float ref, int x, int y) {
+    return ref >= __ldg(&p.atlas[(size_t)y * p.atlas_w + x]) ? 1.0f : 0.0f;
+}
+// the taps at offsets (0,0), (0,1), (0,-1), (1,0), (-1,0), summed in that order, times 0.2
+__device__ __forceinline__ float pcf5_sum(float centre, float up, float down, float right, float left) {
+    return mul_rn(add_rn(add_rn(add_rn(add_rn(centre, up), down), right), left), 0.2f);
+}
+// the general case: every tap reads its own four texels
+__device__ __noinline__ float shadow_pcf5_taps(const ShadeParams& p, const TapAxis ax, const TapAxis ay, float ref) {
+    const int W = (int)p.atlas_w, H = (int)p.atlas_h;
+    const int ox[5] = {0, 0, 0, 1, -1}, oy[5] = {0, 1, -1, 0, 0};
+    float t[5];
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        const int a = ox[k] + 1, b = oy[k] + 1;
+        const int x0 = wrap_texel(ax.i[a], W), x1 = wrap_texel(ax.i[a] + 1, W), y0 = wrap_texel(ay.i[b], H), y1 = wrap_texel(ay.i[b] + 1, H);
+        t[k] = bilinear_rn(texel_ge(p, ref, x0, y0), texel_ge(p, ref, x1, y0), texel_ge(p, ref, x0, y1), texel_ge(p, ref, x1, y1), ax.f[a], ay.f[b]);
+    }
+    return pcf5_sum(t[0], t[1], t[2], t[3], t[4]);
+}
 __device__ __forceinline__ float shadow_pcf5(const ShadeParams& p, float u, float v, float ref) {
-    const float x = u * (float)p.atlas_w - 0.5f, y = v * (float)p.atlas_h - 0.5f;
-    const float fx0 = floorf(x), fy0 = floorf(y), fx = x - fx0, fy = y - fy0;
-    // clamp before the int conversion: coordinates far outside the atlas only arise for fragments outside the light volume
-    const int ix = (int)fminf(fmaxf(fx0, -1.0e9f), 1.0e9f), iy = (int)fminf(fmaxf(fy0, -1.0e9f), 1.0e9f);
+    const TapAxis ax = tap_axis(u, p.atlas_w), ay = tap_axis(v, p.atlas_h);
+    // almost always the offsets -1 and +1 land one texel either side of the centre tap's floor: then the 20 compares are the 12
+    // distinct texels of a 4x4 neighbourhood without corners (each tap still with its own fractions)
+    if (ax.i[0] != ax.i[1] - 1 || ax.i[2] != ax.i[1] + 1 || ay.i[0] != ay.i[1] - 1 || ay.i[2] != ay.i[1] + 1) return shadow_pcf5_taps(p, ax, ay, ref);
     const int W = (int)p.atlas_w, H = (int)p.atlas_h;
     int xs[4], ys[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) { xs[k] = wrap_texel(ix - 1 + k, W); ys[k] = wrap_texel(iy - 1 + k, H); }
+    for (int k = 0; k < 4; ++k) { xs[k] = wrap_texel(ax.i[1] - 1 + k, W); ys[k] = wrap_texel(ay.i[1] - 1 + k, H); }
     float c[4][4];   // c[row][col] = ref >= texel ? 1 : 0
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             const bool corner = (r == 0 || r == 3) && (q == 0 || q == 3);
-            c[r][q] = (!corner && ref >= __ldg(&p.atlas[(size_t)ys[r] * W + xs[q]])) ? 1.0f : 0.0f;
+            c[r][q] = corner ? 0.0f : texel_ge(p, ref, xs[q], ys[r]);
         }
-    const float gx = 1.0f - fx, gy = 1.0f - fy;
-    // bilinear(tap at texel offset (a, b)) = (c[b][a]*gx + c[b][a+1]*fx)*gy + (c[b+1][a]*gx + c[b+1][a+1]*fx)*fy, offsets re-based by +1
-    float h[4][3];   // horizontal lerps h[row][a] = c[row][a]*gx + c[row][a+1]*fx
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int a = 0; a < 3; ++a) h[r][a] = c[r][a] * gx + c[r][a + 1] * fx;
-    const float centre = h[1][1] * gy + h[2][1] * fy;
-    const float up = h[2][1] * gy + h[3][1] * fy;      // offset (0, +1)
-    const float down = h[0][1] * gy + h[1][1] * fy;    // offset (0, -1)
-    const float right = h[1][2] * gy + h[2][2] * fy;   // offset (+1, 0)
-    const float left = h[1][0] * gy + h[2][0] * fy;    // offset (-1, 0)
-    return ((((centre + up) + down) + right) + left) * 0.2f;
+    const float centre = bilinear_rn(c[1][1], c[1][2], c[2][1], c[2][2], ax.f[1], ay.f[1]);
+    const float up = bilinear_rn(c[2][1], c[2][2], c[3][1], c[3][2], ax.f[1], ay.f[2]);
+    const float down = bilinear_rn(c[0][1], c[0][2], c[1][1], c[1][2], ax.f[1], ay.f[0]);
+    const float right = bilinear_rn(c[1][2], c[1][3], c[2][2], c[2][3], ax.f[2], ay.f[1]);
+    const float left = bilinear_rn(c[1][0], c[1][1], c[2][0], c[2][1], ax.f[0], ay.f[1]);
+    return pcf5_sum(centre, up, down, right, left);
 }
 
 // one perspective weight numerator of raster rule R6, oracle order: ((c.x * nx + c.y * ny) + c.z) with c = cross(a, b) over (x, y, w)
@@ -164,7 +197,9 @@ __device__ __forceinline__ FragIn fragment_inputs(const ShadeParams& p, const r3
     // R6: perspective-correct weights b_i ~ cross(p_j, p_k) . (ndc_x, ndc_y, 1)
     const float nx = sub_rn(div_rn((float)px + 0.5f, (float)p.width * 0.5f), 1.0f), ny = sub_rn(1.0f, div_rn((float)py + 0.5f, (float)p.height * 0.5f));
     // The chain b_i -> view_position -> shadow-space depth feeds the (discontinuous) shadow compare, so it is evaluated in
-    // source order without contraction, exactly like the oracle; everything downstream of the compare is continuous.
+    // source order without contraction, exactly like the oracle; so is the rest of the shadow lookup (shade_inputs: region bounds,
+    // atlas-coordinate mix; shadow_pcf5: per-tap coordinates, bilinear weights, tap sum), which makes the shadow factor the oracle's
+    // bit for bit.  Everything downstream of the lookup is continuous.
     float b0 = cross_term_rn(p1, p2, nx, ny), b1 = cross_term_rn(p2, p0, nx, ny), b2 = cross_term_rn(p0, p1, nx, ny);
     const float bsum = add_rn(add_rn(b0, b1), b2);
     b0 = div_rn(b0, bsum); b1 = div_rn(b1, bsum); b2 = div_rn(b2, bsum);
@@ -435,11 +470,11 @@ __device__ __forceinline__ float4 shade_inputs(const ShadeParams& p, const DirPr
             const DirPrep& L = i < MAX_SMEM_DIR ? s_dir[i] : p.dir[i];
             const float4 sn = mat_vec_rn(L.lm, vp.x, vp.y, vp.z, vp.w);
             const float snx = sn.x, sny = sn.y, snz = sn.z;
-            const float flx = add_rn(mul_rn(snx, 0.5f), 0.5f), fly = add_rn(mul_rn(sny, 0.5f), 0.5f), locy = 1.0f - fly;
-            float tlx = L.offset[0], tly = L.offset[1], trx = tlx + L.size[0], try_ = tly + L.size[1];
-            const float cu = tlx * (1.0f - flx) + trx * flx, cv = tly * (1.0f - locy) + try_ * locy;
-            const float bx = L.inv_res[0] * 1.5f, by = L.inv_res[1] * 1.5f;
-            tlx += bx; tly += by; trx -= bx; try_ -= by;
+            const float flx = add_rn(mul_rn(snx, 0.5f), 0.5f), fly = add_rn(mul_rn(sny, 0.5f), 0.5f), locy = sub_rn(1.0f, fly);
+            float tlx = L.offset[0], tly = L.offset[1], trx = add_rn(tlx, L.size[0]), try_ = add_rn(tly, L.size[1]);
+            const float cu = add_rn(mul_rn(tlx, sub_rn(1.0f, flx)), mul_rn(trx, flx)), cv = add_rn(mul_rn(tly, sub_rn(1.0f, locy)), mul_rn(try_, locy));   // mix
+            const float bx = mul_rn(L.inv_res[0], 1.5f), by = mul_rn(L.inv_res[1], 1.5f);
+            tlx = add_rn(tlx, bx); tly = add_rn(tly, by); trx = sub_rn(trx, bx); try_ = sub_rn(try_, by);
             float shadow = 1.0f;
             if ((flx >= tlx || fly >= tly) && (flx <= trx || fly <= try_) && snz >= 0.0f && snz <= 1.0f)   // literal any() quirk (opaque.wgsl:509-514)
                 shadow = shadow_pcf5(p, cu, cv, snz);
