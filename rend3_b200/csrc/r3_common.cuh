@@ -106,8 +106,10 @@ struct r3_ctx {
     // world
     r3_object* d_objects = nullptr; uint32_t n_slots = 0, objects_cap = 0; bool objects_borrowed = false;
     // dense copies of the fields the cull + bake stream reads (r3_cull_bake.cu): transform rows 0-2 (3 float4 per slot), transform row 3,
-    // bounding spheres, enabled bits, affine bits (row 3 is exactly (+0, +0, +0, 1))
+    // bounding spheres, enabled bits, affine bits (row 3 is exactly (+0, +0, +0, 1)), sphere radii, centre bits (the sphere's centre is
+    // exactly the transform's translation column)
     float4* d_hot_xyz = nullptr; float4* d_hot_w = nullptr; float4* d_hot_sphere = nullptr; uint32_t* d_enabled_bits = nullptr; uint32_t* d_affine_bits = nullptr;
+    float* d_hot_radius = nullptr; uint32_t* d_centre_bits = nullptr;
     uint64_t hot_cap = 0; bool hot_valid = false;
     std::vector<uint64_t> sort_key; std::vector<uint8_t> sort_flags; std::vector<float> sort_loc;
     uint32_t* d_live_bits = nullptr; uint32_t live_bits_cap = 0; bool have_live = false;
@@ -223,7 +225,7 @@ int r3_split_objects(r3_ctx* c);
 int r3_split_slots(r3_ctx* c, const uint32_t* d_slots, uint32_t n);
 int r3_grow_hot(r3_ctx* c, uint32_t old_n, uint32_t n);   // r3_resize_objects: keep the hot copies of slots < old_n, zero slots [old_n, n)
 uint64_t r3_hot_capacity(uint64_t want);                    // slots the hot arrays (and a grown object buffer) are allocated for
-int r3_launch_mask_word(r3_ctx* c, uint32_t* word_a, uint32_t* word_b, uint32_t keep_mask);   // *word &= keep_mask (either may be null)
+int r3_launch_mask_word(r3_ctx* c, uint32_t* word_a, uint32_t* word_b, uint32_t* word_c, uint32_t keep_mask);   // *word &= keep_mask (any may be null)
 int r3_launch_triangle_cull(r3_ctx* c, r3_camera* cam);
 int r3_host_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], uint32_t max_dispatch_count);
 int r3_upload_jobs(r3_ctx* c, r3_camera* cam);
@@ -252,6 +254,11 @@ int r3_reserve_point_buffer(r3_ctx* c, uint32_t n_lights);   // r3_lights.cu: ro
 // Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine
 // (a product with -0.0 can carry its sign into MV / MVP).
 __device__ __forceinline__ uint32_t affine_w_bits(uint32_t j) { return j == 3 ? 0x3f800000u : 0u; }
+// The centre bit of a slot: its bounding sphere's centre has the bit patterns of the translation column (elements .w of rows 0-2), so
+// the cull can take the centre from the transform it already holds.  Bits, not floats: -0.0 against +0.0 or two NaN payloads differ.
+__device__ __forceinline__ bool centre_is_translation(float cx, float cy, float cz, float tx, float ty, float tz) {
+    return __float_as_uint(cx) == __float_as_uint(tx) && __float_as_uint(cy) == __float_as_uint(ty) && __float_as_uint(cz) == __float_as_uint(tz);
+}
 // IEEE, never-contracted arithmetic for the bit-exact stages (SURVEY D7)
 __device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }

@@ -81,7 +81,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     r3_peer_destroy(c);
     r3_anim_destroy(c);
     if (!c->objects_borrowed) cudaFree(c->d_objects);
-    cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
+    cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_hot_radius); cudaFree(c->d_centre_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
     cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc); cudaFree(c->d_gsort_keys[0]); cudaFree(c->d_gsort_keys[1]); cudaFree(c->d_gsort_hist); cudaFree(c->d_gsort_header);
     cudaFree(c->d_mesh_spheres); cudaFree(c->d_live_bits); cudaFree(c->d_mesh); cudaFree(c->d_materials); cudaFree(c->d_dir); cudaFree(c->d_point);
     cudaFree(c->d_light_mats); cudaFree(c->d_atlas); cudaFree(c->d_light_src); cudaFree(c->d_shadow_cams); cudaFree(c->d_point_src); cudaFree(c->d_point_live);
@@ -538,7 +538,7 @@ R3_EXPORT int r3_resize_objects(r3_ctx* c, uint32_t n) {
         R3_TRY(r3_reserve_t(c, &c->d_live_bits, &c->live_bits_cap, words, true));
         const uint32_t whole = (sorted & 31u) ? old_words : (uint32_t)(sorted / 32);
         if (words > whole) R3_CUDA(c, cudaMemsetAsync(c->d_live_bits + whole, 0, (size_t)(words - whole) * 4, c->stream));
-        if (sorted & 31u) R3_TRY(r3_launch_mask_word(c, c->d_live_bits + sorted / 32, nullptr, (1u << (sorted & 31u)) - 1u));
+        if (sorted & 31u) R3_TRY(r3_launch_mask_word(c, c->d_live_bits + sorted / 32, nullptr, nullptr, (1u << (sorted & 31u)) - 1u));
         if (n > c->sort_dev_cap || !c->d_sort_key8) {
             const uint32_t cap = (uint32_t)r3_hot_capacity(n);
             uint8_t* k8 = nullptr; float* l = nullptr;

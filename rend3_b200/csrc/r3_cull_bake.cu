@@ -7,17 +7,21 @@
 //       Frustum::contains_sphere, 5 planes        rend3/src/util/frustum.rs:148-161
 // and emits the visible slots as one ASCENDING u32 list (the canonical, bit-exact artefact).
 //
-// Design (HBM-bound: 224 flop against 212 algorithmic bytes per object — 84 read + 128 written; on affine transforms the
-// kernel reads 16 B less, 196 B per object by the same count).
+// Design (HBM-bound: 224 flop against 212 algorithmic bytes per object — 84 read + 128 written; on affine transforms whose
+// sphere centre is the translation the kernel reads 52 B + 3 bits, 184 B per object by the same count).
 //   hot/cold split — the reference's 128-byte Object record (object.rs:23-36) stays the canonical store for the kernels
 //     that need its cold fields (first_index, index_count, material, attribute offsets); the fields this path reads
 //     (transform, bounding sphere, enabled) are ALSO kept as dense arrays — rows_xyz[3n] float4 (rows 0-2 of the
-//     transform, row r of slot o at 3o + r), rows_w[n] float4 (row 3), spheres[n] float4, enabled and affine 1 bit per
-//     slot — filled by split_objects_kernel whenever records are uploaded (r3_set_objects, r3_set_objects_device) and by
-//     split_slots_kernel when they are scattered (r3_update_objects).  The affine bit is set when row 3 has exactly the
-//     bit patterns (+0, +0, +0, 1); rows_w is then never read, because the kernel substitutes those constants.  With the
-//     AoS records every 32-byte sector of a record is touched, i.e. 128 B read per object; the dense arrays bring that
-//     to 64 B + 2 bits for affine transforms, 80 B + 2 bits otherwise (and to 16 B + 1 bit for cull-only).
+//     transform, row r of slot o at 3o + r), rows_w[n] float4 (row 3), spheres[n] float4, radii[n] float, enabled, affine
+//     and centre 1 bit per slot — filled by split_objects_kernel whenever records are uploaded (r3_set_objects,
+//     r3_set_objects_device), by split_slots_kernel when they are scattered (r3_update_objects, the animation posing) and by
+//     object_transforms_kernel when objects move (r3_set_object_transforms).  The affine bit is set when row 3 has exactly the
+//     bit patterns (+0, +0, +0, 1); rows_w is then never read, because the kernel substitutes those constants.  The centre bit
+//     is set when the sphere's centre has exactly the bit patterns of the translation (elements .w of rows 0-2) — true of every
+//     world sphere made from a mesh sphere centred at the mesh origin; the cull then takes the centre from the transform tile
+//     and reads 4 B of radii instead of 16 B of spheres.  With the AoS records every 32-byte sector of a record is touched,
+//     i.e. 128 B read per object; the dense arrays bring that to 52 B + 3 bits for affine, centred slots, 64 B + 3 bits for
+//     affine ones with another centre, 80 B + 3 bits at most (and to 16 B + 1 bit for cull-only, which always reads spheres).
 //   stream kernel  — no inter-CTA dependency:
 //     * a warp owns 32 consecutive slots.  Three fully coalesced 512-byte loads fetch rows 0-2 of their transforms and
 //       a transpose through the warp's 1536 bytes of shared memory hands the lane of (slot o, column j) that column; row
@@ -25,8 +29,10 @@
 //       by `view_proj` (operands straight from the constant bank) and stores column j of MV and of MVP — 64-byte runs,
 //       whole sectors.  Arithmetic is __fmul_rn/__fadd_rn in WGSL's accumulation order, never contracted: MV/MVP are
 //       bit-identical to the CPU oracle;
-//     * lane l loads the sphere of slot base+l (one coalesced 512-byte load) and tests it; the ballot IS the 32-bit
-//       visibility word of the 32 slots (1 bit per object goes to HBM);
+//     * lane l tests the sphere of slot base+l: with the centre bit, the centre is column 3 of the slot's tile in shared memory
+//       and the radius one float of radii; without it, the lane loads the sphere.  The loads are predicated per lane, so a tile
+//       of centred slots touches one 128-byte run of radii and none of spheres.  The ballot IS the 32-bit visibility word of
+//       the 32 slots (1 bit per object goes to HBM);
 //     * each CTA (1024 slots) also leaves its survivor count.
 //   compact kernel — one CTA per 32768 objects: sums the CTA counts in front of it (<= 40 KB, L2 resident),
 //     scans its 1024 visibility words and writes the surviving slot ids in ascending order.  It moves
@@ -64,13 +70,15 @@ constexpr int CAM_FLOATS = 52;   // view[16] | view_proj[16] | frustum[5][4], st
 
 // AoS Object records -> the dense hot arrays.  8 lanes per 128-byte record (coalesced 512-byte loads); float4 #0-3 =
 // transform columns, #4 = bounding sphere, #7.y = `enabled` (byte 116).  Lane k < 4 holds column k and scatters it into
-// element k of rows 0-2 (rows_xyz) and of row 3 (rows_w).
+// element k of rows 0-2 (rows_xyz) and of row 3 (rows_w); lane 4 stores the sphere and its radius and, with column 3 shuffled
+// over from lane 3, decides the centre bit.
 __global__ void __launch_bounds__(256) split_objects_kernel(const float4* __restrict__ objects, uint32_t n, float* __restrict__ rows_xyz, float* __restrict__ rows_w,
-                                                            float4* __restrict__ spheres, uint32_t* __restrict__ enabled_bits, uint32_t* __restrict__ affine_bits) {
+                                                            float4* __restrict__ spheres, float* __restrict__ radii, uint32_t* __restrict__ enabled_bits,
+                                                            uint32_t* __restrict__ affine_bits, uint32_t* __restrict__ centre_bits) {
     const int lane = threadIdx.x & 31, k = lane & 7, g = lane >> 3;
     const uint32_t wtile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, base = wtile * 32u;
     if (base >= n) return;
-    uint32_t bits = 0, abits = 0;
+    uint32_t bits = 0, abits = 0, cbits = 0;
 #pragma unroll
     for (int it = 0; it < 8; ++it) {
         const uint32_t obj = base + it * 4 + g;
@@ -81,20 +89,23 @@ __global__ void __launch_bounds__(256) split_objects_kernel(const float4* __rest
                 float* xyz = rows_xyz + (size_t)obj * 12 + k;
                 xyz[0] = r.x; xyz[4] = r.y; xyz[8] = r.z;
                 rows_w[(size_t)obj * 4 + k] = r.w;
-            } else if (k == 4) spheres[obj] = r;
+            } else if (k == 4) { spheres[obj] = r; radii[obj] = r.w; }
         }
         const uint32_t b = __ballot_sync(0xFFFFFFFFu, k == 7 && obj < n && __float_as_uint(r.y) != 0u);   // lanes 7, 15, 23, 31
         bits |= (((b >> 7) & 1u) | (((b >> 15) & 1u) << 1) | (((b >> 23) & 1u) << 2) | (((b >> 31) & 1u) << 3)) << (it * 4);
         const uint32_t a = __ballot_sync(0xFFFFFFFFu, k < 4 && obj < n && __float_as_uint(r.w) == affine_w_bits(k));   // lanes 0-3 of each record
 #pragma unroll
         for (int q = 0; q < 4; ++q) abits |= (((a >> (8 * q)) & 0xFu) == 0xFu ? 1u : 0u) << (it * 4 + q);
+        const float tx = __shfl_up_sync(0xFFFFFFFFu, r.x, 1), ty = __shfl_up_sync(0xFFFFFFFFu, r.y, 1), tz = __shfl_up_sync(0xFFFFFFFFu, r.z, 1);   // column 3
+        const uint32_t cb = __ballot_sync(0xFFFFFFFFu, k == 4 && obj < n && centre_is_translation(r.x, r.y, r.z, tx, ty, tz));   // lanes 4, 12, 20, 28
+        cbits |= (((cb >> 4) & 1u) | (((cb >> 12) & 1u) << 1) | (((cb >> 20) & 1u) << 2) | (((cb >> 28) & 1u) << 3)) << (it * 4);
     }
-    if (lane == 0) { enabled_bits[wtile] = bits; affine_bits[wtile] = abits; }
+    if (lane == 0) { enabled_bits[wtile] = bits; affine_bits[wtile] = abits; centre_bits[wtile] = cbits; }
 }
 // the same for the records r3_update_objects has just scattered (ScatterCopy, util/scatter_copy.rs:69-136)
 __global__ void __launch_bounds__(256) split_slots_kernel(const float4* __restrict__ objects, const uint32_t* __restrict__ slots, uint32_t n_updates, uint32_t n_slots,
-                                                          float* __restrict__ rows_xyz, float* __restrict__ rows_w, float4* __restrict__ spheres,
-                                                          uint32_t* __restrict__ enabled_bits, uint32_t* __restrict__ affine_bits) {
+                                                          float* __restrict__ rows_xyz, float* __restrict__ rows_w, float4* __restrict__ spheres, float* __restrict__ radii,
+                                                          uint32_t* __restrict__ enabled_bits, uint32_t* __restrict__ affine_bits, uint32_t* __restrict__ centre_bits) {
     const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3, k = threadIdx.x & 7;
     const uint32_t s = i < n_updates ? slots[i] : n_slots;
     const bool ok = s < n_slots;
@@ -105,23 +116,27 @@ __global__ void __launch_bounds__(256) split_slots_kernel(const float4* __restri
             float* xyz = rows_xyz + (size_t)s * 12 + k;
             xyz[0] = r.x; xyz[4] = r.y; xyz[8] = r.z;
             rows_w[(size_t)s * 4 + k] = r.w;
-        } else if (k == 4) spheres[s] = r;
+        } else if (k == 4) { spheres[s] = r; radii[s] = r.w; }
     }
     // the 8 lanes of a record share i and s; the grid is whole warps
     const uint32_t a = __ballot_sync(0xFFFFFFFFu, ok && k < 4 && __float_as_uint(r.w) == affine_w_bits(k));
+    const float tx = __shfl_up_sync(0xFFFFFFFFu, r.x, 1), ty = __shfl_up_sync(0xFFFFFFFFu, r.y, 1), tz = __shfl_up_sync(0xFFFFFFFFu, r.z, 1);   // column 3
+    const uint32_t cb = __ballot_sync(0xFFFFFFFFu, ok && k == 4 && centre_is_translation(r.x, r.y, r.z, tx, ty, tz));
     if (ok && k == 7) {
         const uint32_t bit = 1u << (s & 31u);
         if (__float_as_uint(r.y) != 0u) atomicOr(&enabled_bits[s >> 5], bit);
         else atomicAnd(&enabled_bits[s >> 5], ~bit);
         if (((a >> (threadIdx.x & 24u)) & 0xFu) == 0xFu) atomicOr(&affine_bits[s >> 5], bit);
         else atomicAnd(&affine_bits[s >> 5], ~bit);
+        if ((cb >> ((threadIdx.x & 24u) + 4u)) & 1u) atomicOr(&centre_bits[s >> 5], bit);
+        else atomicAnd(&centre_bits[s >> 5], ~bit);
     }
 }
 
 template <bool BAKE, bool CULL, bool LIVE, typename Params = CullBakeParams>
 __global__ void __launch_bounds__(CB_THREADS)
 cull_bake_kernel(const float4* __restrict__ rows_xyz, const float* __restrict__ rows_w, const uint32_t* __restrict__ affine_bits, const float4* __restrict__ spheres,
-                 const uint32_t* __restrict__ enabled_bits, const uint32_t* __restrict__ live_bits, float4* __restrict__ matrices, uint32_t* __restrict__ words,
+                 const float* __restrict__ radii, const uint32_t* __restrict__ centre_bits, const uint32_t* __restrict__ enabled_bits, const uint32_t* __restrict__ live_bits, float4* __restrict__ matrices, uint32_t* __restrict__ words,
                  uint32_t* __restrict__ cta_counts, const __grid_constant__ Params p) {
     __shared__ uint32_t s_count[CB_WARPS];
     __shared__ float4 s_rows[BAKE ? CB_WARPS : 1][96];   // per warp: rows 0-2 of its 32 slots
@@ -148,7 +163,8 @@ cull_bake_kernel(const float4* __restrict__ rows_xyz, const float* __restrict__ 
         if (base >= p.object_count) break;
         float4 t[3];
         float4 sp = make_float4(0.f, 0.f, 0.f, 0.f);
-        uint32_t enabled = 0u, affine = 0u;
+        uint32_t enabled = 0u, affine = 0u, centred = 0u;
+        if (BAKE && CULL) centred = __ldg(&centre_bits[wtile]);
         if (BAKE) {
 #pragma unroll
             for (int q = 0; q < 3; ++q) {
@@ -156,7 +172,13 @@ cull_bake_kernel(const float4* __restrict__ rows_xyz, const float* __restrict__ 
                 t[q] = base + e / 3u < p.object_count ? __ldcs(&rows_xyz[(size_t)base * 3 + e]) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
         }
-        if (CULL && base + lane < p.object_count) sp = __ldcs(&spheres[base + lane]);
+        // a centred slot's sphere is its translation and the radius: the lane loads 4 B of radii instead of 16 B of spheres (per lane,
+        // so a warp only touches the sectors of the array its lanes need)
+        const bool centre_from_tile = BAKE && CULL && ((centred >> lane) & 1u);
+        if (CULL && base + lane < p.object_count) {
+            if (centre_from_tile) sp.w = __ldcs(&radii[base + lane]);
+            else sp = __ldcs(&spheres[base + lane]);
+        }
         if (BAKE || (CULL && !LIVE)) enabled = __ldg(&enabled_bits[wtile]);
         if (BAKE) affine = __ldg(&affine_bits[wtile]);
         if (BAKE) {
@@ -184,6 +206,12 @@ cull_bake_kernel(const float4* __restrict__ rows_xyz, const float* __restrict__ 
         if (CULL) {
             // one object per lane: Plane::distance = abc.dot(center) + d with glam's scalar dot order (util/frustum.rs:79-81,148-161)
             const uint32_t live = LIVE ? __ldg(&live_bits[wtile]) : enabled;
+            if constexpr (BAKE) {
+                if (centre_from_tile) {   // elements .w of rows 0-2 in the transposed tile (zeros past object_count, where the ballot drops the lane)
+                    const float* tr = reinterpret_cast<const float*>(s_rows[warp]) + lane * 12 + 3;
+                    sp.x = tr[0]; sp.y = tr[4]; sp.z = tr[8];
+                }
+            }
             const float neg_radius = -sp.w;
             bool inside = true;
 #pragma unroll
@@ -382,7 +410,7 @@ static int launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode, const r3_c
     const bool live = c->have_live && cull && c->sort_flags.size() >= (size_t)n;
 #define R3_CB_LAUNCH(B, C, L) \
     cull_bake_kernel<B, C, L><<<n_ctas, CB_THREADS, 0, c->stream>>>(c->d_hot_xyz, reinterpret_cast<const float*>(c->d_hot_w), c->d_affine_bits, c->d_hot_sphere, \
-                                                                    c->d_enabled_bits, c->d_live_bits, mats, words, cta_counts, p)
+                                                                    c->d_hot_radius, c->d_centre_bits, c->d_enabled_bits, c->d_live_bits, mats, words, cta_counts, p)
     r3_stage_begin(c, R3_STAGE_CULL_BAKE);
     if (d_header) {
         // without a live mask the kernel's `live` word is the enabled word, so the LIVE instantiations read the enabled bits instead
@@ -390,7 +418,8 @@ static int launch_cull_bake(r3_ctx* c, r3_camera* cam, uint32_t mode, const r3_c
         const uint32_t* live_bits = live ? c->d_live_bits : c->d_enabled_bits;
 #define R3_CB_DEV_LAUNCH(B, C)                                                                                                                       \
     cull_bake_kernel<B, C, C, DeviceCameraParams><<<n_ctas, CB_THREADS, 0, c->stream>>>(c->d_hot_xyz, reinterpret_cast<const float*>(c->d_hot_w),     \
-                                                                                      c->d_affine_bits, c->d_hot_sphere, c->d_enabled_bits, live_bits, \
+                                                                                      c->d_affine_bits, c->d_hot_sphere, c->d_hot_radius, c->d_centre_bits, \
+                                                                                      c->d_enabled_bits, live_bits, \
                                                                                       mats, words, cta_counts, dp)
         if (bake && cull) R3_CB_DEV_LAUNCH(true, true);
         else if (bake) R3_CB_DEV_LAUNCH(true, false);
@@ -449,19 +478,24 @@ int r3_split_objects(r3_ctx* c) {
     const uint64_t want = n ? n : 1;
     if (want > c->hot_cap) {
         cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits);
-        c->d_hot_xyz = nullptr; c->d_hot_w = nullptr; c->d_hot_sphere = nullptr; c->d_enabled_bits = nullptr; c->d_affine_bits = nullptr; c->hot_cap = 0;
+        cudaFree(c->d_hot_radius); cudaFree(c->d_centre_bits);
+        c->d_hot_xyz = nullptr; c->d_hot_w = nullptr; c->d_hot_sphere = nullptr; c->d_enabled_bits = nullptr; c->d_affine_bits = nullptr;
+        c->d_hot_radius = nullptr; c->d_centre_bits = nullptr; c->hot_cap = 0;
         const uint64_t cap = r3_hot_capacity(want);
         R3_CUDA(c, cudaMalloc((void**)&c->d_hot_xyz, cap * 48));
         R3_CUDA(c, cudaMalloc((void**)&c->d_hot_w, cap * 16));
         R3_CUDA(c, cudaMalloc((void**)&c->d_hot_sphere, cap * 16));
+        R3_CUDA(c, cudaMalloc((void**)&c->d_hot_radius, cap * 4));
         R3_CUDA(c, cudaMalloc((void**)&c->d_enabled_bits, ((cap + 31) / 32 + 1) * 4));
         R3_CUDA(c, cudaMalloc((void**)&c->d_affine_bits, ((cap + 31) / 32 + 1) * 4));
+        R3_CUDA(c, cudaMalloc((void**)&c->d_centre_bits, ((cap + 31) / 32 + 1) * 4));
         c->hot_cap = cap;
     }
     if (n) {
         const uint32_t warps = (n + 31) / 32;
         split_objects_kernel<<<(warps + 7) / 8, 256, 0, c->stream>>>(reinterpret_cast<const float4*>(c->d_objects), n, reinterpret_cast<float*>(c->d_hot_xyz),
-                                                                      reinterpret_cast<float*>(c->d_hot_w), c->d_hot_sphere, c->d_enabled_bits, c->d_affine_bits);
+                                                                      reinterpret_cast<float*>(c->d_hot_w), c->d_hot_sphere, c->d_hot_radius, c->d_enabled_bits,
+                                                                      c->d_affine_bits, c->d_centre_bits);
         R3_CHECK_LAUNCH(c, "split_objects_kernel");
     }
     c->hot_valid = true;
@@ -472,59 +506,71 @@ int r3_split_slots(r3_ctx* c, const uint32_t* d_slots, uint32_t n) {
     if (!c->hot_valid || n == 0) return R3_OK;
     split_slots_kernel<<<(n * 8 + 255) / 256, 256, 0, c->stream>>>(reinterpret_cast<const float4*>(c->d_objects), d_slots, n, c->n_slots,
                                                                     reinterpret_cast<float*>(c->d_hot_xyz), reinterpret_cast<float*>(c->d_hot_w), c->d_hot_sphere,
-                                                                    c->d_enabled_bits, c->d_affine_bits);
+                                                                    c->d_hot_radius, c->d_enabled_bits, c->d_affine_bits, c->d_centre_bits);
     R3_CHECK_LAUNCH(c, "split_slots_kernel");
     return R3_OK;
 }
 namespace {
-__global__ void mask_word_kernel(uint32_t* word_a, uint32_t* word_b, uint32_t keep_mask) {
+__global__ void mask_word_kernel(uint32_t* word_a, uint32_t* word_b, uint32_t* word_c, uint32_t keep_mask) {
     if (word_a) *word_a &= keep_mask;
     if (word_b) *word_b &= keep_mask;
+    if (word_c) *word_c &= keep_mask;
 }
 }  // namespace
-int r3_launch_mask_word(r3_ctx* c, uint32_t* word_a, uint32_t* word_b, uint32_t keep_mask) {
-    mask_word_kernel<<<1, 1, 0, c->stream>>>(word_a, word_b, keep_mask);
+int r3_launch_mask_word(r3_ctx* c, uint32_t* word_a, uint32_t* word_b, uint32_t* word_c, uint32_t keep_mask) {
+    mask_word_kernel<<<1, 1, 0, c->stream>>>(word_a, word_b, word_c, keep_mask);
     R3_CHECK_LAUNCH(c, "mask_word_kernel");
     return R3_OK;
 }
 // r3_resize_objects: the hot copies of slots [0, old_n) are kept by a device copy (FreelistDerivedBuffer::apply, buffer.rs:66-83);
-// slots [old_n, n) are zero records: rows, row 3 and sphere 0, enabled 0, affine 0 (row 3 is not (0, 0, 0, 1)) — what
-// split_objects_kernel derives from them.  Bits at or past old_n read 0, also in the old last partial word.
+// slots [old_n, n) are zero records: rows, row 3, sphere and radius 0, enabled 0, affine 0 (row 3 is not (0, 0, 0, 1)) and centre 0
+// — what split_objects_kernel derives from them, except the centre bit, which it would set (a zero centre is the zero translation);
+// a clear bit is always correct, since the cull then reads the sphere.  Bits at or past old_n read 0, also in the old last partial word.
 int r3_grow_hot(r3_ctx* c, uint32_t old_n, uint32_t n) {
     if (!c->hot_valid) old_n = 0;
     const uint64_t old_words = ((uint64_t)old_n + 31) / 32;
     if ((uint64_t)n > c->hot_cap || !c->d_hot_xyz) {
         const uint64_t cap = r3_hot_capacity(n ? n : 1), bit_words = (cap + 31) / 32 + 1;
         float4 *xyz = nullptr, *w = nullptr, *sph = nullptr;
-        uint32_t *en = nullptr, *af = nullptr;
+        float* rad = nullptr;
+        uint32_t *en = nullptr, *af = nullptr, *ce = nullptr;
         R3_CUDA(c, cudaMalloc((void**)&xyz, cap * 48));
         R3_CUDA(c, cudaMalloc((void**)&w, cap * 16));
         R3_CUDA(c, cudaMalloc((void**)&sph, cap * 16));
+        R3_CUDA(c, cudaMalloc((void**)&rad, cap * 4));
         R3_CUDA(c, cudaMalloc((void**)&en, bit_words * 4));
         R3_CUDA(c, cudaMalloc((void**)&af, bit_words * 4));
+        R3_CUDA(c, cudaMalloc((void**)&ce, bit_words * 4));
         if (old_n) {
             R3_CUDA(c, cudaMemcpyAsync(xyz, c->d_hot_xyz, (size_t)old_n * 48, cudaMemcpyDeviceToDevice, c->stream));
             R3_CUDA(c, cudaMemcpyAsync(w, c->d_hot_w, (size_t)old_n * 16, cudaMemcpyDeviceToDevice, c->stream));
             R3_CUDA(c, cudaMemcpyAsync(sph, c->d_hot_sphere, (size_t)old_n * 16, cudaMemcpyDeviceToDevice, c->stream));
+            R3_CUDA(c, cudaMemcpyAsync(rad, c->d_hot_radius, (size_t)old_n * 4, cudaMemcpyDeviceToDevice, c->stream));
             R3_CUDA(c, cudaMemcpyAsync(en, c->d_enabled_bits, old_words * 4, cudaMemcpyDeviceToDevice, c->stream));
             R3_CUDA(c, cudaMemcpyAsync(af, c->d_affine_bits, old_words * 4, cudaMemcpyDeviceToDevice, c->stream));
+            R3_CUDA(c, cudaMemcpyAsync(ce, c->d_centre_bits, old_words * 4, cudaMemcpyDeviceToDevice, c->stream));
         }
         R3_CUDA(c, r3_stream_sync(c));
         cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits);
+        cudaFree(c->d_hot_radius); cudaFree(c->d_centre_bits);
         c->d_hot_xyz = xyz; c->d_hot_w = w; c->d_hot_sphere = sph; c->d_enabled_bits = en; c->d_affine_bits = af; c->hot_cap = cap;
+        c->d_hot_radius = rad; c->d_centre_bits = ce;
     }
     const uint64_t first_word = old_n / 32, new_words = ((uint64_t)n + 31) / 32;
     if (n > old_n) {
         R3_CUDA(c, cudaMemsetAsync(c->d_hot_xyz + (size_t)old_n * 3, 0, (size_t)(n - old_n) * 48, c->stream));
         R3_CUDA(c, cudaMemsetAsync(c->d_hot_w + old_n, 0, (size_t)(n - old_n) * 16, c->stream));
         R3_CUDA(c, cudaMemsetAsync(c->d_hot_sphere + old_n, 0, (size_t)(n - old_n) * 16, c->stream));
+        R3_CUDA(c, cudaMemsetAsync(c->d_hot_radius + old_n, 0, (size_t)(n - old_n) * 4, c->stream));
     }
     const uint64_t whole = (old_n & 31u) ? first_word + 1 : first_word;   // first word that holds no kept slot
     if (new_words > whole) {
         R3_CUDA(c, cudaMemsetAsync(c->d_enabled_bits + whole, 0, (new_words - whole) * 4, c->stream));
         R3_CUDA(c, cudaMemsetAsync(c->d_affine_bits + whole, 0, (new_words - whole) * 4, c->stream));
+        R3_CUDA(c, cudaMemsetAsync(c->d_centre_bits + whole, 0, (new_words - whole) * 4, c->stream));
     }
-    if (old_n & 31u) R3_TRY(r3_launch_mask_word(c, c->d_enabled_bits + first_word, c->d_affine_bits + first_word, (1u << (old_n & 31u)) - 1u));
+    if (old_n & 31u)
+        R3_TRY(r3_launch_mask_word(c, c->d_enabled_bits + first_word, c->d_affine_bits + first_word, c->d_centre_bits + first_word, (1u << (old_n & 31u)) - 1u));
     c->hot_valid = true;
     return R3_OK;
 }

@@ -4,14 +4,14 @@
 // A moved object brings 64 bytes of new information, its matrix; the world bounding sphere (mesh sphere.apply_transform,
 // util/frustum.rs:22-32) and the sort location (transform_point3a(ZERO)) are functions of it and of the mesh sphere, which stays
 // resident per slot.  One kernel reads matrix, mesh sphere and (sparse form) slot and writes everything that depends on them: float4
-// #0-4 of the record, the cull + bake's dense copies (rows_xyz, rows_w, spheres, the affine bit) and the sort location — about 256 B per
-// object, HBM-bound.  `enabled`, the cold fields, key and flags are never touched.  Arithmetic: rule R12's object half (DESIGN.md §2),
+// #0-4 of the record, the cull + bake's dense copies (rows_xyz, rows_w, spheres, radii, the affine and centre bits) and the sort
+// location — about 260 B per object, HBM-bound.  `enabled`, the cold fields, key and flags are never touched.  Arithmetic: rule R12's object half (DESIGN.md §2),
 // one IEEE f32 operation at a time, never contracted (-fmad=false and the _rn intrinsics).
 //
 // Layout: four lanes per object, lane k owning column k as one float4 (16-byte loads and stores, 64-byte runs per object); a warp walks
 // 32 consecutive entries in four steps of eight.  The lanes of an object exchange the columns' xyz by shuffles and each evaluates the
-// sums in the rule's order.  In the dense form entry i is slot i, so a warp owns one 32-slot word of the affine bits and stores it
-// whole; only a ragged last word and the sparse form use atomics, as split_slots_kernel does.
+// sums in the rule's order.  In the dense form entry i is slot i, so a warp owns one 32-slot word of the affine and of the centre bits
+// and stores them whole; only a ragged last word and the sparse form use atomics, as split_slots_kernel does.
 #include <cstring>
 #include <vector>
 
@@ -25,11 +25,12 @@ template <bool SPARSE>
 __global__ void __launch_bounds__(OT_THREADS, 4)
 object_transforms_kernel(const float4* __restrict__ mats, const uint32_t* __restrict__ slots, uint32_t n, uint32_t n_slots, const float4* __restrict__ mesh_spheres,
                          float4* __restrict__ objects, float* __restrict__ rows_xyz, float* __restrict__ rows_w, float4* __restrict__ spheres,
-                         uint32_t* __restrict__ affine_bits, float* __restrict__ sort_loc, uint32_t sort_n) {
+                         float* __restrict__ radii, uint32_t* __restrict__ affine_bits, uint32_t* __restrict__ centre_bits, float* __restrict__ sort_loc,
+                         uint32_t sort_n) {
     const uint32_t lane = threadIdx.x & 31u, k = lane & 3u, g = lane >> 2, first = lane & ~3u;
     const uint32_t wtile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, base = wtile * 32u;
     if (base >= n) return;   // the whole warp
-    uint32_t abits = 0;
+    uint32_t abits = 0, cbits = 0;
 #pragma unroll
     for (uint32_t it = 0; it < 4; ++it) {
         const uint32_t i = base + it * 8u + g;
@@ -45,28 +46,34 @@ object_transforms_kernel(const float4* __restrict__ mats, const uint32_t* __rest
         }
         const uint32_t a = __ballot_sync(0xFFFFFFFFu, ok && __float_as_uint(col.w) == affine_w_bits(k));
         const bool affine = ((a >> first) & 0xFu) == 0xFu;
+        // BoundingSphere::apply_transform: Vec3::length_squared of each axis, f32::max (fmaxf ignores a NaN operand as it does), sqrt;
+        // centre = matrix * (c, 1) in mul_vec4's order; radius = max_scale * r.  Every lane of the object evaluates it (zeros when !ok).
+        float ls[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) ls[c] = add_rn(add_rn(mul_rn(x[c], x[c]), mul_rn(y[c], y[c])), mul_rn(z[c], z[c]));
+        const float max_scale = __fsqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
+        float4 sph;
+        sph.x = add_rn(add_rn(add_rn(mul_rn(x[0], ms.x), mul_rn(x[1], ms.y)), mul_rn(x[2], ms.z)), mul_rn(x[3], 1.0f));
+        sph.y = add_rn(add_rn(add_rn(mul_rn(y[0], ms.x), mul_rn(y[1], ms.y)), mul_rn(y[2], ms.z)), mul_rn(y[3], 1.0f));
+        sph.z = add_rn(add_rn(add_rn(mul_rn(z[0], ms.x), mul_rn(z[1], ms.y)), mul_rn(z[2], ms.z)), mul_rn(z[3], 1.0f));
+        sph.w = mul_rn(max_scale, ms.w);
+        // the four lanes of an object agree, so the ballot carries each object's centre bit four times
+        const uint32_t cb = __ballot_sync(0xFFFFFFFFu, ok && centre_is_translation(sph.x, sph.y, sph.z, x[3], y[3], z[3]));
+        const bool centred = (cb >> first) & 1u;
         if (!SPARSE) {
 #pragma unroll
-            for (uint32_t q = 0; q < 8; ++q) abits |= (((a >> (4u * q)) & 0xFu) == 0xFu ? 1u : 0u) << (it * 8u + q);
+            for (uint32_t q = 0; q < 8; ++q) {
+                abits |= (((a >> (4u * q)) & 0xFu) == 0xFu ? 1u : 0u) << (it * 8u + q);
+                cbits |= ((cb >> (4u * q)) & 1u) << (it * 8u + q);
+            }
         }
         if (ok) {
-            // BoundingSphere::apply_transform: Vec3::length_squared of each axis, f32::max (fmaxf ignores a NaN operand as it does), sqrt;
-            // centre = matrix * (c, 1) in mul_vec4's order; radius = max_scale * r
-            float ls[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) ls[c] = add_rn(add_rn(mul_rn(x[c], x[c]), mul_rn(y[c], y[c])), mul_rn(z[c], z[c]));
-            const float max_scale = __fsqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
-            float4 sph;
-            sph.x = add_rn(add_rn(add_rn(mul_rn(x[0], ms.x), mul_rn(x[1], ms.y)), mul_rn(x[2], ms.z)), mul_rn(x[3], 1.0f));
-            sph.y = add_rn(add_rn(add_rn(mul_rn(y[0], ms.x), mul_rn(y[1], ms.y)), mul_rn(y[2], ms.z)), mul_rn(y[3], 1.0f));
-            sph.z = add_rn(add_rn(add_rn(mul_rn(z[0], ms.x), mul_rn(z[1], ms.y)), mul_rn(z[2], ms.z)), mul_rn(z[3], 1.0f));
-            sph.w = mul_rn(max_scale, ms.w);
             objects[(size_t)s * 8 + k] = col;
             float* xyz = rows_xyz + (size_t)s * 12 + k;
             xyz[0] = col.x; xyz[4] = col.y; xyz[8] = col.z;
             rows_w[(size_t)s * 4 + k] = col.w;
             if (k == 0) objects[(size_t)s * 8 + 4] = sph;
-            else if (k == 1) spheres[s] = sph;
+            else if (k == 1) { spheres[s] = sph; radii[s] = sph.w; }
             else if (k == 2) {
                 // location = transform_point3a(Vec3A::ZERO): w + ((x * 0 + y * 0) + z * 0) per component — NaN for an inf axis
                 if (sort_loc && s < sort_n) {
@@ -79,15 +86,19 @@ object_transforms_kernel(const float4* __restrict__ mats, const uint32_t* __rest
                 const uint32_t bit = 1u << (s & 31u);   // other slots of the word may be written by other warps
                 if (affine) atomicOr(&affine_bits[s >> 5], bit);
                 else atomicAnd(&affine_bits[s >> 5], ~bit);
+                if (centred) atomicOr(&centre_bits[s >> 5], bit);
+                else atomicAnd(&centre_bits[s >> 5], ~bit);
             }
         }
     }
     if (!SPARSE && lane == 0) {
-        if (n - base >= 32u) affine_bits[wtile] = abits;
+        if (n - base >= 32u) { affine_bits[wtile] = abits; centre_bits[wtile] = cbits; }
         else {   // the last word also holds slots past n: they keep their bits
             const uint32_t mask = (1u << (n - base)) - 1u;
             atomicAnd(&affine_bits[wtile], ~mask | abits);
             atomicOr(&affine_bits[wtile], abits);
+            atomicAnd(&centre_bits[wtile], ~mask | cbits);
+            atomicOr(&centre_bits[wtile], cbits);
         }
     }
 }
@@ -122,8 +133,8 @@ int launch_transforms(r3_ctx* c, const uint32_t* d_slots, const float* d_mats, u
     const uint32_t ctas = (uint32_t)(((uint64_t)n + OT_THREADS - 1) / OT_THREADS);   // a warp walks 32 entries: 256 per CTA
     auto kernel = d_slots ? object_transforms_kernel<true> : object_transforms_kernel<false>;
     kernel<<<ctas, OT_THREADS, 0, c->stream>>>(reinterpret_cast<const float4*>(d_mats), d_slots, n, c->n_slots, c->d_mesh_spheres, reinterpret_cast<float4*>(c->d_objects),
-                                               reinterpret_cast<float*>(c->d_hot_xyz), reinterpret_cast<float*>(c->d_hot_w), c->d_hot_sphere, c->d_affine_bits,
-                                               sort_n ? c->d_sort_loc : nullptr, sort_n);
+                                               reinterpret_cast<float*>(c->d_hot_xyz), reinterpret_cast<float*>(c->d_hot_w), c->d_hot_sphere, c->d_hot_radius,
+                                               c->d_affine_bits, c->d_centre_bits, sort_n ? c->d_sort_loc : nullptr, sort_n);
     R3_CHECK_LAUNCH(c, "object_transforms_kernel");
     r3_new_frame_epoch(c);                       // a frame-wide sort made before the move is stale
     if (sort_n) c->locations_moved = true;       // the host batching's mirror c->sort_loc is behind the device's
