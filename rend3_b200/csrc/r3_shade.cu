@@ -61,12 +61,14 @@ __device__ __forceinline__ float sqrt_approx(float x) { float r; asm("sqrt.appro
 __device__ __forceinline__ float rcp_approx(float x) { float r; asm("rcp.approx.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 
 // surface_shading (opaque.wgsl:440-468) with brdf_d_ggx / brdf_f_schlick / brdf_v_smith_ggx_correlated / brdf_fd_lambert.
-// When roughness > 0 every term is finite, so a light with n.l <= 0 contributes exactly 0 and is skipped; with
-// roughness == 0 the reference's 0 * inf = NaN must survive to the caller's max(), so the full path runs.
+// When roughness > 0 and n.v is a number every term is finite, so a light with n.l <= 0 contributes exactly 0 and is skipped.
+// With roughness == 0 the reference's 0 * inf = NaN must survive to the caller's max(), so the full path runs; so it does for a
+// NaN normal (a zero vertex normal, an axis scaled by 0, a normal map without tangents): saturate() turns n.l into 0 but n.v stays
+// NaN, the reference's term is NaN, and fs_main's final max() then yields ambient * albedo, not max(ambient * albedo, 0).
 __device__ __forceinline__ float3 surface_shading(const float3 l, const float3 intensity, const Pixel& px, const float3 v, float nov, float occlusion) {
     const float nol = saturate(dot3(px.normal, l));
     const float a = px.roughness, a2 = a * a;
-    if (nol <= 0.0f && a2 > 0.0f) return make_float3(0.f, 0.f, 0.f);
+    if (nol <= 0.0f && a2 > 0.0f && nov == nov) return make_float3(0.f, 0.f, 0.f);
     const float3 h = normalize3(make_float3(v.x + l.x, v.y + l.y, v.z + l.z));
     const float noh = saturate(dot3(px.normal, h));
     const float loh = saturate(dot3(l, h));
