@@ -20,7 +20,8 @@
  *   - one context per GPU; calls on a context must be externally serialised (this is the
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
- *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_evaluate_shadow_cameras,
+ *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
+ *     r3_evaluate_shadow_cameras,
  *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
@@ -29,7 +30,7 @@
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
  *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices, r3_set_object_animations,
- *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_directional_light_sources,
+ *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_directional_light_sources,
  *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
@@ -148,6 +149,32 @@ int r3_resize_objects(r3_ctx*, uint32_t n_slots);
 int r3_set_object_mesh_spheres(r3_ctx*, const uint32_t* slots_or_null, const float* center_radius /* n x 4 */, uint32_t n);
 int r3_set_object_transforms(r3_ctx*, const uint32_t* slots_or_null, const float* mat4s /* n x 16, column-major */, uint32_t n);
 int r3_set_object_transforms_device(r3_ctx*, const uint32_t* d_slots_or_null, const float* d_mat4s, uint32_t n);
+/* Objects that come and go: ObjectManager::add into a slot prepared earlier, and remove (object.rs:122-160, 330-342), for n slots in one
+ * kernel, from host or device memory.  The host prepares a pool once (records with mesh, material and transform, sort info with the
+ * keys); each frame switches slots on and off.  Entry i makes slot slots[i] present (enabled[i] != 0) or absent (== 0): it writes the
+ * record's `enabled` word (1 or 0), the slot's bit of the cull + bake's enabled bits and, when sort info is set, its live bit
+ * (enumerated_objects, flags bit 0).  Nothing else changes — transform, sphere, cold fields, key, flags bits 1-2 and location stay — so
+ * switching a slot on again restores it exactly.  Placing a spawned object with r3_set_object_transforms_device in the same frame is
+ * independent of the order of the two calls: they write disjoint fields.
+ *   slots == NULL: slots 0 .. n-1 (the dense form, n <= the slot count).
+ *   r3_set_objects_enabled         host pointers, blocking.  Every slot below the slot count, none named twice, no null pointer, checked
+ *                                  before anything is written (R3_E_INVALID, context unchanged).  The host's mirrors stay exact: the live
+ *                                  bits of the sort flags and the count of live key-2 slots that decides whether the blend routine runs.
+ *   r3_set_objects_enabled_device  the same from DEVICE memory, enqueue only; legal between r3_frame_begin and r3_frame_end (a frame graph
+ *                                  updates its arguments in place).  Producer ordering as for r3_set_object_transforms_device;
+ *                                  out-of-range slots are dropped, distinct slots are a precondition.  From this call until the next
+ *                                  r3_set_object_sort_info the host cannot know which slots are live, so the blend routine runs whenever
+ *                                  SOME slot has material key 2, present or not.  A frame without a present key-2 object then collects
+ *                                  no fragments and gives the same image, but waits for the fragment count as every frame with
+ *                                  transparent objects does (a recorded frame flushes there).
+ * R3_E_STATE before r3_set_objects and while the object buffer is borrowed (r3_set_objects_device).  n == 0 is R3_OK and enqueues
+ * nothing.  Each call starts a new frame epoch.  A later r3_update_objects, r3_set_objects or r3_update_object_sort_info of a slot
+ * overwrites what these calls wrote, and the reverse.
+ * Departure from the reference: rend3's remove leaves the object enumerated (live) but disabled for one frame before its handle is
+ * reclaimed (handle_alloc.rs:21-29); here an absent slot is disabled and not live at once.  The image is the same (a disabled object
+ * draws nothing); the batch records of that one frame differ. */
+int r3_set_objects_enabled(r3_ctx*, const uint32_t* slots_or_null, const uint8_t* enabled, uint32_t n);
+int r3_set_objects_enabled_device(r3_ctx*, const uint32_t* d_slots_or_null, const uint8_t* d_enabled, uint32_t n);
 int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);               /* eval_output.mesh_buffer (mesh.rs:99) */
 /* MeshManager::add (mesh.rs:123-184): write nbytes at byte_offset of the megabuffer (both multiples of 4).  A write past the end extends it;
  * words between the old end and byte_offset read 0.  The allocation grows to the next power of two, keeping its contents (also what

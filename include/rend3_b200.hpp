@@ -83,6 +83,9 @@ struct EvalOutput {
     // objects the application moved this frame (Renderer::set_object_transform in bulk): matrices (and slots, null = slots 0 .. n-1)
     // in DEVICE memory, their producer ordered on the context's stream; applied at the skinning node before posed_objects, enqueue only
     const uint32_t* d_moved_slots = nullptr; const float* d_moved_transforms = nullptr; uint32_t n_moved = 0;
+    // objects that appear or disappear this frame (ObjectManager::add into a prepared slot / remove): presence bytes (and slots, null =
+    // slots 0 .. n-1) in DEVICE memory, their producer ordered on the context's stream; applied at the skinning node before the moves
+    const uint32_t* d_presence_slots = nullptr; const uint8_t* d_presence = nullptr; uint32_t n_presence = 0;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -124,6 +127,8 @@ public:
     }
     // Renderer::set_object_transform (object.rs:302-316) for n objects from host memory (slots == nullptr: slots 0 .. n-1); blocking
     void set_object_transforms(const uint32_t* slots, const float* mat4s, uint32_t n) { check(r3_set_object_transforms(ctx_, slots, mat4s, n)); }
+    // ObjectManager::add into a prepared slot / remove for n slots from host memory (slots == nullptr: slots 0 .. n-1); blocking
+    void set_objects_enabled(const uint32_t* slots, const uint8_t* enabled, uint32_t n) { check(r3_set_objects_enabled(ctx_, slots, enabled, n)); }
     void sync() { check(r3_sync(ctx_)); }
 
 private:
@@ -147,6 +152,7 @@ class GpuSkinner {   // skinning.rs:54-199: add_skinning_to_graph — skinned po
 public:
     void add_skinning_to_graph(Renderer& r, const EvalOutput& ev) const {
         if (ev.n_skeletons) r.check(r3_skin(r.raw(), ev.skinning_inputs, ev.n_skeletons, ev.joint_matrices, ev.n_joints));
+        if (ev.n_presence) r.check(r3_set_objects_enabled_device(r.raw(), ev.d_presence_slots, ev.d_presence, ev.n_presence));
         if (ev.n_moved) r.check(r3_set_object_transforms_device(r.raw(), ev.d_moved_slots, ev.d_moved_transforms, ev.n_moved));
         if (ev.posed_objects) r.check(r3_pose_objects(r.raw()));
         if (ev.posed_skinning) {

@@ -44,6 +44,7 @@ ENTRY_POINTS = [
     "set_animations", "set_skeletons", "set_pose_jobs", "pose_skeletons", "skin_posed", "readback_joint_matrices",
     "set_object_animations", "set_object_pose_jobs", "pose_objects", "readback_objects",
     "set_object_mesh_spheres", "set_object_transforms", "set_object_transforms_device",
+    "set_objects_enabled", "set_objects_enabled_device",
 ]
 
 
@@ -196,6 +197,36 @@ class Backend:
         n = mn if n is None else n
         assert n is not None and (sn is None or sn == n)
         self._call("set_object_transforms_device", C.c_void_p(sp), C.c_void_p(mp), C.c_uint32(n))
+
+    # ---- objects that come and go (ObjectManager::add into a prepared slot / remove)
+    def set_objects_enabled(self, enabled, slots=None):
+        """Slots 0 .. n-1, or the listed slots, present (enabled != 0) or absent, from host memory.  Blocking."""
+        e = np.asarray(enabled)
+        assert e.ndim == 1 and (e.dtype == np.bool_ or e.dtype == np.uint8), "enabled: a 1-d bool or uint8 array"
+        e = np.ascontiguousarray(e).view(np.uint8)
+        s = None
+        if slots is not None:
+            s = np.asarray(slots)
+            assert s.ndim == 1 and s.dtype.kind in "iu" and len(s) == len(e), "slots: a 1-d integer array as long as enabled"
+            assert not len(s) or (s.min() >= 0 and s.max() <= 0xFFFFFFFF), "slots: out of the uint32 range"
+            s = np.ascontiguousarray(s, dtype=np.uint32)
+        self._call("set_objects_enabled", _ptr(s), _ptr(e) if len(e) else None, C.c_uint32(len(e)))
+
+    def set_objects_enabled_device(self, enabled, slots=None, n: Optional[int] = None):
+        """The same from device memory, enqueue only.  `enabled` (bool / uint8 (n,)) and `slots` (int32 / uint32 (n,), None: slots
+        0 .. n-1) are contiguous CUDA tensors, or raw device pointers with `n` given; the caller keeps them alive and orders their producer
+        on stream()."""
+        def pointer(x, sizes, what):
+            if x is None or isinstance(x, int):
+                return x, None
+            assert getattr(x, "is_cuda", False) and x.is_contiguous() and x.dim() == 1 and x.element_size() in sizes \
+                and not x.is_floating_point(), f"{what}: a contiguous 1-d CUDA tensor of {sizes[0]}-byte integers"
+            return x.data_ptr(), x.numel()
+        ep, en = pointer(enabled, (1,), "enabled")
+        sp, sn = pointer(slots, (4,), "slots")
+        n = en if n is None else n
+        assert n is not None and (sn is None or sn == n) and (en is None or en == n), "enabled and slots differ in length"
+        self._call("set_objects_enabled_device", C.c_void_p(sp), C.c_void_p(ep), C.c_uint32(n))
 
     def set_mesh_buffer(self, words: np.ndarray):
         words = np.ascontiguousarray(words, dtype=np.uint32)

@@ -118,6 +118,8 @@ struct r3_ctx {
     float4* d_mesh_spheres = nullptr; uint32_t n_mesh_spheres = 0, mesh_spheres_cap = 0;
     bool locations_moved = false;             // r3_set_object_transforms* ran since c->sort_loc last took the device's locations
     uint32_t sort_live_blend = 0, sort_wide_keys = 0;   // live slots with material key 2 (any_blend), slots with a key >= 64 (host batching)
+    uint32_t sort_blend_slots = 0;            // slots with material key 2, live or not (any_blend while presence_on_device)
+    bool presence_on_device = false;          // r3_set_objects_enabled_device ran since r3_set_object_sort_info: the host's live bits are stale
     // frame-wide sort shared by the cameras of one frame (r3_gpu_batching.cu)
     unsigned long long* d_gsort_keys[2] = {nullptr, nullptr}; uint64_t gsort_cap[2] = {0, 0}; uint32_t* d_gsort_hist = nullptr; uint64_t gsort_hist_cap = 0;
     uint32_t* d_gsort_header = nullptr; int gsort_src = 0; uint32_t gsort_n = 0; bool gsort_valid = false; float gsort_loc[3] = {0, 0, 0};
@@ -155,7 +157,7 @@ struct r3_ctx {
     bool any_frag_alpha = false;              // a material discards per fragment (cutout alpha from its albedo texture / vertex colour)
     unsigned long long* d_stats = nullptr;    // [8]: [0..3] forward statistics, [4] scratch of r3_compute_max_invocations
     // blend routine: per-sample fragment lists (head = node index + 1, 0 = empty; node = {record, depth bits, next, 0})
-    bool any_blend = false;                   // some live object carries material key 2 (TransparencyType::Blend)
+    bool any_blend = false;                   // some live object carries material key 2 (TransparencyType::Blend); see sort_blend_slots
     uint32_t* d_frag_heads = nullptr; uint64_t frag_heads_cap = 0;
     uint4* d_frag_nodes = nullptr; uint64_t frag_nodes_cap = 0;
     void* d_scratch = nullptr; uint64_t scratch_cap = 0;
@@ -248,6 +250,10 @@ void r3_anim_apply_posed_locations(r3_ctx* c);
 // copy of every location into c->sort_loc, complete once the caller has drained the stream
 int r3_stage_moved_locations(r3_ctx* c, bool* staged);
 int r3_grow_mesh_spheres(r3_ctx* c, uint32_t n);   // r3_resize_objects: zero spheres for the new slots, once spheres are set
+// r3_ctx.cu: the host bookkeeping of r3_set_objects_enabled (exact: live bits of c->sort_flags, live key-2 count, any_blend) and, after
+// the device form has set c->presence_on_device, any_blend's conservative rule
+void r3_presence_set_host(r3_ctx* c, const uint32_t* slots, const uint8_t* enabled, uint32_t n);
+void r3_presence_derive(r3_ctx* c);
 int r3_reserve_point_buffer(r3_ctx* c, uint32_t n_lights);   // r3_lights.cu: room for n lights in c->d_point, contents kept
 
 #ifdef __CUDACC__

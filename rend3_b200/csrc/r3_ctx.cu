@@ -298,8 +298,11 @@ static inline uint8_t sort_key8(uint64_t key, uint8_t flags) {
 }
 static inline uint32_t sort_live_blend(uint64_t key, uint8_t flags) { return key == 2 && (flags & 1) ? 1u : 0u; }   // TransparencyType::Blend as u64 (pbr/material.rs:497-503)
 static inline uint32_t sort_wide_key(uint64_t key) { return key >= 64 ? 1u : 0u; }                                 // only the host batching sorts such keys
+static inline uint32_t sort_blend_slot(uint64_t key) { return key == 2 ? 1u : 0u; }                                  // live or not
 static void sort_derive(r3_ctx* c) {
-    c->any_blend = c->sort_live_blend != 0;
+    // after r3_set_objects_enabled_device only the device knows which slots are live: then any slot with key 2 runs the blend routine
+    // (over no fragments when none of them is present, which leaves the image as it is)
+    c->any_blend = (c->presence_on_device ? c->sort_blend_slots : c->sort_live_blend) != 0;
     c->gpu_batching_ok = c->sort_wide_keys == 0 && c->sort_key.size() < (1u << 24) && !getenv("R3_HOST_BATCHING");
 }
 
@@ -317,9 +320,10 @@ R3_EXPORT int r3_set_object_sort_info(r3_ctx* c, const uint64_t* key, const uint
     R3_CUDA(c, cudaMemcpyAsync(c->d_live_bits, bits.data(), (size_t)words * 4, cudaMemcpyHostToDevice, c->stream));
     // device copies for the on-device batch_objects
     std::vector<uint8_t> key8(n ? n : 1, 0);
-    c->sort_live_blend = 0; c->sort_wide_keys = 0;
+    c->sort_live_blend = 0; c->sort_wide_keys = 0; c->sort_blend_slots = 0;
     for (uint32_t i = 0; i < n; ++i) {
         c->sort_wide_keys += sort_wide_key(key[i]);
+        c->sort_blend_slots += sort_blend_slot(key[i]);
         c->sort_live_blend += sort_live_blend(key[i], flags[i]);
         key8[i] = sort_key8(key[i], flags[i]);
     }
@@ -337,6 +341,7 @@ R3_EXPORT int r3_set_object_sort_info(r3_ctx* c, const uint64_t* key, const uint
     R3_CUDA(c, r3_stream_sync(c));
     r3_new_frame_epoch(c);
     c->have_live = true;
+    c->presence_on_device = false;   // the flags say again which slots are live
     sort_derive(c);
     return R3_OK;
 }
@@ -481,6 +486,7 @@ R3_EXPORT int r3_update_object_sort_info(r3_ctx* c, const uint32_t* slots, const
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t s = slots[i];
         c->sort_wide_keys += sort_wide_key(key[i]) - sort_wide_key(c->sort_key[s]);
+        c->sort_blend_slots += sort_blend_slot(key[i]) - sort_blend_slot(c->sort_key[s]);
         c->sort_live_blend += sort_live_blend(key[i], flags[i]) - sort_live_blend(c->sort_key[s], c->sort_flags[s]);
         c->sort_key[s] = key[i]; c->sort_flags[s] = flags[i];
         memcpy(&c->sort_loc[3 * (size_t)s], loc + 3 * (size_t)i, 12);
@@ -513,6 +519,22 @@ R3_EXPORT int r3_update_object_sort_info(r3_ctx* c, const uint32_t* slots, const
     sort_derive(c);
     return R3_OK;
 }
+
+// r3_set_objects_enabled (r3_object_transforms.cu): the host form's entries, once on the device, go into the live bits of the host
+// mirror and the live key-2 count (slots == nullptr: slots 0 .. n-1; slots without sort info have no live bit)
+void r3_presence_set_host(r3_ctx* c, const uint32_t* slots, const uint8_t* enabled, uint32_t n) {
+    if (!c->have_live) return;
+    const size_t count = c->sort_flags.size();
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t s = slots ? slots[i] : i;
+        if (s >= count) continue;
+        const uint8_t was = c->sort_flags[s], now = (uint8_t)((was & ~1u) | (enabled[i] ? 1u : 0u));
+        c->sort_live_blend += sort_live_blend(c->sort_key[s], now) - sort_live_blend(c->sort_key[s], was);
+        c->sort_flags[s] = now;
+    }
+    sort_derive(c);
+}
+void r3_presence_derive(r3_ctx* c) { sort_derive(c); }
 
 // FreelistDerivedBuffer::apply's growth (util/freelist/buffer.rs:66-83): a larger buffer that starts with a device copy of the old one
 R3_EXPORT int r3_resize_objects(r3_ctx* c, uint32_t n) {

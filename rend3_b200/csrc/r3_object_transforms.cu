@@ -12,6 +12,10 @@
 // 32 consecutive entries in four steps of eight.  The lanes of an object exchange the columns' xyz by shuffles and each evaluates the
 // sums in the rule's order.  In the dense form entry i is slot i, so a warp owns one 32-slot word of the affine and of the centre bits
 // and stores them whole; only a ragged last word and the sparse form use atomics, as split_slots_kernel does.
+//
+// The same unit switches prepared slots on and off (ObjectManager::add into a prepared slot / remove, object.rs:122-160, 330-342):
+// r3_set_objects_enabled, r3_set_objects_enabled_device write the record's `enabled` word, the enabled bit and the live bit of each
+// listed slot — 4 B + 2 bits per entry, from 1 B (dense) or 5 B (sparse) read.
 #include <cstring>
 #include <vector>
 
@@ -141,7 +145,105 @@ int launch_transforms(r3_ctx* c, const uint32_t* d_slots, const float* d_mats, u
     return R3_OK;
 }
 
+// ---- ObjectManager::add into a prepared slot / remove: r3_set_objects_enabled, r3_set_objects_enabled_device
+// Entry i makes slot s present or absent: the record's `enabled` word (u32 @116), the slot's bit of the cull + bake's enabled bits and,
+// below sort_n, its live bit.  Nothing else of the record, the hot arrays or the sort facts changes.
+constexpr uint32_t EN_THREADS = 256;
+constexpr uint32_t EN_WORD = offsetof(r3_object, enabled) / 4;
+
+// sparse: one thread per entry; slots of one bit word come from different threads, so the words take atomics
+__global__ void __launch_bounds__(EN_THREADS)
+objects_enabled_sparse_kernel(const uint32_t* __restrict__ slots, const uint8_t* __restrict__ enabled, uint32_t n, uint32_t n_slots,
+                              uint32_t* __restrict__ objects, uint32_t* __restrict__ enabled_bits, uint32_t* __restrict__ live_bits, uint32_t sort_n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t s = __ldg(slots + i);
+    if (s >= n_slots) return;   // out-of-range writes are dropped (ScatterCopy's robust access)
+    const bool on = __ldg(enabled + i) != 0;
+    objects[(size_t)s * 32 + EN_WORD] = on ? 1u : 0u;
+    const uint32_t bit = 1u << (s & 31u);
+    if (on) atomicOr(&enabled_bits[s >> 5], bit);
+    else atomicAnd(&enabled_bits[s >> 5], ~bit);
+    if (s < sort_n) {
+        if (on) atomicOr(&live_bits[s >> 5], bit);
+        else atomicAnd(&live_bits[s >> 5], ~bit);
+    }
+}
+
+// *word = (*word & ~mask) | (bits & mask): a plain store when the warp owns the whole word, atomics when slots past the range share it
+__device__ __forceinline__ void store_bits(uint32_t* word, uint32_t bits, uint32_t mask) {
+    if (mask == 0xFFFFFFFFu) *word = bits;
+    else if (mask) { atomicAnd(word, ~mask | bits); atomicOr(word, bits & mask); }
+}
+
+// dense: entry i is slot i; a warp owns one 32-slot word, ballots the 32 flags and stores the bit words whole
+__global__ void __launch_bounds__(EN_THREADS)
+objects_enabled_dense_kernel(const uint8_t* __restrict__ enabled, uint32_t n, uint32_t* __restrict__ objects, uint32_t* __restrict__ enabled_bits,
+                             uint32_t* __restrict__ live_bits, uint32_t sort_n) {
+    const uint32_t lane = threadIdx.x & 31u, wtile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, base = wtile * 32u;
+    if (base >= n) return;   // the whole warp
+    const uint32_t s = base + lane;
+    const bool on = s < n && __ldg(enabled + s) != 0;
+    const uint32_t bits = __ballot_sync(0xFFFFFFFFu, on);
+    if (s < n) objects[(size_t)s * 32 + EN_WORD] = on ? 1u : 0u;
+    if (lane == 0) {
+        const auto below = [base](uint32_t end) { return end >= base + 32u ? 0xFFFFFFFFu : end > base ? (1u << (end - base)) - 1u : 0u; };
+        store_bits(&enabled_bits[wtile], bits, below(n));
+        if (live_bits) store_bits(&live_bits[wtile], bits, below(n < sort_n ? n : sort_n));
+    }
+}
+
+int check_presence_state(r3_ctx* c, const char* who) {
+    if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, who);
+    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_objects_enabled: the object buffer is borrowed (r3_set_objects_device)");
+    return R3_OK;
+}
+
+int launch_enabled(r3_ctx* c, const uint32_t* d_slots, const uint8_t* d_enabled, uint32_t n) {
+    const uint32_t sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    uint32_t* objects = reinterpret_cast<uint32_t*>(c->d_objects);
+    uint32_t* live = sort_n ? c->d_live_bits : nullptr;
+    const uint32_t ctas = (uint32_t)(((uint64_t)n + EN_THREADS - 1) / EN_THREADS);
+    if (d_slots) objects_enabled_sparse_kernel<<<ctas, EN_THREADS, 0, c->stream>>>(d_slots, d_enabled, n, c->n_slots, objects, c->d_enabled_bits, live, sort_n);
+    else objects_enabled_dense_kernel<<<ctas, EN_THREADS, 0, c->stream>>>(d_enabled, n, objects, c->d_enabled_bits, live, sort_n);
+    R3_CHECK_LAUNCH(c, "objects_enabled_kernel");
+    r3_new_frame_epoch(c);
+    return R3_OK;
+}
+
 }  // namespace
+
+R3_EXPORT int r3_set_objects_enabled(r3_ctx* c, const uint32_t* slots, const uint8_t* enabled, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (n == 0) return R3_OK;
+    if (!enabled) return r3_fail(c, R3_E_INVALID, "set_objects_enabled: null");
+    R3_TRY(check_presence_state(c, "set_objects_enabled before set_objects"));
+    if (!slots && n > c->n_slots) return r3_fail(c, R3_E_INVALID, "set_objects_enabled: more flags than slots");
+    if (slots) R3_TRY(check_slots(c, slots, n, c->n_slots, "set_objects_enabled: slot beyond the object buffer", "set_objects_enabled: one slot named twice"));
+    cudaSetDevice(c->device);
+    R3_TRY(r3_reserve(c, &c->d_scratch, &c->scratch_cap, (uint64_t)n * 5, 1, false, false));
+    uint32_t* d_slots = slots ? (uint32_t*)c->d_scratch : nullptr;
+    uint8_t* d_enabled = (uint8_t*)c->d_scratch + (slots ? (size_t)n * 4 : 0);
+    if (slots) R3_CUDA(c, cudaMemcpyAsync(d_slots, slots, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
+    R3_CUDA(c, cudaMemcpyAsync(d_enabled, enabled, n, cudaMemcpyHostToDevice, c->stream));
+    R3_TRY(launch_enabled(c, d_slots, d_enabled, n));
+    R3_CUDA(c, r3_stream_sync(c));               // host pointers are only borrowed for the call
+    r3_presence_set_host(c, slots, enabled, n);  // the host sees every entry: its mirrors stay exact
+    return R3_OK;
+}
+
+R3_EXPORT int r3_set_objects_enabled_device(r3_ctx* c, const uint32_t* d_slots, const uint8_t* d_enabled, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (n == 0) return R3_OK;
+    if (!d_enabled || ((uintptr_t)d_slots & 3u)) return r3_fail(c, R3_E_INVALID, "set_objects_enabled_device: null or misaligned pointer (slots: 4 bytes)");
+    R3_TRY(check_presence_state(c, "set_objects_enabled_device before set_objects"));
+    if (!d_slots && n > c->n_slots) return r3_fail(c, R3_E_INVALID, "set_objects_enabled_device: more flags than slots");
+    cudaSetDevice(c->device);
+    R3_TRY(launch_enabled(c, d_slots, d_enabled, n));
+    c->presence_on_device = true;                // which slots are live is now known on the device only
+    r3_presence_derive(c);
+    return R3_OK;
+}
 
 R3_EXPORT int r3_set_object_mesh_spheres(r3_ctx* c, const uint32_t* slots, const float* center_radius, uint32_t n) {
     if (!c) return R3_E_INVALID;
