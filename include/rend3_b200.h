@@ -21,14 +21,14 @@
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
- *     r3_evaluate_shadow_cameras,
+ *     r3_update_materials_device, r3_evaluate_shadow_cameras,
  *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
  *     r3_batch_counts / r3_batching_info / r3_forward_stats / r3_stage_times (small device-to-host reads), and the
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
- *     r3_set_mesh_buffer, r3_set_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
+ *     r3_set_mesh_buffer, r3_set_materials, r3_update_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices, r3_set_object_animations,
  *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_directional_light_sources,
  *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
@@ -181,6 +181,31 @@ int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);            
  * r3_skin wrote) — MeshManager::reallocate_buffers (mesh.rs:264-308). */
 int r3_update_mesh_buffer(r3_ctx*, uint64_t byte_offset, const void* bytes, uint64_t nbytes);
 int r3_set_materials(r3_ctx*, const r3_material* records, uint32_t count);         /* material_manager.archetype_view::<M>().buffer() */
+/* Materials that change: MaterialManager::update and evaluate's scatter of the stale records (material.rs:163-189, 202-227), from host or
+ * device memory.  Entry i replaces material indices[i] with records[i] (the 208 GpuMaterialData bytes the shading reads); indices == NULL
+ * is the dense form for materials 0 .. n-1.  Nothing else changes: object records, sort info, the frame epoch and textures stay.  A
+ * material's transparency key is not in its record (Material::key, pbr/material.rs:497-503): a change of transparency also needs
+ * r3_update_object_sort_info of the objects that use the material, as with r3_set_materials.
+ *   r3_update_materials         host pointers, blocking: one copy, one kernel, one drain.  A null pointer, an index named twice or index
+ *                               0xFFFFFFFF returns R3_E_INVALID, checked before anything is written (context unchanged).  An index at or
+ *                               past the table's count grows the table, as add_material does (material.rs:131-160): the records in
+ *                               between are zero, the contents are kept.  The dense form with n past the count is R3_E_INVALID.  Whether
+ *                               some material discards per fragment stays exact (the host keeps that one bit per material).
+ *   r3_update_materials_device  the same from DEVICE memory, enqueue only; legal between r3_frame_begin and r3_frame_end (a frame graph
+ *                               updates its arguments in place).  Records 16-byte aligned; producer ordering as for
+ *                               r3_set_object_transforms_device.  The table cannot grow without the host: indices at or past the count are
+ *                               dropped (robust access, as in r3_update_objects), the dense form with n past the count is R3_E_INVALID,
+ *                               distinct indices are a precondition.  From this call until the next r3_set_materials the host cannot know
+ *                               whether some material discards per fragment, so the rasteriser runs its alpha-testing kernels, which give
+ *                               the same image for materials that never discard.
+ * R3_E_STATE from the device form while the table is empty (before r3_set_materials or a growing host update); the host form may start a
+ * table by growth.  n == 0 is R3_OK and enqueues nothing.  A later r3_set_materials replaces everything, and the reverse.  Texture slots
+ * and material indices need no new check: the sampler reads 0 for a slot past the texture table, and the raster and shading kernels read
+ * material 0 for an object whose material_index is past the material table.
+ * r3_readback_materials copies materials [first, first + n) to the host; blocking. */
+int r3_update_materials(r3_ctx*, const uint32_t* indices_or_null, const r3_material* records, uint32_t n);
+int r3_update_materials_device(r3_ctx*, const uint32_t* d_indices_or_null, const r3_material* d_records, uint32_t n);
+int r3_readback_materials(r3_ctx*, r3_material* out, uint32_t first, uint32_t n);
 /* the bindless d2 texture table the material records index (TextureManager::add / fill, rend3/src/managers/texture.rs;
  * `textures[material.albedo_tex - 1u]`, opaque.wgsl:152-161): descriptors + one blob with every mip level.  Sampling is
  * textureSampleGrad with the linear or nearest Repeat sampler of common/samplers.rs:42-56 (trilinear, no anisotropy). */

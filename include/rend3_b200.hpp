@@ -86,6 +86,11 @@ struct EvalOutput {
     // objects that appear or disappear this frame (ObjectManager::add into a prepared slot / remove): presence bytes (and slots, null =
     // slots 0 .. n-1) in DEVICE memory, their producer ordered on the context's stream; applied at the skinning node before the moves
     const uint32_t* d_presence_slots = nullptr; const uint8_t* d_presence = nullptr; uint32_t n_presence = 0;
+    // materials that change this frame (MaterialManager::update + evaluate's scatter of the stale records): records (and indices, null =
+    // materials 0 .. n-1) in HOST memory (blocking, an index past the table grows it) or in DEVICE memory (enqueue only, records 16-byte
+    // aligned, producer ordered on the context's stream); applied at the skinning node, before the shadow passes read the materials
+    const uint32_t* material_indices = nullptr; const r3_material* material_records = nullptr; uint32_t n_material_updates = 0;
+    const uint32_t* d_material_indices = nullptr; const r3_material* d_material_records = nullptr; uint32_t n_d_material_updates = 0;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -206,6 +211,8 @@ public:
         r.check(r3_set_frame_uniforms(r.raw(), &ev.uniforms));                                       // :142
         if (device_shadow_cameras) r.check(r3_evaluate_shadow_cameras(r.raw(), ev.viewport_location));
         if (device_point_lights) r.check(r3_evaluate_point_lights(r.raw()));                       // renderer/eval.rs:180
+        if (ev.n_material_updates) r.check(r3_update_materials(r.raw(), ev.material_indices, ev.material_records, ev.n_material_updates));
+        if (ev.n_d_material_updates) r.check(r3_update_materials_device(r.raw(), ev.d_material_indices, ev.d_material_records, ev.n_d_material_updates));
         gpu_skinner.add_skinning_to_graph(r, ev);                                                    // :145 state.skinning — before any camera culls
         for (uint32_t i = 0; i < ev.shadows.size(); ++i) {                                          // :148
             if (device_shadow_cameras) r.check(r3_shadow_uniform_upload(r.raw(), i, ev.n_slots, R3_CB_BAKE | R3_CB_CULL));

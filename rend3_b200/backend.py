@@ -45,6 +45,7 @@ ENTRY_POINTS = [
     "set_object_animations", "set_object_pose_jobs", "pose_objects", "readback_objects",
     "set_object_mesh_spheres", "set_object_transforms", "set_object_transforms_device",
     "set_objects_enabled", "set_objects_enabled_device",
+    "update_materials", "update_materials_device", "readback_materials",
 ]
 
 
@@ -247,6 +248,52 @@ class Backend:
         records = np.ascontiguousarray(records)
         assert records.dtype.itemsize == 208
         self._call("set_materials", _ptr(records), C.c_uint32(len(records)))
+
+    # ---- materials that change (MaterialManager::update, evaluate's scatter of the stale records)
+    def update_materials(self, records, indices=None):
+        """Materials 0 .. n-1, or the listed indices, replaced by MATERIAL_DTYPE records from host memory; an index past the table's count
+        grows it.  Blocking."""
+        from .layouts import MATERIAL_DTYPE
+
+        r = np.asarray(records)
+        assert r.ndim == 1 and r.dtype == MATERIAL_DTYPE, "records: a 1-d MATERIAL_DTYPE array"
+        r = np.ascontiguousarray(r)
+        i = None
+        if indices is not None:
+            i = np.asarray(indices)
+            assert i.ndim == 1 and i.dtype.kind in "iu" and len(i) == len(r), "indices: a 1-d integer array as long as records"
+            assert not len(i) or (i.min() >= 0 and i.max() <= 0xFFFFFFFF), "indices: out of the uint32 range"
+            i = np.ascontiguousarray(i, dtype=np.uint32)
+        self._call("update_materials", _ptr(i), _ptr(r) if len(r) else None, C.c_uint32(len(r)))
+
+    def update_materials_device(self, records, indices=None, n: Optional[int] = None):
+        """The same from device memory, enqueue only; indices past the count are dropped.  `records` (uint8 (n, 208) or (n * 208,), or
+        float32 / int32 / uint32 (n, 52): the 208-byte records, 16-byte aligned) and `indices` (int32 / uint32 (n,), None: materials
+        0 .. n-1) are contiguous CUDA tensors, or raw device pointers with `n` given; the caller keeps them alive and orders their
+        producer on stream()."""
+        def pointer(x, what, ok, count):
+            if x is None or isinstance(x, int):
+                return x, None
+            assert getattr(x, "is_cuda", False) and x.is_contiguous() and ok(x), what
+            return x.data_ptr(), count(x)
+        rp, rn = pointer(records, "records: a contiguous CUDA tensor of 208-byte rows (uint8 x 208 or 4-byte x 52), 16-byte aligned",
+                         lambda x: x.numel() * x.element_size() % 208 == 0 and x.data_ptr() % 16 == 0
+                         and (x.element_size() == 1 and not x.is_floating_point() or x.element_size() == 4)
+                         and (x.dim() == 1 or x.dim() == 2 and x.shape[1] * x.element_size() == 208),
+                         lambda x: x.numel() * x.element_size() // 208)
+        ip, inn = pointer(indices, "indices: a contiguous 1-d CUDA tensor of 4-byte integers",
+                          lambda x: x.dim() == 1 and x.element_size() == 4 and not x.is_floating_point(), lambda x: x.numel())
+        n = rn if n is None else n
+        assert n is not None and (inn is None or inn == n) and (rn is None or rn == n), "records and indices differ in length"
+        self._call("update_materials_device", C.c_void_p(ip), C.c_void_p(rp), C.c_uint32(n))
+
+    def readback_materials(self, first: int, n: int):
+        """MATERIAL_DTYPE[n]: materials [first, first + n) of the table the shading reads.  Blocking."""
+        from .layouts import MATERIAL_DTYPE
+
+        out = np.zeros(max(n, 1), dtype=MATERIAL_DTYPE)
+        self._call("readback_materials", _ptr(out), C.c_uint32(first), C.c_uint32(n))
+        return out[:n]
 
     def set_textures(self, descs: np.ndarray, texels: np.ndarray):
         descs = np.ascontiguousarray(descs)

@@ -155,6 +155,9 @@ struct r3_ctx {
     float** d_hiz_ptrs = nullptr; uint32_t* d_hiz_dims = nullptr;
     r3_tri_record* d_tris[4] = {nullptr, nullptr, nullptr, nullptr}; uint64_t tris_cap[4] = {0, 0, 0, 0}; uint64_t n_tris[4] = {0, 0, 0, 0};   // predicted, residual, blend, shadow scratch
     bool any_frag_alpha = false;              // a material discards per fragment (cutout alpha from its albedo texture / vertex colour)
+    std::vector<uint8_t> mat_frag_alpha;      // per material: it discards per fragment (r3_ctx.cu frag_alpha); n_frag_alpha of them set
+    uint32_t n_frag_alpha = 0;
+    bool materials_on_device = false;         // r3_update_materials_device ran since r3_set_materials: any_frag_alpha stays true
     unsigned long long* d_stats = nullptr;    // [8]: [0..3] forward statistics, [4] scratch of r3_compute_max_invocations
     // blend routine: per-sample fragment lists (head = node index + 1, 0 = empty; node = {record, depth bits, next, 0})
     bool any_blend = false;                   // some live object carries material key 2 (TransparencyType::Blend); see sort_blend_slots

@@ -265,14 +265,18 @@ R3_EXPORT int r3_set_objects_device(r3_ctx* c, const void* dptr, uint32_t n) {
     return r3_split_objects(c);   // snapshot of the hot fields: call again after changing the records
 }
 
-__global__ void scatter_objects_kernel(r3_object* dst, const r3_object* src, const uint32_t* slots, uint32_t n, uint32_t n_slots) {
-    // ScatterCopy (rend3/shaders/scatter_copy.wgsl): one 16-byte lane per float4 of the 128-byte record
-    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3, k = threadIdx.x & 7;
+// ScatterCopy (rend3/shaders/scatter_copy.wgsl) of records of Q float4s (8: r3_object, 13: r3_material): entry i copies src record i
+// to dst record idx[i], one 16-byte lane per float4.  blockDim.x must be a multiple of Q, so that a lane's float4 is threadIdx.x % Q.
+template <uint32_t Q>
+__global__ void scatter_records_kernel(float4* dst, const float4* src, const uint32_t* idx, uint32_t n, uint32_t count) {
+    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) / Q, k = threadIdx.x % Q;
     if (i >= n) return;
-    const uint32_t s = slots[i];
-    if (s >= n_slots) return;   // out-of-range writes are dropped (robust buffer access)
-    reinterpret_cast<float4*>(dst)[(size_t)s * 8 + k] = reinterpret_cast<const float4*>(src)[(size_t)i * 8 + k];
+    const uint32_t s = idx[i];
+    if (s >= count) return;   // out-of-range writes are dropped (robust buffer access)
+    dst[(size_t)s * Q + k] = src[(size_t)i * Q + k];
 }
+constexpr uint32_t OBJECT_Q = sizeof(r3_object) / 16, MATERIAL_Q = sizeof(r3_material) / 16;
+static_assert(sizeof(r3_object) == 16 * OBJECT_Q && sizeof(r3_material) == 16 * MATERIAL_Q, "records are whole float4s");
 R3_EXPORT int r3_update_objects(r3_ctx* c, const uint32_t* slots, const r3_object* recs, uint32_t n) {
     if (!c || !slots || !recs) return r3_fail(c, R3_E_INVALID, "update_objects: null");
     if (n == 0) return R3_OK;
@@ -283,8 +287,8 @@ R3_EXPORT int r3_update_objects(r3_ctx* c, const uint32_t* slots, const r3_objec
     uint32_t* d_slots = (uint32_t*)((uint8_t*)c->d_scratch + (size_t)n * sizeof(r3_object));
     R3_CUDA(c, cudaMemcpyAsync(d_recs, recs, (size_t)n * sizeof(r3_object), cudaMemcpyHostToDevice, c->stream));
     R3_CUDA(c, cudaMemcpyAsync(d_slots, slots, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
-    scatter_objects_kernel<<<(n * 8 + 255) / 256, 256, 0, c->stream>>>(c->d_objects, d_recs, d_slots, n, c->n_slots);
-    R3_CHECK_LAUNCH(c, "scatter_objects_kernel");
+    scatter_records_kernel<OBJECT_Q><<<(n * 8 + 255) / 256, 256, 0, c->stream>>>((float4*)c->d_objects, (const float4*)d_recs, d_slots, n, c->n_slots);
+    R3_CHECK_LAUNCH(c, "scatter_records_kernel<8>");
     R3_TRY(r3_split_slots(c, d_slots, n));
     c->max_invocations_valid = false;
     R3_CUDA(c, r3_stream_sync(c));
@@ -354,6 +358,16 @@ R3_EXPORT int r3_set_mesh_buffer(r3_ctx* c, const void* bytes, uint64_t nbytes) 
     c->mesh_words = nbytes / 4;
     return R3_OK;
 }
+// any_frag_alpha (the raster's MODE_ALPHA kernels) follows three facts of each material: its flags, alpha_cutout > 0 and its albedo
+// texture slot.  The host keeps that one bit per material, so that r3_update_materials can keep the count exact.
+static inline uint8_t frag_alpha(const r3_material& m) {
+    return (m.flags & R3_MAT_ALBEDO_ACTIVE) && m.alpha_cutout > 0.0f && (m.textures[R3_TEX_ALBEDO] || (m.flags & R3_MAT_ALBEDO_BLEND)) ? 1 : 0;
+}
+static void material_derive(r3_ctx* c) {
+    // after r3_update_materials_device only the device knows the records: then the MODE_ALPHA kernels run, which give the same image
+    // for materials that never discard (their triangles are not alpha-tested)
+    c->any_frag_alpha = c->materials_on_device || c->n_frag_alpha != 0;
+}
 R3_EXPORT int r3_set_materials(r3_ctx* c, const r3_material* recs, uint32_t n) {
     if (!c || (!recs && n)) return r3_fail(c, R3_E_INVALID, "set_materials: null");
     cudaSetDevice(c->device);
@@ -361,9 +375,94 @@ R3_EXPORT int r3_set_materials(r3_ctx* c, const r3_material* recs, uint32_t n) {
     if (n) R3_CUDA(c, cudaMemcpyAsync(c->d_materials, recs, (size_t)n * sizeof(r3_material), cudaMemcpyHostToDevice, c->stream));
     R3_CUDA(c, r3_stream_sync(c));
     c->n_materials = n;
-    c->any_frag_alpha = false;
-    for (uint32_t i = 0; i < n; ++i)
-        if ((recs[i].flags & R3_MAT_ALBEDO_ACTIVE) && recs[i].alpha_cutout > 0.0f && (recs[i].textures[R3_TEX_ALBEDO] || (recs[i].flags & R3_MAT_ALBEDO_BLEND))) c->any_frag_alpha = true;
+    c->mat_frag_alpha.resize(n);
+    c->n_frag_alpha = 0;
+    for (uint32_t i = 0; i < n; ++i) c->n_frag_alpha += c->mat_frag_alpha[i] = frag_alpha(recs[i]);
+    c->materials_on_device = false;   // the host sees every record again
+    material_derive(c);
+    return R3_OK;
+}
+
+// MaterialManager::update + evaluate's scatter of the stale records (material.rs:163-189, 202-227; util/freelist/buffer.rs)
+static int launch_scatter_materials(r3_ctx* c, const uint32_t* d_idx, const r3_material* d_recs, uint32_t n, uint32_t count) {
+    // 32 records per CTA: 13 full warps
+    scatter_records_kernel<MATERIAL_Q><<<(uint32_t)(((uint64_t)n + 31) / 32), 32 * MATERIAL_Q, 0, c->stream>>>((float4*)c->d_materials, (const float4*)d_recs, d_idx, n, count);
+    R3_CHECK_LAUNCH(c, "scatter_records_kernel<13>");
+    return R3_OK;
+}
+
+R3_EXPORT int r3_update_materials(r3_ctx* c, const uint32_t* indices, const r3_material* recs, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (n == 0) return R3_OK;
+    if (!recs) return r3_fail(c, R3_E_INVALID, "update_materials: null records");
+    uint32_t count = c->n_materials;
+    if (!indices) {
+        if (n > count) return r3_fail(c, R3_E_INVALID, "update_materials: the dense form names materials past the table's count");
+    } else {
+        std::vector<uint32_t> sorted(indices, indices + n);
+        std::sort(sorted.begin(), sorted.end());
+        if (sorted.back() == 0xFFFFFFFFu) return r3_fail(c, R3_E_INVALID, "update_materials: index 0xFFFFFFFF");
+        for (uint32_t i = 1; i < n; ++i)
+            if (sorted[i] == sorted[i - 1]) return r3_fail(c, R3_E_INVALID, "update_materials: one index named twice");
+        if (sorted.back() >= count) count = sorted.back() + 1;   // add_material's growth (material.rs:131-160)
+    }
+    cudaSetDevice(c->device);
+    if (count > c->n_materials) {
+        if (count > c->materials_cap || !c->d_materials) {
+            uint64_t p = 16;
+            while (p < count) p <<= 1;
+            R3_TRY(r3_reserve_t(c, &c->d_materials, &c->materials_cap, p, true));
+        }
+        R3_CUDA(c, cudaMemsetAsync(c->d_materials + c->n_materials, 0, (size_t)(count - c->n_materials) * sizeof(r3_material), c->stream));
+    }
+    if (!indices) {
+        R3_CUDA(c, cudaMemcpyAsync(c->d_materials, recs, (size_t)n * sizeof(r3_material), cudaMemcpyHostToDevice, c->stream));
+    } else {
+        // records then indices, staged on the host so that one copy carries both (the records stay 16-byte aligned on the device)
+        const size_t rec_bytes = (size_t)n * sizeof(r3_material), bytes = rec_bytes + (size_t)n * 4;
+        std::vector<uint8_t> staged(bytes);
+        memcpy(staged.data(), recs, rec_bytes);
+        memcpy(staged.data() + rec_bytes, indices, (size_t)n * 4);
+        R3_TRY(r3_reserve(c, &c->d_scratch, &c->scratch_cap, bytes, 1, false, false));
+        R3_CUDA(c, cudaMemcpyAsync(c->d_scratch, staged.data(), bytes, cudaMemcpyHostToDevice, c->stream));
+        R3_TRY(launch_scatter_materials(c, (const uint32_t*)((uint8_t*)c->d_scratch + rec_bytes), (const r3_material*)c->d_scratch, n, count));
+    }
+    R3_CUDA(c, r3_stream_sync(c));   // host pointers are only borrowed for the call
+    c->mat_frag_alpha.resize(count, 0);
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t m = indices ? indices[i] : i;
+        const uint8_t now = frag_alpha(recs[i]);
+        c->n_frag_alpha += now - c->mat_frag_alpha[m];
+        c->mat_frag_alpha[m] = now;
+    }
+    c->n_materials = count;
+    material_derive(c);
+    return R3_OK;
+}
+
+R3_EXPORT int r3_update_materials_device(r3_ctx* c, const uint32_t* d_indices, const r3_material* d_recs, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (n == 0) return R3_OK;
+    if (!d_recs || ((uintptr_t)d_recs & 15u) || ((uintptr_t)d_indices & 3u))
+        return r3_fail(c, R3_E_INVALID, "update_materials_device: null or misaligned pointer (records: 16 bytes, indices: 4 bytes)");
+    if (!c->n_materials) return r3_fail(c, R3_E_STATE, "update_materials_device: the material table is empty (r3_set_materials first)");
+    if (!d_indices && n > c->n_materials) return r3_fail(c, R3_E_INVALID, "update_materials_device: the dense form names materials past the table's count");
+    cudaSetDevice(c->device);
+    if (!d_indices) R3_CUDA(c, cudaMemcpyAsync(c->d_materials, d_recs, (size_t)n * sizeof(r3_material), cudaMemcpyDeviceToDevice, c->stream));
+    else R3_TRY(launch_scatter_materials(c, d_indices, d_recs, n, c->n_materials));
+    c->materials_on_device = true;   // which materials discard per fragment is now known on the device only
+    material_derive(c);
+    return R3_OK;
+}
+
+R3_EXPORT int r3_readback_materials(r3_ctx* c, r3_material* out, uint32_t first, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (!out && n) return r3_fail(c, R3_E_INVALID, "readback_materials: null");
+    if ((uint64_t)first + n > c->n_materials) return r3_fail(c, R3_E_INVALID, "readback_materials: range outside the material table");
+    if (n == 0) return R3_OK;
+    cudaSetDevice(c->device);
+    R3_CUDA(c, r3_stream_sync(c));
+    R3_CUDA(c, cudaMemcpy(out, c->d_materials + first, (size_t)n * sizeof(r3_material), cudaMemcpyDeviceToHost));
     return R3_OK;
 }
 R3_EXPORT int r3_set_textures(r3_ctx* c, const r3_texture_desc* descs, uint32_t n, const void* texels, uint64_t nbytes) {

@@ -142,7 +142,8 @@ class BaseRenderGraph:
                      upload: bool = True, scissor_rows: Optional[Tuple[int, int]] = None, shadow_filter=None, after_shadows=None,
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
-                     movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None):
+                     movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None,
+                     material_updates=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -169,7 +170,10 @@ class BaseRenderGraph:
         stream — and host arrays through r3_update_point_light_sources, which waits for the stream.  `object_presence` = (slots or None,
         enabled) switches prepared slots on and off at the skinning node, before `object_transforms` (ObjectManager::add into a prepared
         slot / remove): CUDA tensors through r3_set_objects_enabled_device — enqueue only — and host arrays through
-        r3_set_objects_enabled, which waits for the stream."""
+        r3_set_objects_enabled, which waits for the stream.  `material_updates` = (indices or None, records) replaces materials before
+        the first pass that reads them (MaterialManager::update + evaluate's scatter): CUDA tensors through r3_update_materials_device —
+        enqueue only, their producer ordered on the context's stream — and host arrays through r3_update_materials, which waits for the
+        stream.  A transparency change also needs the objects' sort info (r3_update_object_sort_info) before the frame."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -205,6 +209,12 @@ class BaseRenderGraph:
             b.evaluate_point_lights()
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
+        if material_updates is not None:                                          # :145 materials that change, before the shadow passes
+            indices, records = material_updates
+            if getattr(records, "is_cuda", False):
+                b.update_materials_device(records, indices)
+            else:
+                b.update_materials(records, indices)
         if object_presence is not None:                                           # :145 objects that appear or disappear this frame
             slots, enabled = object_presence
             if getattr(enabled, "is_cuda", False):

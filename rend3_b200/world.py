@@ -546,6 +546,9 @@ class EvalOutput:
     # PointLightManager's handle table behind point_buffer: (POINT_LIGHT_SOURCE_DTYPE[n_handles], u8 live[n_handles]), dead handles
     # zero records — what r3_set_point_light_sources takes so that the device evaluates the lights
     point_sources: Optional[Tuple[np.ndarray, np.ndarray]] = None
+    # the material buffer's stale indices since the previous evaluate (MaterialManager::update's use_index, material.rs:163-189), sorted
+    # and distinct: what r3_update_materials scatters from material_buffer instead of r3_set_materials uploading all of it
+    material_stale: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.uint32))
 
 
 class Renderer:
@@ -569,6 +572,7 @@ class Renderer:
         self.obj_reserved = self.STARTING_SIZE
         self.obj_gpu = np.zeros(self.STARTING_SIZE, dtype=OBJECT_DTYPE)
         self.stale: List[int] = []
+        self.material_stale: List[int] = []
         self.dir_lights: List[Optional[DirectionalLight]] = []
         self.point_lights: List[Optional[PointLight]] = []
         self.camera = CameraState(Camera(("raw", glam.identity()), glam.identity()), handedness, aspect_ratio)
@@ -627,6 +631,13 @@ class Renderer:
     def add_material(self, material: PbrMaterial) -> int:
         self.materials.append(material)
         return len(self.materials) - 1
+
+    def update_material(self, handle: int, material: PbrMaterial):
+        """Renderer::update_material (renderer/mod.rs:254-267) -> MaterialManager::update (material.rs:163-189): the material replaces
+        the one at `handle` and its index goes stale in the material buffer.  Objects keep the handle; their sort info follows the new
+        material's key from the next evaluate on."""
+        self.materials[handle] = material
+        self.material_stale.append(handle)
 
     # ---- objects (managers/object.rs:230-293, handle_alloc.rs:46-77)
     def _alloc_object_handle(self) -> int:
@@ -750,6 +761,8 @@ class Renderer:
         mats = np.zeros(max(len(self.materials), 1), dtype=MATERIAL_DTYPE)
         for i, m in enumerate(self.materials):
             mats[i] = m.to_record()
+        material_stale = np.unique(np.asarray(self.material_stale, dtype=np.uint32))
+        self.material_stale = []
 
         # directional lights + shadow atlas (directional.rs:99-157)
         live_lights = [(i, l) for i, l in enumerate(self.dir_lights) if l is not None]
@@ -814,4 +827,5 @@ class Renderer:
             shadow_target_size=size,
             camera=self.camera,
             object_mesh_sphere=mesh_sphere,
+            material_stale=material_stale,
         )
