@@ -1,5 +1,6 @@
 /* r3_anim_check.h — argument checks of r3_set_animations / r3_set_pose_jobs and r3_set_object_animations / r3_set_object_pose_jobs,
- * shared by the library and its CPU oracle so that both reject exactly the same inputs.  Plain C99 / C++, header only.
+ * shared by the library and its CPU oracle so that both reject exactly the same inputs, and of r3_set_joint_matrices.  Plain C99 / C++,
+ * header only.
  *
  * The checks turn the reference's panic sites into errors (rend3-anim/src/lib.rs:166-175, 190; skeleton.rs:151-162):
  *   an empty key channel (`times.len() - 1` underflow), fewer values than key times, a NaN or negative duration (f32::clamp's assert),
@@ -83,6 +84,14 @@ static inline int r3_anim_range_cmp(const void* a, const void* b) {
     return x < y ? -1 : x > y ? 1 : 0;
 }
 
+/* n ranges [r[2i], r[2i + 1]) of the joint buffer, sorted in place by their start: R3_E_INVALID with *msg = overlap_msg when two overlap */
+static inline int r3_anim_check_disjoint(uint64_t* r, uint64_t n, const char* overlap_msg, const char** msg) {
+    qsort(r, n, 2 * sizeof(uint64_t), r3_anim_range_cmp);
+    for (uint64_t i = 1; i < n; ++i)
+        if (r[2 * i] < r[2 * (i - 1) + 1]) { *msg = overlap_msg; return R3_E_INVALID; }
+    return R3_OK;
+}
+
 /* jobs against the skins / clips of the library that is set and a joint buffer of n_joint_matrices matrices */
 static inline int r3_anim_check_jobs(const r3_anim_skin* skins, const r3_anim_clip* clips, uint32_t n_clips, uint32_t n_joint_matrices,
                                      const r3_pose_job* jobs, uint32_t n_jobs, const r3_pose_target* targets, uint32_t n_targets,
@@ -110,10 +119,33 @@ static inline int r3_anim_check_jobs(const r3_anim_skin* skins, const r3_anim_cl
             const r3_pose_target tg = targets[jobs[i].first_target + t];
             if (tg.joint_count) { r[2 * n] = tg.joint_matrix_base_offset; r[2 * n + 1] = (uint64_t)tg.joint_matrix_base_offset + tg.joint_count; ++n; }
         }
-    qsort(r, n, 2 * sizeof(uint64_t), r3_anim_range_cmp);
-    int rc = R3_OK;
-    for (uint64_t i = 1; i < n; ++i)
-        if (r[2 * i] < r[2 * (i - 1) + 1]) { *msg = "set_pose_jobs: two targets write overlapping joint ranges"; rc = R3_E_INVALID; break; }
+    const int rc = r3_anim_check_disjoint(r, n, "set_pose_jobs: two targets write overlapping joint ranges", msg);
+    free(r);
+    return rc;
+}
+
+/* r3_set_joint_matrices' writes against a joint buffer of n_joint_matrices matrices, n_mat4s source matrices and, when with_inverse_binds,
+ * n_inverse_binds inverse binds: every range inside its array (64-bit sums), the destinations of the writes with joint_count > 0 disjoint */
+static inline int r3_anim_check_joint_writes(uint32_t n_joint_matrices, const r3_joint_write* writes, uint32_t n_writes, uint32_t n_mat4s,
+                                             int with_inverse_binds, uint32_t n_inverse_binds, const char** msg) {
+    *msg = "";
+    uint64_t n_ranges = 0;
+    for (uint32_t i = 0; i < n_writes; ++i) {
+        const r3_joint_write w = writes[i];
+        if (w.joint_count == 0) continue;   /* does nothing, wherever it points */
+        if ((uint64_t)w.joint_matrix_base_offset + w.joint_count > n_joint_matrices) { *msg = "set_joint_matrices: destination outside the joint buffer"; return R3_E_INVALID; }
+        if ((uint64_t)w.first_matrix + w.joint_count > n_mat4s) { *msg = "set_joint_matrices: source outside the matrices"; return R3_E_INVALID; }
+        if (with_inverse_binds && (uint64_t)w.first_inverse_bind + w.joint_count > n_inverse_binds) {
+            *msg = "set_joint_matrices: source outside the inverse binds"; return R3_E_INVALID;
+        }
+        n_ranges++;
+    }
+    uint64_t* r = (uint64_t*)malloc(n_ranges ? n_ranges * 2 * sizeof(uint64_t) : 16);
+    if (!r) { *msg = "set_joint_matrices: out of host memory"; return R3_E_INVALID; }
+    uint64_t n = 0;
+    for (uint32_t i = 0; i < n_writes; ++i)
+        if (writes[i].joint_count) { r[2 * n] = writes[i].joint_matrix_base_offset; r[2 * n + 1] = (uint64_t)writes[i].joint_matrix_base_offset + writes[i].joint_count; ++n; }
+    const int rc = r3_anim_check_disjoint(r, n, "set_joint_matrices: two writes' destinations overlap", msg);
     free(r);
     return rc;
 }

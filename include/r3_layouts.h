@@ -385,6 +385,17 @@ typedef struct r3_pose_target {
 } r3_pose_target;
 R3_STATIC_ASSERT(sizeof(r3_pose_target) == 8, "r3_pose_target");
 
+/* One skeleton's joint matrices set by the application (Renderer::set_skeleton_joint_transforms / set_skeleton_joint_matrices,
+ * rend3/src/renderer/mod.rs:302-337, managers/skeleton.rs:151-162), for r3_set_joint_matrices[_device].  The sources are indices, so
+ * several writes may read one range (the armature's primitives posed alike; a crowd sharing one skin's inverse binds). */
+typedef struct r3_joint_write {
+    uint32_t joint_matrix_base_offset;  /* destination: the skeleton's GpuSkinningInput::joint_matrix_base_offset */
+    uint32_t joint_count;               /* matrices written: the skeleton's joint count (set_joint_matrices keeps the first joint_count) */
+    uint32_t first_matrix;              /* source: mat4s[first_matrix .. first_matrix + joint_count) */
+    uint32_t first_inverse_bind;        /* source: inverse_binds[first_inverse_bind ..), read only when the call passes inverse binds */
+} r3_joint_write;
+R3_STATIC_ASSERT(sizeof(r3_joint_write) == 16, "r3_joint_write");
+
 /* ---- object animation: the object-transform half of pose_animation_frame (rend3-anim/src/lib.rs:192-212, posed on the device by
  * r3_pose_objects).  Tracks are r3_anim_track over the key blob of r3_anim_object_library. */
 

@@ -21,7 +21,7 @@
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
- *     r3_update_materials_device, r3_evaluate_shadow_cameras,
+ *     r3_update_materials_device, r3_set_joint_matrices_device, r3_evaluate_shadow_cameras,
  *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
@@ -29,7 +29,7 @@
  *     r3_batch_counts / r3_batching_info / r3_forward_stats / r3_stage_times (small device-to-host reads), and the
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
  *     r3_set_mesh_buffer, r3_set_materials, r3_update_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
- *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_readback_joint_matrices, r3_set_object_animations,
+ *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_set_joint_matrices, r3_readback_joint_matrices, r3_set_object_animations,
  *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_directional_light_sources,
  *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
@@ -315,6 +315,31 @@ int r3_set_pose_jobs(r3_ctx*, const r3_pose_job* jobs, uint32_t n_jobs, const r3
 int r3_pose_skeletons(r3_ctx*);
 int r3_skin_posed(r3_ctx*);
 int r3_readback_joint_matrices(r3_ctx*, float* out /* n x 16 */, uint32_t first, uint32_t n);
+/* Skeletons posed by the application (IK, ragdolls, blended clips, crowd simulations): Renderer::set_skeleton_joint_matrices /
+ * set_skeleton_joint_transforms (rend3/src/renderer/mod.rs:302-337, managers/skeleton.rs:151-162) for many skeletons in one kernel, from
+ * host or device memory, into the resident joint buffer that r3_skin_posed reads.  Write i (r3_joint_write) fills joints
+ * [joint_matrix_base_offset, + joint_count) of the buffer:
+ *   inverse_binds == NULL  set_skeleton_joint_matrices: mat4s[first_matrix + k] copied bit for bit (NaN payloads and -0.0 survive);
+ *   otherwise              set_skeleton_joint_transforms (Skeleton::compute_joint_matrices, rend3-types/src/lib.rs:1233-1239):
+ *                          mat4s[first_matrix + k] * inverse_binds[first_inverse_bind + k], rule R12's Mat4 x Mat4 (DESIGN.md §2), the
+ *                          product r3_pose_skeletons stores, bit for bit.
+ * Matrices are column-major, 16 floats each.  Several writes may read one source range.  A write with joint_count == 0 does nothing
+ * (its offsets are not checked);
+ * ranges no write names keep their matrices; nothing but the joint buffer changes.  On any range the later of this call and
+ * r3_pose_skeletons wins (a ragdoll overriding the clip is written after the pose); r3_set_skeletons replaces the whole buffer.
+ *   r3_set_joint_matrices         host pointers, blocking: one copy, one kernel, one drain.  R3_E_INVALID, nothing written, for a null
+ *                                 pointer whose count is not 0 (writes, mat4s, inverse binds), a destination outside the joint buffer, a
+ *                                 source outside n_mat4s or n_inverse_binds, two writes whose destinations overlap.
+ *   r3_set_joint_matrices_device  the same from DEVICE memory, enqueue only; legal between r3_frame_begin and r3_frame_end (a frame graph
+ *                                 updates its arguments in place).  The counts come from the host; a write whose destination or sources
+ *                                 fall outside them or the joint buffer is dropped whole (robust access, as in the other _device calls);
+ *                                 distinct destinations are a precondition.  mat4s and inverse binds 16-byte aligned, writes 4-byte
+ *                                 aligned (R3_E_INVALID otherwise); producer ordering as for r3_set_object_transforms_device.
+ * R3_E_STATE before r3_set_skeletons.  n_writes == 0 is R3_OK and enqueues nothing. */
+int r3_set_joint_matrices(r3_ctx*, const r3_joint_write* writes, uint32_t n_writes, const float* mat4s, uint32_t n_mat4s,
+                          const float* inverse_binds_or_null, uint32_t n_inverse_binds);
+int r3_set_joint_matrices_device(r3_ctx*, const r3_joint_write* d_writes, uint32_t n_writes, const float* d_mat4s, uint32_t n_mat4s,
+                                 const float* d_inverse_binds_or_null, uint32_t n_inverse_binds);
 
 /* ------------------------------------------------------------------ object animation on the device
  * The object-transform half of rend3-anim's pose_animation_frame (rend3-anim/src/lib.rs:181-212): every posed node's TRS matrix becomes

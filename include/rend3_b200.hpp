@@ -91,6 +91,13 @@ struct EvalOutput {
     // aligned, producer ordered on the context's stream); applied at the skinning node, before the shadow passes read the materials
     const uint32_t* material_indices = nullptr; const r3_material* material_records = nullptr; uint32_t n_material_updates = 0;
     const uint32_t* d_material_indices = nullptr; const r3_material* d_material_records = nullptr; uint32_t n_d_material_updates = 0;
+    // skeletons posed by the application this frame (Renderer::set_skeleton_joint_matrices, or set_skeleton_joint_transforms when inverse
+    // binds are given): writes and matrices in HOST memory (blocking) or in DEVICE memory (enqueue only, matrices 16-byte aligned, producer
+    // ordered on the context's stream); applied at the skinning node after the posed_skinning pose, then r3_skin_posed skins from them
+    const r3_joint_write* joint_writes = nullptr; uint32_t n_joint_writes = 0; const float* joint_mat4s = nullptr; uint32_t n_joint_mat4s = 0;
+    const float* joint_inverse_binds = nullptr; uint32_t n_joint_inverse_binds = 0;
+    const r3_joint_write* d_joint_writes = nullptr; uint32_t n_d_joint_writes = 0; const float* d_joint_mat4s = nullptr; uint32_t n_d_joint_mat4s = 0;
+    const float* d_joint_inverse_binds = nullptr; uint32_t n_d_joint_inverse_binds = 0;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -160,10 +167,15 @@ public:
         if (ev.n_presence) r.check(r3_set_objects_enabled_device(r.raw(), ev.d_presence_slots, ev.d_presence, ev.n_presence));
         if (ev.n_moved) r.check(r3_set_object_transforms_device(r.raw(), ev.d_moved_slots, ev.d_moved_transforms, ev.n_moved));
         if (ev.posed_objects) r.check(r3_pose_objects(r.raw()));
-        if (ev.posed_skinning) {
-            r.check(r3_pose_skeletons(r.raw()));
-            r.check(r3_skin_posed(r.raw()));
-        }
+        if (ev.posed_skinning) r.check(r3_pose_skeletons(r.raw()));
+        // the application's matrices after the clip's pose, so that an override (a ragdoll) wins
+        if (ev.n_joint_writes)
+            r.check(r3_set_joint_matrices(r.raw(), ev.joint_writes, ev.n_joint_writes, ev.joint_mat4s, ev.n_joint_mat4s, ev.joint_inverse_binds,
+                                          ev.n_joint_inverse_binds));
+        if (ev.n_d_joint_writes)
+            r.check(r3_set_joint_matrices_device(r.raw(), ev.d_joint_writes, ev.n_d_joint_writes, ev.d_joint_mat4s, ev.n_d_joint_mat4s,
+                                                 ev.d_joint_inverse_binds, ev.n_d_joint_inverse_binds));
+        if (ev.posed_skinning || ev.n_joint_writes || ev.n_d_joint_writes) r.check(r3_skin_posed(r.raw()));
     }
 };
 

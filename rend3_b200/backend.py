@@ -46,6 +46,7 @@ ENTRY_POINTS = [
     "set_object_mesh_spheres", "set_object_transforms", "set_object_transforms_device",
     "set_objects_enabled", "set_objects_enabled_device",
     "update_materials", "update_materials_device", "readback_materials",
+    "set_joint_matrices", "set_joint_matrices_device",
 ]
 
 
@@ -434,6 +435,48 @@ class Backend:
         out = np.empty((max(n, 1), 16), dtype=np.float32)
         self._call("readback_joint_matrices", _ptr(out), C.c_uint32(first), C.c_uint32(n))
         return out[:n]
+
+    # ---- joint matrices set by the application (Renderer::set_skeleton_joint_matrices / set_skeleton_joint_transforms)
+    def set_joint_matrices(self, writes, mat4s, inverse_binds=None):
+        """JOINT_WRITE_DTYPE writes into the joint buffer from host memory: mat4s ((m, 16) or (m, 4, 4) float32, column-major) copied bit
+        for bit, or times `inverse_binds` (the same shapes) when given.  Blocking."""
+        from .layouts import JOINT_WRITE_DTYPE
+
+        w = np.asarray(writes)
+        assert w.ndim == 1 and w.dtype == JOINT_WRITE_DTYPE, "writes: a 1-d JOINT_WRITE_DTYPE array"
+        w = np.ascontiguousarray(w)
+
+        def mats(x, what):
+            x = np.asarray(x)
+            assert x.dtype == np.float32 and x.ndim in (2, 3) and x.shape[1:] in ((16,), (4, 4)), f"{what}: float32 (m, 16) or (m, 4, 4)"
+            return np.ascontiguousarray(x).reshape(-1, 16)
+        m = mats(mat4s, "mat4s")
+        ib = None if inverse_binds is None else mats(inverse_binds, "inverse_binds")
+        # an empty inverse-bind array still passes a pointer: null selects the copy form
+        self._call("set_joint_matrices", _ptr(w), C.c_uint32(len(w)), _ptr(m), C.c_uint32(len(m)), _ptr(ib), C.c_uint32(0 if ib is None else len(ib)))
+
+    def set_joint_matrices_device(self, writes, mat4s, inverse_binds=None, n_writes: Optional[int] = None, n_mat4s: Optional[int] = None,
+                                  n_inverse_binds: Optional[int] = None):
+        """The same from device memory, enqueue only; writes outside their arrays or the joint buffer are dropped whole.  `writes` (uint8
+        (n, 16) / (n * 16,), or int32 / uint32 (n, 4): JOINT_WRITE_DTYPE records), `mat4s` and `inverse_binds` (float32 (m, 16) or
+        (m, 4, 4), 16-byte aligned) are contiguous CUDA tensors, or raw device pointers with their count given; the caller keeps them alive
+        and orders their producer on stream()."""
+        def pointer(x, count, what, ok, rows):
+            if x is None or isinstance(x, int):
+                assert x is None or count is not None, f"{what}: a raw pointer needs its count"
+                return x, (0 if x is None else count)
+            assert getattr(x, "is_cuda", False) and x.is_contiguous() and ok(x), what
+            return x.data_ptr(), rows(x)
+        wp, wn = pointer(writes, n_writes, "writes: a contiguous CUDA tensor of 16-byte JOINT_WRITE records (uint8 x 16 or 4-byte integers x 4)",
+                         lambda x: not x.is_floating_point() and x.element_size() in (1, 4) and x.numel() * x.element_size() % 16 == 0
+                         and (x.dim() == 1 or x.dim() == 2 and x.shape[1] * x.element_size() == 16),
+                         lambda x: x.numel() * x.element_size() // 16)
+        mat_ok = lambda x: (str(x.dtype) == "torch.float32" and x.data_ptr() % 16 == 0 and x.dim() in (2, 3)
+                            and tuple(x.shape[1:]) in ((16,), (4, 4)))
+        mp, mn = pointer(mat4s, n_mat4s, "mat4s: a contiguous float32 CUDA tensor (m, 16) or (m, 4, 4), 16-byte aligned", mat_ok, lambda x: x.shape[0])
+        ip, inn = pointer(inverse_binds, n_inverse_binds, "inverse_binds: a contiguous float32 CUDA tensor (m, 16) or (m, 4, 4), 16-byte aligned",
+                          mat_ok, lambda x: x.shape[0])
+        self._call("set_joint_matrices_device", C.c_void_p(wp), C.c_uint32(wn), C.c_void_p(mp), C.c_uint32(mn), C.c_void_p(ip), C.c_uint32(inn))
 
     # ---- object animation (the object-transform half of pose_animation_frame, posed on the device)
     def set_object_animations(self, nodes: np.ndarray, clips: np.ndarray, channels: np.ndarray, keys: np.ndarray, left_handed: bool):

@@ -202,6 +202,44 @@ __global__ void __launch_bounds__(R3_ANIM_THREADS) pose_kernel(const r3_pose_job
     }
 }
 
+constexpr uint32_t R3_JOINT_WRITE_THREADS = 256;   // 8 writes per CTA
+
+// set_skeleton_joint_matrices / set_skeleton_joint_transforms (renderer/mod.rs:302-337): one warp per write, lanes striding over its
+// joints, each joint a 64-byte matrix read as four float4s (plus the inverse bind's 64 bytes) and stored as four float4s.  Without inverse
+// binds the float4s are moved untouched, so every bit survives; with them the stored matrix is mat_mul(global, inverse_bind), pose_kernel's
+// product.  A write whose destination or sources leave their arrays is dropped whole (64-bit sums): the host form checked them already,
+// the device form cannot.
+__global__ void __launch_bounds__(R3_JOINT_WRITE_THREADS) joint_write_kernel(const r3_joint_write* __restrict__ writes, uint32_t n_writes,
+                                                                             const float4* __restrict__ mat4s, uint32_t n_mat4s,
+                                                                             const float4* __restrict__ inverse_binds, uint32_t n_inverse_binds,
+                                                                             float4* __restrict__ joint_buf, uint32_t n_joint_mats) {
+    const uint32_t w = blockIdx.x * (R3_JOINT_WRITE_THREADS / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (w >= n_writes) return;
+    const r3_joint_write jw = writes[w];
+    const uint64_t n = jw.joint_count;
+    if (jw.joint_matrix_base_offset + n > n_joint_mats || jw.first_matrix + n > n_mat4s) return;
+    if (inverse_binds && jw.first_inverse_bind + n > n_inverse_binds) return;
+    for (uint32_t k = lane; k < n; k += 32) {
+        const float4* src = mat4s + ((size_t)jw.first_matrix + k) * 4;
+        float4* dst = joint_buf + ((size_t)jw.joint_matrix_base_offset + k) * 4;
+        float4 g[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) g[e] = __ldg(src + e);
+        if (inverse_binds) {
+            const float4* ibp = inverse_binds + ((size_t)jw.first_inverse_bind + k) * 4;
+            float4 ib[4], m[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) ib[e] = __ldg(ibp + e);
+            mat_mul(reinterpret_cast<const float*>(g), reinterpret_cast<const float*>(ib), reinterpret_cast<float*>(m));
+#pragma unroll
+            for (int e = 0; e < 4; ++e) dst[e] = m[e];
+        } else {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) dst[e] = g[e];
+        }
+    }
+}
+
 constexpr uint32_t R3_OBJ_POSE_THREADS = 128;
 
 // The object-transform half of pose_animation_frame (lib.rs:190-212) + set_object_transform (object.rs:302-316), one thread per
@@ -306,6 +344,9 @@ struct r3_anim_state {
     r3_pose_job* d_jobs = nullptr; r3_pose_target* d_targets = nullptr; uint32_t n_jobs = 0;
     uint64_t* d_spill_offset = nullptr; float* d_spill = nullptr; uint32_t smem_bytes = 0;
     uint64_t jobs_cap = 0, targets_cap = 0, spill_offset_cap = 0, spill_cap = 0;   // grow-only (r3_set_pose_jobs runs every frame)
+    // r3_set_joint_matrices' copies of its host arrays, grow-only (the call runs every frame)
+    r3_joint_write* d_jw_writes = nullptr; float4* d_jw_mats = nullptr; float4* d_jw_ibs = nullptr;
+    uint64_t jw_writes_cap = 0, jw_mats_cap = 0, jw_ibs_cap = 0;
     // r3_set_object_animations (independent of the skeletal state above)
     bool has_obj_library = false; uint32_t left_handed = 0;
     std::vector<r3_anim_node_clip> obj_clips;
@@ -328,6 +369,8 @@ struct r3_anim_state {
     void free_jobs() { for (void* p : {(void*)d_jobs, (void*)d_targets, (void*)d_spill_offset, (void*)d_spill}) cudaFree(p);
                        d_jobs = nullptr; d_targets = nullptr; d_spill_offset = nullptr; d_spill = nullptr;
                        jobs_cap = targets_cap = spill_offset_cap = spill_cap = 0; drop_jobs(); }
+    void free_joint_writes() { for (void* p : {(void*)d_jw_writes, (void*)d_jw_mats, (void*)d_jw_ibs}) cudaFree(p);
+                               d_jw_writes = nullptr; d_jw_mats = nullptr; d_jw_ibs = nullptr; jw_writes_cap = jw_mats_cap = jw_ibs_cap = 0; }
     void free_obj_library() { for (void* p : {(void*)d_nodes, (void*)d_node_clips, (void*)d_node_channels, (void*)d_obj_keys}) cudaFree(p);
                               d_nodes = nullptr; d_node_clips = nullptr; d_node_channels = nullptr; d_obj_keys = nullptr;
                               has_obj_library = false; left_handed = 0; obj_clips.clear(); }
@@ -340,7 +383,7 @@ struct r3_anim_state {
 void r3_anim_destroy(r3_ctx* c) {
     if (!c->anim) return;
     c->anim->free_obj_jobs(); c->anim->free_obj_library();
-    c->anim->free_jobs(); c->anim->free_skeletons(); c->anim->free_library();
+    c->anim->free_joint_writes(); c->anim->free_jobs(); c->anim->free_skeletons(); c->anim->free_library();
     delete c->anim;
     c->anim = nullptr;
 }
@@ -491,6 +534,54 @@ R3_EXPORT int r3_readback_joint_matrices(r3_ctx* c, float* out, uint32_t first, 
     R3_CUDA(c, r3_stream_sync(c));
     R3_CUDA(c, cudaMemcpy(out, a->d_joint_buf + (size_t)first * 16, (size_t)n * 64, cudaMemcpyDeviceToHost));
     return R3_OK;
+}
+
+// ------------------------------------------------------------------ joint matrices set by the application (set_skeleton_joint_*)
+static int launch_joint_writes(r3_ctx* c, const r3_joint_write* d_writes, uint32_t n_writes, const float* d_mat4s, uint32_t n_mat4s,
+                               const float* d_inverse_binds, uint32_t n_inverse_binds) {
+    constexpr uint32_t per_cta = R3_JOINT_WRITE_THREADS / 32;
+    r3_anim_state* a = c->anim;
+    joint_write_kernel<<<(uint32_t)(((uint64_t)n_writes + per_cta - 1) / per_cta), R3_JOINT_WRITE_THREADS, 0, c->stream>>>(
+        d_writes, n_writes, reinterpret_cast<const float4*>(d_mat4s), n_mat4s, reinterpret_cast<const float4*>(d_inverse_binds), n_inverse_binds,
+        reinterpret_cast<float4*>(a->d_joint_buf), a->n_joint_mats);
+    R3_CHECK_LAUNCH(c, "joint_write_kernel");
+    return R3_OK;
+}
+
+R3_EXPORT int r3_set_joint_matrices(r3_ctx* c, const r3_joint_write* writes, uint32_t n_writes, const float* mat4s, uint32_t n_mat4s,
+                                    const float* inverse_binds, uint32_t n_inverse_binds) {
+    if (!c) return R3_E_INVALID;
+    r3_anim_state* a = c->anim;
+    if (!a || !a->has_skeletons) return r3_fail(c, R3_E_STATE, "set_joint_matrices before set_skeletons");
+    if ((!writes && n_writes) || (!mat4s && n_mat4s) || (!inverse_binds && n_inverse_binds)) return r3_fail(c, R3_E_INVALID, "set_joint_matrices: null");
+    const char* msg = "";
+    if (r3_anim_check_joint_writes(a->n_joint_mats, writes, n_writes, n_mat4s, inverse_binds != nullptr, n_inverse_binds, &msg) != R3_OK)
+        return r3_fail(c, R3_E_INVALID, msg);
+    if (n_writes == 0) return R3_OK;
+    cudaSetDevice(c->device);
+    R3_TRY(r3_reserve_t(c, &a->d_jw_writes, &a->jw_writes_cap, n_writes));
+    R3_TRY(r3_reserve_t(c, &a->d_jw_mats, &a->jw_mats_cap, std::max<uint64_t>(4ull * n_mat4s, 1u)));
+    if (inverse_binds) R3_TRY(r3_reserve_t(c, &a->d_jw_ibs, &a->jw_ibs_cap, std::max<uint64_t>(4ull * n_inverse_binds, 1u)));
+    R3_CUDA(c, cudaMemcpyAsync(a->d_jw_writes, writes, (size_t)n_writes * sizeof(r3_joint_write), cudaMemcpyHostToDevice, c->stream));
+    if (n_mat4s) R3_CUDA(c, cudaMemcpyAsync(a->d_jw_mats, mat4s, (size_t)n_mat4s * 64, cudaMemcpyHostToDevice, c->stream));
+    if (inverse_binds && n_inverse_binds) R3_CUDA(c, cudaMemcpyAsync(a->d_jw_ibs, inverse_binds, (size_t)n_inverse_binds * 64, cudaMemcpyHostToDevice, c->stream));
+    R3_TRY(launch_joint_writes(c, a->d_jw_writes, n_writes, (const float*)a->d_jw_mats, n_mat4s, inverse_binds ? (const float*)a->d_jw_ibs : nullptr,
+                               n_inverse_binds));
+    R3_CUDA(c, r3_stream_sync(c));                                    // host pointers are only borrowed for the call
+    return R3_OK;
+}
+
+R3_EXPORT int r3_set_joint_matrices_device(r3_ctx* c, const r3_joint_write* d_writes, uint32_t n_writes, const float* d_mat4s, uint32_t n_mat4s,
+                                           const float* d_inverse_binds, uint32_t n_inverse_binds) {
+    if (!c) return R3_E_INVALID;
+    r3_anim_state* a = c->anim;
+    if (!a || !a->has_skeletons) return r3_fail(c, R3_E_STATE, "set_joint_matrices_device before set_skeletons");
+    if (n_writes == 0) return R3_OK;
+    if (!d_writes || (!d_mat4s && n_mat4s) || (!d_inverse_binds && n_inverse_binds) || ((uintptr_t)d_writes & 3u) || ((uintptr_t)d_mat4s & 15u) ||
+        ((uintptr_t)d_inverse_binds & 15u))
+        return r3_fail(c, R3_E_INVALID, "set_joint_matrices_device: null or misaligned pointer (matrices: 16 bytes, writes: 4 bytes)");
+    cudaSetDevice(c->device);
+    return launch_joint_writes(c, d_writes, n_writes, d_mat4s, n_mat4s, d_inverse_binds, n_inverse_binds);
 }
 
 // ------------------------------------------------------------------ object animation (the object-transform half of pose_animation_frame)

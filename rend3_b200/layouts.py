@@ -203,6 +203,8 @@ ANIM_CHANNEL_DTYPE = _dt([("translation", ANIM_TRACK_DTYPE, 0), ("rotation", ANI
 ANIM_CLIP_DTYPE = _dt([("skin", u4, 0), ("first_channel", u4, 4), ("duration", f4, 8)], 16)
 POSE_JOB_DTYPE = _dt([("clip", u4, 0), ("time", f4, 4), ("first_target", u4, 8), ("target_count", u4, 12)], 16)
 POSE_TARGET_DTYPE = _dt([("joint_matrix_base_offset", u4, 0), ("joint_count", u4, 4)], 8)
+# r3_set_joint_matrices[_device]: one skeleton's joint range and where its matrices (and inverse binds) are read from
+JOINT_WRITE_DTYPE = _dt([("joint_matrix_base_offset", u4, 0), ("joint_count", u4, 4), ("first_matrix", u4, 8), ("first_inverse_bind", u4, 12)], 16)
 # object animation (r3_set_object_animations / r3_set_object_pose_jobs); jobs are POSE_JOB_DTYPE records
 ANIM_NODE_DTYPE = _dt([("bind_translation", (f4, 3), 0), ("bind_rotation", (f4, 4), 16), ("bind_scale", (f4, 3), 32)], 48)
 ANIM_NODE_CHANNEL_DTYPE = _dt([("translation", ANIM_TRACK_DTYPE, 0), ("rotation", ANIM_TRACK_DTYPE, 16), ("scale", ANIM_TRACK_DTYPE, 32),

@@ -143,7 +143,7 @@ class BaseRenderGraph:
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
                      movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None,
-                     material_updates=None):
+                     material_updates=None, joint_matrices=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -173,7 +173,12 @@ class BaseRenderGraph:
         r3_set_objects_enabled, which waits for the stream.  `material_updates` = (indices or None, records) replaces materials before
         the first pass that reads them (MaterialManager::update + evaluate's scatter): CUDA tensors through r3_update_materials_device —
         enqueue only, their producer ordered on the context's stream — and host arrays through r3_update_materials, which waits for the
-        stream.  A transparency change also needs the objects' sort info (r3_update_object_sort_info) before the frame."""
+        stream.  A transparency change also needs the objects' sort info (r3_update_object_sort_info) before the frame.
+        `joint_matrices` = (writes, mat4s, inverse_binds or None) sets skeletons' joint matrices at the skinning node
+        (Renderer::set_skeleton_joint_matrices, or set_skeleton_joint_transforms with inverse binds), after the pose of `posed_skinning`
+        so that an application's override (a ragdoll) wins over the clip, and then skins from the resident joint buffer (r3_skin_posed,
+        after r3_set_skeletons): CUDA tensors through r3_set_joint_matrices_device — enqueue only, their producer ordered on the
+        context's stream — and host arrays through r3_set_joint_matrices, which waits for the stream."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -231,6 +236,13 @@ class BaseRenderGraph:
             b.pose_objects()
         if posed_skinning:                                                        # :145 from resident data (r3_set_skeletons / r3_set_pose_jobs)
             b.pose_skeletons()
+        if joint_matrices is not None:                                            # :145 skeletons posed by the application, over the clip
+            writes, mat4s, inverse_binds = joint_matrices
+            if getattr(mat4s, "is_cuda", False):
+                b.set_joint_matrices_device(writes, mat4s, inverse_binds)
+            else:
+                b.set_joint_matrices(writes, mat4s, inverse_binds)
+        if posed_skinning or joint_matrices is not None:
             b.skin_posed()
         mine = [(i, s) for i, s in enumerate(ev.shadows) if shadow_filter is None or shadow_filter(i)]
         for i, s in mine:                                                         # :148

@@ -9,7 +9,14 @@ Workload: --instances instances (default 4096) of a 65-joint humanoid-shaped ski
 of --vertices vertices each (default 1000), one clip with translation, rotation and scale channels of 60 keys on every joint.  The
 instances share the two meshes' source attributes and each skeleton has its own skinned ranges, as SkeletonManager lays them out.
 
-Usage: python tools/bench_animation.py [--instances N] [--vertices V] [--objects K] [--iters I] [--warmup W]"""
+With --joint-writes the line gains "joint_writes": skeletons posed by the application (set_skeleton_joint_transforms) for 1 %, 10 % and
+100 % of the skeletons per frame (--joint-write-fractions), each a write of 65 globals times the skin's shared inverse binds.  Per
+fraction: the device time of joint_write_kernel (192 B per joint: 64 B matrix + 64 B inverse bind read, 64 B written) against the
+3.35 TB/s data-sheet bandwidth, the host time of one call, and the frame rate and early flushes of --frames frame graphs that hold the
+skinning node — r3_set_joint_matrices (host form) or r3_set_joint_matrices_device, then r3_skin_posed — against r3_skin of the whole
+host joint array.
+
+Usage: python tools/bench_animation.py [--instances N] [--vertices V] [--objects K] [--iters I] [--warmup W] [--joint-writes]"""
 import argparse
 import json
 import math
@@ -128,6 +135,83 @@ def object_bench(args, b, device_ms):
             "device_pose_equals_oracle": same}
 
 
+def joint_write_bench(args, b, recs, buf, device_ms):
+    """r3_set_joint_matrices[_device] (set_skeleton_joint_transforms: globals times the skin's shared inverse binds) for a fraction of the
+    skeletons per frame, against r3_skin of the whole host joint array.  Frames are recorded as frame graphs (r3_frame_begin / end) that
+    hold the skinning node only: the write (or r3_skin) and r3_skin_posed."""
+    import torch
+    from rend3_b200.layouts import JOINT_WRITE_DTYPE
+
+    rng = np.random.default_rng(3)
+    n_skel, nj = len(recs), 65
+    binds = rng.uniform(-1, 1, (nj, 16)).astype(f32)
+    full = rng.uniform(-1, 1, (len(buf), 16)).astype(f32)   # what r3_skin uploads every frame
+    reps = args.frames
+
+    def frames(fn):
+        """frames per second of `reps` frame graphs back to back, and early flushes per frame"""
+        fn()
+        b.sync()
+        before = b.frame_graph_stats()["flushed"]
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            b.frame_begin()
+            fn()
+            b.frame_end()
+        b.sync()
+        dt = time.perf_counter() - t0
+        return reps / dt, (b.frame_graph_stats()["flushed"] - before) / reps
+
+    def host_ms(fn, n=50):
+        fn()
+        b.sync()
+        t0 = time.perf_counter()
+        for _ in range(n):
+            fn()
+        ms = (time.perf_counter() - t0) * 1e3 / n
+        b.sync()
+        return ms
+
+    skin_fps, skin_flush = frames(lambda: b.skin(recs, full))
+    out = {"skeletons": n_skel, "joints_per_skeleton": nj, "frames_per_measure": reps,
+           "r3_skin_host_matrices": {"fps": round(skin_fps, 1), "early_flushes_per_frame": skin_flush, "bytes_uploaded_per_frame": full.nbytes},
+           "fractions": {}}
+    for frac in args.joint_write_fractions:
+        n = max(1, round(frac * n_skel))
+        chosen = np.sort(rng.choice(n_skel, n, replace=False))
+        writes = np.zeros(n, dtype=JOINT_WRITE_DTYPE)
+        writes["joint_matrix_base_offset"] = recs["joint_matrix_base_offset"][chosen]
+        writes["joint_count"] = nj
+        writes["first_matrix"] = nj * np.arange(n)
+        mats = rng.uniform(-1, 1, (n * nj, 16)).astype(f32)
+        dw, dm, db = (torch.from_numpy(a).cuda() for a in (writes.view(np.int32).reshape(-1, 4), mats, binds))
+        torch.cuda.synchronize()
+        host_call = lambda: b.set_joint_matrices(writes, mats, binds)
+        dev_call = lambda: b.set_joint_matrices_device(dw, dm, db)
+        b.set_skeletons(recs, buf)   # both forms start from the same buffer
+        host_call()
+        via_host = b.readback_joint_matrices(0, len(buf))
+        b.set_skeletons(recs, buf)
+        dev_call()
+        same = bool(np.array_equal(b.readback_joint_matrices(0, len(buf)).view(np.uint32), via_host.view(np.uint32)))
+        kernel_ms = device_ms(dev_call)
+        joints = n * nj
+        host_fps, host_flush = frames(lambda: (host_call(), b.skin_posed()))
+        dev_fps, dev_flush = frames(lambda: (dev_call(), b.skin_posed()))
+        out["fractions"][str(frac)] = {
+            "skeletons_written": n, "joints_written": joints,
+            "kernel_ms": round(kernel_ms, 5), "bytes_per_joint": 192,
+            "kernel_bytes_per_s": 192 * joints / (kernel_ms * 1e-3),
+            "share_of_3_35_tb_s": 192 * joints / (kernel_ms * 1e-3) / 3.35e12,
+            "host_form": {"call_host_ms": round(host_ms(host_call), 4), "fps": round(host_fps, 1), "early_flushes_per_frame": host_flush,
+                          "bytes_uploaded_per_frame": writes.nbytes + mats.nbytes + binds.nbytes},
+            "device_form": {"call_host_ms": round(host_ms(dev_call, 200), 4), "fps": round(dev_fps, 1), "early_flushes_per_frame": dev_flush},
+            "device_equals_host": same,
+        }
+        del dw, dm, db
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--instances", type=int, default=4096)
@@ -135,6 +219,9 @@ def main():
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--objects", type=int, default=0, help="posed objects per instance (0: skeletons only)")
+    ap.add_argument("--joint-writes", action="store_true", help="also time r3_set_joint_matrices[_device] against r3_skin (frame graphs)")
+    ap.add_argument("--joint-write-fractions", type=lambda s: [float(x) for x in s.split(",")], default=[0.01, 0.1, 1.0])
+    ap.add_argument("--frames", type=int, default=50, help="frame graphs per frame-rate measurement (--joint-writes)")
     args = ap.parse_args()
 
     import torch
@@ -217,6 +304,7 @@ def main():
     same = bool(np.array_equal(orc.readback_joint_matrices(0, len(buf)).view(np.uint32), posed.view(np.uint32)))
     orc.close()
     objects = object_bench(args, b, device_ms) if args.objects > 0 else None
+    joint_writes = joint_write_bench(args, b, recs, buf, device_ms) if args.joint_writes else None
     b.close()
 
     model = pose_bytes(jobs, targets, data.library, 60)
@@ -234,6 +322,7 @@ def main():
                              "joint_bytes_uploaded_per_frame": 64 * len(buf)},
         "device_pose_equals_oracle": same,
         **({"objects": objects} if objects is not None else {}),
+        **({"joint_writes": joint_writes} if joint_writes is not None else {}),
     }))
 
 
