@@ -305,6 +305,27 @@ typedef struct r3_skinning_input {
 } r3_skinning_input;
 R3_STATIC_ASSERT(sizeof(r3_skinning_input) == 40, "GpuSkinningInput");
 
+/* One mesh of a deformable set (r3_set_deformable_meshes): where MeshBuilder::build put its attributes and indices in the mesh buffer
+ * (rend3-types/src/lib.rs:477-512, managers/mesh.rs:123-184) and which of them build computed from the positions.  r3_deform_meshes
+ * writes the positions and recomputes what the flags name, as rebuilding the mesh from the new positions would. */
+#define R3_DEFORM_LEFT_HANDED 0x1u           /* the renderer's handedness is Left: face normal edge1 x edge2 (else edge2 x edge1) */
+#define R3_DEFORM_NORMALS 0x2u               /* built without normals: calculate_normals_for_buffers (lib.rs:662-702) */
+#define R3_DEFORM_TANGENTS 0x4u              /* built without tangents and with uv0: calculate_tangents_for_buffers (lib.rs:784-836) */
+typedef struct r3_deformable_mesh {
+    uint32_t position_offset;     /* @0  byte offsets in the mesh buffer, R3_ATTR_ABSENT if missing */
+    uint32_t normal_offset;       /* @4 */
+    uint32_t tangent_offset;      /* @8 */
+    uint32_t uv0_offset;          /* @12 */
+    uint32_t first_index;         /* @16 the objects' first_index (a word index) and index_count; indices local to the mesh */
+    uint32_t index_count;         /* @20 */
+    uint32_t vertex_count;        /* @24 */
+    uint32_t flags;               /* @28 R3_DEFORM_* */
+} r3_deformable_mesh;
+R3_STATIC_ASSERT(sizeof(r3_deformable_mesh) == 32, "r3_deformable_mesh");
+R3_STATIC_ASSERT(offsetof(r3_deformable_mesh, uv0_offset) == 12, "uv0_offset");
+R3_STATIC_ASSERT(offsetof(r3_deformable_mesh, first_index) == 16, "first_index");
+R3_STATIC_ASSERT(offsetof(r3_deformable_mesh, flags) == 28, "flags");
+
 /* ---- skeletal animation (rend3-anim/src/lib.rs:37-263, posed on the device by r3_pose_skeletons) */
 #define R3_ANIM_NO_PARENT 0xFFFFFFFFu        /* the joint's node has no parent: global = local (lib.rs:253-255) */
 #define R3_ANIM_PARENT_NOT_JOINT 0xFFFFFFFEu /* the parent node is not a joint of the skin: global = IDENTITY * local (lib.rs:249) */

@@ -21,7 +21,7 @@
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
- *     r3_update_materials_device, r3_set_joint_matrices_device, r3_evaluate_shadow_cameras,
+ *     r3_update_materials_device, r3_set_joint_matrices_device, r3_deform_meshes_device, r3_evaluate_shadow_cameras,
  *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
@@ -30,7 +30,8 @@
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
  *     r3_set_mesh_buffer, r3_set_materials, r3_update_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_set_joint_matrices, r3_readback_joint_matrices, r3_set_object_animations,
- *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_directional_light_sources,
+ *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_deformable_meshes,
+ *     r3_deform_meshes, r3_set_directional_light_sources,
  *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
@@ -176,6 +177,46 @@ int r3_set_object_transforms_device(r3_ctx*, const uint32_t* d_slots_or_null, co
 int r3_set_objects_enabled(r3_ctx*, const uint32_t* slots_or_null, const uint8_t* enabled, uint32_t n);
 int r3_set_objects_enabled_device(r3_ctx*, const uint32_t* d_slots_or_null, const uint8_t* d_enabled, uint32_t n);
 int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);               /* eval_output.mesh_buffer (mesh.rs:99) */
+/* Meshes that deform every frame (cloth, flags, a water grid, soft bodies, blend shapes evaluated by a CUDA kernel), from host or device
+ * memory.  rend3's meshes are immutable: the reference rebuilds such a mesh each frame (MeshBuilder::build recomputes smooth normals and
+ * tangents, rend3-types/src/lib.rs:477-512, 617-837; MeshManager::add recomputes BoundingSphere::from_mesh, mesh.rs:169) and re-adds its
+ * objects (ObjectManager::add, object.rs:267-284: a new world sphere, and the sort location becomes its centre).  Here the mesh stays
+ * where it is and one call rewrites, for every mesh of the set, exactly what that rebuild and re-add would produce, bit for bit: the
+ * positions, the normals and tangents the build computed (R3_DEFORM_NORMALS / R3_DEFORM_TANGENTS), the mesh sphere, and for every listed
+ * object slot its mesh sphere, world sphere (record, cull + bake's copies and centre bit) and sort location = the world sphere's centre.
+ * Transform, rows, affine bit, `enabled`, key and flags stay.  Arithmetic: rule R15 (DESIGN.md §2).  The one departure is slot
+ * identity: a re-add would take a new handle and delete the old one a frame later; the image is the same.
+ *   r3_set_deformable_meshes            blocking, once per set: n_meshes r3_deformable_mesh records and n_objects (slot, mesh) pairs.  It
+ *                                       reads the meshes' indices back from the device, checks everything and uploads each mesh's vertex
+ *                                       -> corner lists (a stable counting sort by vertex, in triangle order).  R3_E_INVALID, the context
+ *                                       unchanged, for: a null pointer with a non-zero count; unknown flag bits; an offset that is not a
+ *                                       multiple of 4; position_offset absent; R3_DEFORM_NORMALS without normal_offset; R3_DEFORM_TANGENTS
+ *                                       without tangent_offset, uv0_offset or normal_offset; a range outside the mesh buffer; index_count
+ *                                       not a multiple of 3; an index >= vertex_count; more than 2^31 - 1 vertices or 2^32 - 1 indices in
+ *                                       the set; written ranges (positions, and normals / tangents when recomputed) that overlap each other
+ *                                       or a read range of the set (indices, uv0 and authored normals when tangents are recomputed); an
+ *                                       object mesh >= n_meshes; a slot named twice or at or past the slot count; a slot whose record does
+ *                                       not draw its mesh (first_index, index_count and attr_offset[POSITION] differ).  R3_E_STATE before
+ *                                       r3_set_objects and while the object buffer is borrowed.  n_meshes == 0 removes the set.
+ *   r3_deform_meshes                    host positions: sum(vertex_count) x 3 floats, mesh after mesh in set order (n_floats must be that
+ *                                       count, R3_E_INVALID otherwise).  One copy, the kernels, one drain.
+ *   r3_deform_meshes_device             the same from DEVICE memory, enqueue only; legal between r3_frame_begin and r3_frame_end (a frame
+ *                                       graph updates its arguments in place).  d_positions 4-byte aligned and n_floats as above
+ *                                       (R3_E_INVALID otherwise); producer ordering as for r3_set_object_transforms_device.
+ *   r3_readback_deformable_mesh_spheres blocking: the mesh spheres (centre, radius) of meshes [first, first + n) from the last deform
+ *                                       (zeros before it); R3_E_INVALID past the set.
+ * Every call deforms every mesh of the set.  R3_E_STATE from both deform calls: before a set exists; after r3_set_mesh_buffer; after an
+ * r3_update_mesh_buffer that writes into one of the set's index ranges (call r3_set_deformable_meshes again); while the object buffer is
+ * borrowed (r3_set_objects_device); while r3_set_object_mesh_spheres does not cover every listed slot; while a listed slot is at or past
+ * the slot count.  Both start a new frame epoch; the host batching's mirror of the locations is refreshed in the drain it makes anyway, as
+ * after a move.  Ordering: r3_set_object_transforms* after a deform in the same frame gives the move's location with the new mesh sphere
+ * (set_object_transform after add); r3_pose_objects takes its targets' own mesh spheres, so on a slot both posed and deformed the later
+ * call wins; r3_skin / r3_skin_posed after a deform skins from the new positions. */
+int r3_set_deformable_meshes(r3_ctx*, const r3_deformable_mesh* meshes, uint32_t n_meshes,
+                             const uint32_t* object_slots, const uint32_t* object_meshes, uint32_t n_objects);
+int r3_deform_meshes(r3_ctx*, const float* positions, uint64_t n_floats);
+int r3_deform_meshes_device(r3_ctx*, const float* d_positions, uint64_t n_floats);
+int r3_readback_deformable_mesh_spheres(r3_ctx*, float* out /* n x 4 */, uint32_t first, uint32_t n);
 /* MeshManager::add (mesh.rs:123-184): write nbytes at byte_offset of the megabuffer (both multiples of 4).  A write past the end extends it;
  * words between the old end and byte_offset read 0.  The allocation grows to the next power of two, keeping its contents (also what
  * r3_skin wrote) — MeshManager::reallocate_buffers (mesh.rs:264-308). */

@@ -98,6 +98,11 @@ struct EvalOutput {
     const float* joint_inverse_binds = nullptr; uint32_t n_joint_inverse_binds = 0;
     const r3_joint_write* d_joint_writes = nullptr; uint32_t n_d_joint_writes = 0; const float* d_joint_mat4s = nullptr; uint32_t n_d_joint_mat4s = 0;
     const float* d_joint_inverse_binds = nullptr; uint32_t n_d_joint_inverse_binds = 0;
+    // meshes that deform this frame (the set of r3_set_deformable_meshes rebuilt from new positions, its objects re-added): 3 floats per
+    // vertex of the set, mesh after mesh, in HOST memory (blocking) or in DEVICE memory (enqueue only, 4-byte aligned, producer ordered on
+    // the context's stream); applied first at the skinning node, so that a move wins the location and skinning reads the new positions
+    const float* deform_positions = nullptr; uint64_t n_deform_floats = 0;
+    const float* d_deform_positions = nullptr; uint64_t n_d_deform_floats = 0;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -163,6 +168,8 @@ public:
 class GpuSkinner {   // skinning.rs:54-199: add_skinning_to_graph — skinned positions / normals / tangents into the skeletons' overridden mesh ranges
 public:
     void add_skinning_to_graph(Renderer& r, const EvalOutput& ev) const {
+        if (ev.n_deform_floats) r.check(r3_deform_meshes(r.raw(), ev.deform_positions, ev.n_deform_floats));
+        if (ev.n_d_deform_floats) r.check(r3_deform_meshes_device(r.raw(), ev.d_deform_positions, ev.n_d_deform_floats));
         if (ev.n_skeletons) r.check(r3_skin(r.raw(), ev.skinning_inputs, ev.n_skeletons, ev.joint_matrices, ev.n_joints));
         if (ev.n_presence) r.check(r3_set_objects_enabled_device(r.raw(), ev.d_presence_slots, ev.d_presence, ev.n_presence));
         if (ev.n_moved) r.check(r3_set_object_transforms_device(r.raw(), ev.d_moved_slots, ev.d_moved_transforms, ev.n_moved));

@@ -47,6 +47,7 @@ ENTRY_POINTS = [
     "set_objects_enabled", "set_objects_enabled_device",
     "update_materials", "update_materials_device", "readback_materials",
     "set_joint_matrices", "set_joint_matrices_device",
+    "set_deformable_meshes", "deform_meshes", "deform_meshes_device", "readback_deformable_mesh_spheres",
 ]
 
 
@@ -477,6 +478,46 @@ class Backend:
         ip, inn = pointer(inverse_binds, n_inverse_binds, "inverse_binds: a contiguous float32 CUDA tensor (m, 16) or (m, 4, 4), 16-byte aligned",
                           mat_ok, lambda x: x.shape[0])
         self._call("set_joint_matrices_device", C.c_void_p(wp), C.c_uint32(wn), C.c_void_p(mp), C.c_uint32(mn), C.c_void_p(ip), C.c_uint32(inn))
+
+    # ---- meshes that deform every frame (rebuild of the mesh + re-add of its objects, on the device)
+    def set_deformable_meshes(self, meshes, object_slots=None, object_meshes=None):
+        """DEFORMABLE_MESH_DTYPE records and the (slot, mesh) pairs of the objects that draw them.  Blocking."""
+        from .layouts import DEFORMABLE_MESH_DTYPE
+
+        m = np.asarray(meshes)
+        assert m.ndim == 1 and m.dtype == DEFORMABLE_MESH_DTYPE, "meshes: a 1-d DEFORMABLE_MESH_DTYPE array"
+        m = np.ascontiguousarray(m)
+        s = np.ascontiguousarray(np.zeros(0) if object_slots is None else object_slots, dtype=np.uint32).reshape(-1)
+        o = np.ascontiguousarray(np.zeros(0) if object_meshes is None else object_meshes, dtype=np.uint32).reshape(-1)
+        assert len(s) == len(o), "object_slots and object_meshes: one mesh per slot"
+        self._call("set_deformable_meshes", _ptr(m) if len(m) else None, C.c_uint32(len(m)), _ptr(s) if len(s) else None,
+                   _ptr(o) if len(o) else None, C.c_uint32(len(s)))
+
+    def deform_meshes(self, positions):
+        """New positions of every mesh of the set from host memory: float32 (sum(vertex_count), 3), mesh after mesh.  Blocking."""
+        p = np.asarray(positions)
+        assert p.dtype == np.float32 and p.ndim == 2 and p.shape[1] == 3, "positions: float32 (n, 3)"
+        p = np.ascontiguousarray(p)
+        self._call("deform_meshes", _ptr(p) if p.size else None, C.c_uint64(p.size))
+
+    def deform_meshes_device(self, positions, n_floats: Optional[int] = None):
+        """The same from device memory, enqueue only: a contiguous float32 CUDA tensor (n, 3), or a raw device pointer with n_floats
+        given; the caller keeps it alive and orders its producer on stream()."""
+        if isinstance(positions, int):
+            assert n_floats is not None, "positions: a raw pointer needs n_floats"
+            ptr, n = positions, n_floats
+        else:
+            assert getattr(positions, "is_cuda", False) and positions.is_contiguous() and str(positions.dtype) == "torch.float32" \
+                and positions.dim() == 2 and positions.shape[1] == 3 and positions.data_ptr() % 4 == 0, \
+                "positions: a contiguous float32 CUDA tensor (n, 3)"
+            ptr, n = positions.data_ptr(), positions.numel()
+        self._call("deform_meshes_device", C.c_void_p(ptr), C.c_uint64(n))
+
+    def readback_deformable_mesh_spheres(self, first: int, n: int) -> np.ndarray:
+        """(n, 4) mesh spheres (centre, radius) of the set's meshes [first, first + n) from the last deform"""
+        out = np.zeros((max(n, 1), 4), dtype=np.float32)
+        self._call("readback_deformable_mesh_spheres", _ptr(out), C.c_uint32(first), C.c_uint32(n))
+        return out[:n]
 
     # ---- object animation (the object-transform half of pose_animation_frame, posed on the device)
     def set_object_animations(self, nodes: np.ndarray, clips: np.ndarray, channels: np.ndarray, keys: np.ndarray, left_handed: bool):

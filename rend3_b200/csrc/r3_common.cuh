@@ -91,6 +91,7 @@ struct r3_camera {
 };
 
 struct r3_anim_state;                        // skeletal animation + resident skinning data (r3_animation.cu)
+struct r3_deform_state;                      // the deformable mesh set (r3_mesh_deform.cu)
 
 struct r3_tri_record { float xyw[3][3]; uint32_t object_id; uint32_t vid[3]; uint32_t _pad[3]; };   // 64 B
 static_assert(sizeof(r3_tri_record) == 64, "triangle record");
@@ -168,6 +169,7 @@ struct r3_ctx {
     r3_peer_state peer;
     uint32_t tri_shard_index = 0, tri_shard_count = 1;   // r3_set_cull_shard
     r3_anim_state* anim = nullptr;            // created by the first r3_set_animations / r3_set_skeletons
+    r3_deform_state* deform = nullptr;        // created by the first r3_set_deformable_meshes
     // frame graph
     bool capturing = false;                   // between r3_frame_begin and the submission (or an early flush)
     cudaGraphExec_t frame_exec[2] = {nullptr, nullptr};   // instantiated graphs of even / odd frames (the culling buffers ping-pong), updated in place
@@ -258,6 +260,10 @@ int r3_grow_mesh_spheres(r3_ctx* c, uint32_t n);   // r3_resize_objects: zero sp
 void r3_presence_set_host(r3_ctx* c, const uint32_t* slots, const uint8_t* enabled, uint32_t n);
 void r3_presence_derive(r3_ctx* c);
 int r3_reserve_point_buffer(r3_ctx* c, uint32_t n_lights);   // r3_lights.cu: room for n lights in c->d_point, contents kept
+// r3_mesh_deform.cu: free c->deform (r3_ctx_destroy); a mesh-buffer write that invalidates the set's corner lists (r3_set_mesh_buffer:
+// every byte; r3_update_mesh_buffer: [offset, offset + nbytes), which matters when it meets one of the set's index ranges)
+void r3_deform_destroy(r3_ctx* c);
+void r3_deform_note_mesh_write(r3_ctx* c, bool whole_buffer, uint64_t byte_offset, uint64_t nbytes);
 
 #ifdef __CUDACC__
 // Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine
@@ -273,6 +279,21 @@ __device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, 
 __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
 __device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
 __device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+// BoundingSphere::apply_transform (util/frustum.rs:22-32), rule R12's object half: Vec3::length_squared of each axis, f32::max (fmaxf
+// ignores a NaN operand as it does), sqrt; centre = matrix * (c, 1) in mul_vec4's order; radius = max_scale * r.  x, y, z: the xyz of the
+// matrix's four columns; ms: the mesh sphere (centre, radius).  Shared by r3_set_object_transforms and r3_deform_meshes.
+__device__ __forceinline__ float4 sphere_apply_transform_rn(const float (&x)[4], const float (&y)[4], const float (&z)[4], const float4& ms) {
+    float ls[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) ls[c] = add_rn(add_rn(mul_rn(x[c], x[c]), mul_rn(y[c], y[c])), mul_rn(z[c], z[c]));
+    const float max_scale = __fsqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
+    float4 sph;
+    sph.x = add_rn(add_rn(add_rn(mul_rn(x[0], ms.x), mul_rn(x[1], ms.y)), mul_rn(x[2], ms.z)), mul_rn(x[3], 1.0f));
+    sph.y = add_rn(add_rn(add_rn(mul_rn(y[0], ms.x), mul_rn(y[1], ms.y)), mul_rn(y[2], ms.z)), mul_rn(y[3], 1.0f));
+    sph.z = add_rn(add_rn(add_rn(mul_rn(z[0], ms.x), mul_rn(z[1], ms.y)), mul_rn(z[2], ms.z)), mul_rn(z[3], 1.0f));
+    sph.w = mul_rn(max_scale, ms.w);
+    return sph;
+}
 // M * (x, y, z, w): column-major, accumulated x,y,z,w like WGSL's mat4x4*vec4
 __device__ __forceinline__ float4 mat_vec_rn(const float* __restrict__ m, float x, float y, float z, float w) {
     float4 r;

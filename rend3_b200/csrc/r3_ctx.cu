@@ -80,6 +80,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     if (c->side_stream) cudaStreamSynchronize(c->side_stream);
     r3_peer_destroy(c);
     r3_anim_destroy(c);
+    r3_deform_destroy(c);
     if (!c->objects_borrowed) cudaFree(c->d_objects);
     cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_hot_radius); cudaFree(c->d_centre_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
     cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc); cudaFree(c->d_gsort_keys[0]); cudaFree(c->d_gsort_keys[1]); cudaFree(c->d_gsort_hist); cudaFree(c->d_gsort_header);
@@ -352,6 +353,7 @@ R3_EXPORT int r3_set_object_sort_info(r3_ctx* c, const uint64_t* key, const uint
 R3_EXPORT int r3_set_mesh_buffer(r3_ctx* c, const void* bytes, uint64_t nbytes) {
     if (!c || (!bytes && nbytes) || (nbytes & 3)) return r3_fail(c, R3_E_INVALID, "set_mesh_buffer: bad size");
     cudaSetDevice(c->device);
+    r3_deform_note_mesh_write(c, true, 0, nbytes);   // the deformable set's indices are gone
     R3_TRY(r3_reserve_t(c, &c->d_mesh, &c->mesh_cap, nbytes / 4 + 4));
     if (nbytes) R3_CUDA(c, cudaMemcpyAsync(c->d_mesh, bytes, nbytes, cudaMemcpyHostToDevice, c->stream));
     R3_CUDA(c, r3_stream_sync(c));
@@ -510,6 +512,7 @@ R3_EXPORT int r3_update_mesh_buffer(r3_ctx* c, uint64_t byte_offset, const void*
     if (!bytes || (byte_offset & 3) || (nbytes & 3)) return r3_fail(c, R3_E_INVALID, "update_mesh_buffer: offset and size must be multiples of 4");
     if (byte_offset + nbytes < byte_offset || (byte_offset + nbytes) / 4 + 4 > (1ull << 62)) return r3_fail(c, R3_E_INVALID, "update_mesh_buffer: range overflows");
     cudaSetDevice(c->device);
+    r3_deform_note_mesh_write(c, false, byte_offset, nbytes);   // new indices under the deformable set's corner lists
     uint64_t cap = c->d_mesh ? c->mesh_cap * 4 : 0, used = c->mesh_words * 4;
     void* p = c->d_mesh;
     const int rc = blob_write(c, &p, &cap, &used, byte_offset, bytes, nbytes, 16);   // >= 4 words of slack, as r3_set_mesh_buffer keeps

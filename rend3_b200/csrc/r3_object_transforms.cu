@@ -50,17 +50,8 @@ object_transforms_kernel(const float4* __restrict__ mats, const uint32_t* __rest
         }
         const uint32_t a = __ballot_sync(0xFFFFFFFFu, ok && __float_as_uint(col.w) == affine_w_bits(k));
         const bool affine = ((a >> first) & 0xFu) == 0xFu;
-        // BoundingSphere::apply_transform: Vec3::length_squared of each axis, f32::max (fmaxf ignores a NaN operand as it does), sqrt;
-        // centre = matrix * (c, 1) in mul_vec4's order; radius = max_scale * r.  Every lane of the object evaluates it (zeros when !ok).
-        float ls[3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) ls[c] = add_rn(add_rn(mul_rn(x[c], x[c]), mul_rn(y[c], y[c])), mul_rn(z[c], z[c]));
-        const float max_scale = __fsqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
-        float4 sph;
-        sph.x = add_rn(add_rn(add_rn(mul_rn(x[0], ms.x), mul_rn(x[1], ms.y)), mul_rn(x[2], ms.z)), mul_rn(x[3], 1.0f));
-        sph.y = add_rn(add_rn(add_rn(mul_rn(y[0], ms.x), mul_rn(y[1], ms.y)), mul_rn(y[2], ms.z)), mul_rn(y[3], 1.0f));
-        sph.z = add_rn(add_rn(add_rn(mul_rn(z[0], ms.x), mul_rn(z[1], ms.y)), mul_rn(z[2], ms.z)), mul_rn(z[3], 1.0f));
-        sph.w = mul_rn(max_scale, ms.w);
+        // BoundingSphere::apply_transform; every lane of the object evaluates it (zeros when !ok)
+        const float4 sph = sphere_apply_transform_rn(x, y, z, ms);
         // the four lanes of an object agree, so the ballot carries each object's centre bit four times
         const uint32_t cb = __ballot_sync(0xFFFFFFFFu, ok && centre_is_translation(sph.x, sph.y, sph.z, x[3], y[3], z[3]));
         const bool centred = (cb >> first) & 1u;

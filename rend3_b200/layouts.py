@@ -205,6 +205,10 @@ POSE_JOB_DTYPE = _dt([("clip", u4, 0), ("time", f4, 4), ("first_target", u4, 8),
 POSE_TARGET_DTYPE = _dt([("joint_matrix_base_offset", u4, 0), ("joint_count", u4, 4)], 8)
 # r3_set_joint_matrices[_device]: one skeleton's joint range and where its matrices (and inverse binds) are read from
 JOINT_WRITE_DTYPE = _dt([("joint_matrix_base_offset", u4, 0), ("joint_count", u4, 4), ("first_matrix", u4, 8), ("first_inverse_bind", u4, 12)], 16)
+# r3_set_deformable_meshes: where one mesh's attributes and indices are and what MeshBuilder::build computed (DEFORM_* flags)
+DEFORMABLE_MESH_DTYPE = _dt([("position_offset", u4, 0), ("normal_offset", u4, 4), ("tangent_offset", u4, 8), ("uv0_offset", u4, 12),
+                             ("first_index", u4, 16), ("index_count", u4, 20), ("vertex_count", u4, 24), ("flags", u4, 28)], 32)
+DEFORM_LEFT_HANDED, DEFORM_NORMALS, DEFORM_TANGENTS = 0x1, 0x2, 0x4
 # object animation (r3_set_object_animations / r3_set_object_pose_jobs); jobs are POSE_JOB_DTYPE records
 ANIM_NODE_DTYPE = _dt([("bind_translation", (f4, 3), 0), ("bind_rotation", (f4, 4), 16), ("bind_scale", (f4, 3), 32)], 48)
 ANIM_NODE_CHANNEL_DTYPE = _dt([("translation", ANIM_TRACK_DTYPE, 0), ("rotation", ANIM_TRACK_DTYPE, 16), ("scale", ANIM_TRACK_DTYPE, 32),

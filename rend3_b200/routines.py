@@ -143,7 +143,7 @@ class BaseRenderGraph:
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
                      movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None,
-                     material_updates=None, joint_matrices=None):
+                     material_updates=None, joint_matrices=None, mesh_deforms=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -178,7 +178,13 @@ class BaseRenderGraph:
         (Renderer::set_skeleton_joint_matrices, or set_skeleton_joint_transforms with inverse binds), after the pose of `posed_skinning`
         so that an application's override (a ragdoll) wins over the clip, and then skins from the resident joint buffer (r3_skin_posed,
         after r3_set_skeletons): CUDA tensors through r3_set_joint_matrices_device — enqueue only, their producer ordered on the
-        context's stream — and host arrays through r3_set_joint_matrices, which waits for the stream."""
+        context's stream — and host arrays through r3_set_joint_matrices, which waits for the stream.
+        `mesh_deforms` = positions ((n, 3) float32, every mesh of the set made by r3_set_deformable_meshes, mesh after mesh) deforms the
+        set at the skinning node (the rebuild of each mesh and the re-add of its objects): before `skinning`, `object_presence`,
+        `object_transforms`, `posed_objects` and the skeletons, so that a move in the same frame wins the location (set_object_transform
+        after add) and a deformed skinning base is skinned from the new positions.  A CUDA tensor goes through r3_deform_meshes_device —
+        enqueue only, its producer ordered on the context's stream — and a host array through r3_deform_meshes, which waits for the
+        stream."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -212,6 +218,11 @@ class BaseRenderGraph:
                 b.update_point_light_sources(handles, sources, live)
         if device_point_lights or point_light_updates is not None:                # PointLightManager::evaluate (renderer/eval.rs:180)
             b.evaluate_point_lights()
+        if mesh_deforms is not None:                                              # :145 meshes rebuilt from new positions, objects re-added
+            if getattr(mesh_deforms, "is_cuda", False):
+                b.deform_meshes_device(mesh_deforms)
+            else:
+                b.deform_meshes(mesh_deforms)
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
         if material_updates is not None:                                          # :145 materials that change, before the shadow passes

@@ -75,6 +75,10 @@ class Mesh:
     attributes: List[Tuple[int, np.ndarray]]
     vertex_count: int
     indices: np.ndarray
+    # how MeshBuilder::build made it, for a mesh that is later rebuilt from new positions (r3_set_deformable_meshes' flags)
+    left_handed: bool = True
+    normals_calculated: bool = False
+    tangents_calculated: bool = False
 
 
 class MeshBuilder:
@@ -128,7 +132,8 @@ class MeshBuilder:
         if self.uv0 is not None:
             normals = next(a for slot, a in attrs if slot == 1)
             attrs.append((2, calculate_tangents(self.positions, normals, self.uv0, indices)))
-        return Mesh(attrs, n, indices)
+        return Mesh(attrs, n, indices, left_handed=self.handedness == LEFT, normals_calculated=self.normals is None,
+                    tangents_calculated=self.uv0 is not None)
 
 
 def calculate_normals(positions: np.ndarray, indices: np.ndarray, left_handed: bool) -> np.ndarray:
@@ -593,7 +598,9 @@ class Renderer:
         self.mesh_words = np.concatenate(words)
         center, radius = bounding_sphere_from_mesh(mesh.attributes[0][1])
         self.meshes.append(
-            dict(ranges=ranges, index_start=index_start, index_count=len(mesh.indices), center=center, radius=radius)
+            dict(ranges=ranges, index_start=index_start, index_count=len(mesh.indices), center=center, radius=radius,
+                 vertex_count=mesh.vertex_count, left_handed=mesh.left_handed, normals_calculated=mesh.normals_calculated,
+                 tangents_calculated=mesh.tangents_calculated)
         )
         return len(self.meshes) - 1
 
