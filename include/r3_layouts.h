@@ -326,6 +326,33 @@ R3_STATIC_ASSERT(offsetof(r3_deformable_mesh, uv0_offset) == 12, "uv0_offset");
 R3_STATIC_ASSERT(offsetof(r3_deformable_mesh, first_index) == 16, "first_index");
 R3_STATIC_ASSERT(offsetof(r3_deformable_mesh, flags) == 28, "flags");
 
+/* One mesh of a remeshable set (r3_set_remeshable_meshes): a mesh whose topology changes every frame (an isosurface, a voxel chunk, a
+ * fractured or cut mesh).  Its ranges in the mesh buffer are sized by the capacities; each remesh writes the first vertex_count entries
+ * of every range and the first index_count indices, as MeshBuilder::build + MeshManager::add of the new vertices and indices would.
+ * flags: R3_DEFORM_*, with the same meaning as in r3_deformable_mesh. */
+typedef struct r3_remeshable_mesh {
+    uint32_t position_offset;     /* @0  byte offsets in the mesh buffer, R3_ATTR_ABSENT if missing */
+    uint32_t normal_offset;       /* @4 */
+    uint32_t tangent_offset;      /* @8 */
+    uint32_t uv0_offset;          /* @12 */
+    uint32_t color0_offset;       /* @16 4 bytes per vertex */
+    uint32_t first_index;         /* @20 the objects' first_index (a word index); indices local to the mesh */
+    uint32_t index_capacity;      /* @24 */
+    uint32_t vertex_capacity;     /* @28 */
+    uint32_t flags;               /* @32 R3_DEFORM_* */
+    uint32_t _pad[3];             /* @36 */
+} r3_remeshable_mesh;
+R3_STATIC_ASSERT(sizeof(r3_remeshable_mesh) == 48, "r3_remeshable_mesh");
+R3_STATIC_ASSERT(offsetof(r3_remeshable_mesh, color0_offset) == 16, "color0_offset");
+R3_STATIC_ASSERT(offsetof(r3_remeshable_mesh, first_index) == 20, "first_index");
+R3_STATIC_ASSERT(offsetof(r3_remeshable_mesh, flags) == 32, "flags");
+/* per-mesh status of the last remesh (r3_readback_remesh_status): Mesh::validate's reasons (rend3-types/src/lib.rs:533-567), the first
+ * that applies */
+#define R3_REMESH_APPLIED 0u
+#define R3_REMESH_OVER_CAPACITY 1u           /* vertex_count > vertex_capacity or index_count > index_capacity */
+#define R3_REMESH_NOT_TRIANGLES 2u           /* index_count % 3 != 0 */
+#define R3_REMESH_INDEX_OUT_OF_RANGE 3u      /* an index >= vertex_count */
+
 /* ---- skeletal animation (rend3-anim/src/lib.rs:37-263, posed on the device by r3_pose_skeletons) */
 #define R3_ANIM_NO_PARENT 0xFFFFFFFFu        /* the joint's node has no parent: global = local (lib.rs:253-255) */
 #define R3_ANIM_PARENT_NOT_JOINT 0xFFFFFFFEu /* the parent node is not a joint of the skin: global = IDENTITY * local (lib.rs:249) */

@@ -21,7 +21,7 @@
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
- *     r3_update_materials_device, r3_set_joint_matrices_device, r3_deform_meshes_device, r3_evaluate_shadow_cameras,
+ *     r3_update_materials_device, r3_set_joint_matrices_device, r3_deform_meshes_device, r3_remesh_meshes_device, r3_evaluate_shadow_cameras,
  *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
@@ -31,7 +31,7 @@
  *     r3_set_mesh_buffer, r3_set_materials, r3_update_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_set_joint_matrices, r3_readback_joint_matrices, r3_set_object_animations,
  *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_deformable_meshes,
- *     r3_deform_meshes, r3_set_directional_light_sources,
+ *     r3_deform_meshes, r3_set_remeshable_meshes, r3_remesh_meshes, r3_readback_remesh_status, r3_set_directional_light_sources,
  *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
@@ -184,27 +184,28 @@ int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);            
  * where it is and one call rewrites, for every mesh of the set, exactly what that rebuild and re-add would produce, bit for bit: the
  * positions, the normals and tangents the build computed (R3_DEFORM_NORMALS / R3_DEFORM_TANGENTS), the mesh sphere, and for every listed
  * object slot its mesh sphere, world sphere (record, cull + bake's copies and centre bit) and sort location = the world sphere's centre.
- * Transform, rows, affine bit, `enabled`, key and flags stay.  Arithmetic: rule R15 (DESIGN.md §2).  The one departure is slot
+ * Transform, rows, affine bit, `enabled`, index_count, key and flags stay.  Arithmetic: rule R15 (DESIGN.md §2).  The one departure is slot
  * identity: a re-add would take a new handle and delete the old one a frame later; the image is the same.
  *   r3_set_deformable_meshes            blocking, once per set: n_meshes r3_deformable_mesh records and n_objects (slot, mesh) pairs.  It
- *                                       reads the meshes' indices back from the device, checks everything and uploads each mesh's vertex
- *                                       -> corner lists (a stable counting sort by vertex, in triangle order).  R3_E_INVALID, the context
+ *                                       reads the meshes' indices back from the device, checks everything and builds each mesh's vertex
+ *                                       -> corner lists on the device (a stable radix sort by vertex, in triangle order).  R3_E_INVALID, the context
  *                                       unchanged, for: a null pointer with a non-zero count; unknown flag bits; an offset that is not a
  *                                       multiple of 4; position_offset absent; R3_DEFORM_NORMALS without normal_offset; R3_DEFORM_TANGENTS
  *                                       without tangent_offset, uv0_offset or normal_offset; a range outside the mesh buffer; index_count
- *                                       not a multiple of 3; an index >= vertex_count; more than 2^31 - 1 vertices or 2^32 - 1 indices in
+ *                                       not a multiple of 3; an index >= vertex_count; more than 2^31 - 1 vertices or 2^32 - 2^11 indices in
  *                                       the set; written ranges (positions, and normals / tangents when recomputed) that overlap each other
  *                                       or a read range of the set (indices, uv0 and authored normals when tangents are recomputed); an
  *                                       object mesh >= n_meshes; a slot named twice or at or past the slot count; a slot whose record does
  *                                       not draw its mesh (first_index, index_count and attr_offset[POSITION] differ).  R3_E_STATE before
- *                                       r3_set_objects and while the object buffer is borrowed.  n_meshes == 0 removes the set.
+ *                                       r3_set_objects and while the object buffer is borrowed.  n_meshes == 0 removes the set.  A context
+ *                                       holds one dynamic-mesh set: this call replaces a set of r3_set_remeshable_meshes, and the reverse.
  *   r3_deform_meshes                    host positions: sum(vertex_count) x 3 floats, mesh after mesh in set order (n_floats must be that
  *                                       count, R3_E_INVALID otherwise).  One copy, the kernels, one drain.
  *   r3_deform_meshes_device             the same from DEVICE memory, enqueue only; legal between r3_frame_begin and r3_frame_end (a frame
  *                                       graph updates its arguments in place).  d_positions 4-byte aligned and n_floats as above
  *                                       (R3_E_INVALID otherwise); producer ordering as for r3_set_object_transforms_device.
  *   r3_readback_deformable_mesh_spheres blocking: the mesh spheres (centre, radius) of meshes [first, first + n) from the last deform
- *                                       (zeros before it); R3_E_INVALID past the set.
+ *                                       or remesh (zeros before it), of whichever set is current; R3_E_INVALID past the set.
  * Every call deforms every mesh of the set.  R3_E_STATE from both deform calls: before a set exists; after r3_set_mesh_buffer; after an
  * r3_update_mesh_buffer that writes into one of the set's index ranges (call r3_set_deformable_meshes again); while the object buffer is
  * borrowed (r3_set_objects_device); while r3_set_object_mesh_spheres does not cover every listed slot; while a listed slot is at or past
@@ -217,6 +218,57 @@ int r3_set_deformable_meshes(r3_ctx*, const r3_deformable_mesh* meshes, uint32_t
 int r3_deform_meshes(r3_ctx*, const float* positions, uint64_t n_floats);
 int r3_deform_meshes_device(r3_ctx*, const float* d_positions, uint64_t n_floats);
 int r3_readback_deformable_mesh_spheres(r3_ctx*, float* out /* n x 4 */, uint32_t first, uint32_t n);
+/* Meshes whose topology changes every frame (marching-cubes isosurfaces, voxel terrain chunks being dug into, fracture and cutting, holes
+ * opening in cloth, GPU decimation), from host or device memory.  The reference rebuilds such a mesh each frame (MeshBuilder::build,
+ * MeshManager::add) and re-adds its objects.  Here each mesh owns ranges sized by its capacities (r3_remeshable_mesh) and one call writes,
+ * for every mesh of the set, what that rebuild and re-add of the new vertices and indices would produce, bit for bit under rule R15: the
+ * first vertex_count entries of every attribute range, the first index_count indices, the recomputed normals and tangents and the mesh
+ * sphere; for every listed slot what a deform writes (mesh sphere, world sphere, sort location) and the record's new index_count.
+ * Entries past the counts stay as they were and are never drawn.  The vertex -> corner lists are rebuilt on the device by every call.
+ *   r3_set_remeshable_meshes     blocking, once per set.  Checks everything before it writes anything; R3_E_INVALID, the context
+ *                                unchanged, for: a null pointer with a non-zero count; the flag and offset rules of
+ *                                r3_set_deformable_meshes (color0_offset included); a capacity-sized range outside the mesh buffer; written
+ *                                ranges (every present attribute, and the indices) that overlap; more than 2^31 - 1 vertices or 2^32 - 2^11
+ *                                indices of capacity in the set; an object mesh >= n_meshes; a slot named twice or at or past the slot
+ *                                count; a listed record that does not draw its mesh (first_index, the position, normal, tangent, uv0 and
+ *                                color0 offsets differ, or index_count > index_capacity).  R3_E_STATE before r3_set_objects and while the
+ *                                object buffer is borrowed.  n_meshes == 0 removes the set.  The set replaces a set of
+ *                                r3_set_deformable_meshes, and the reverse; the calls of the set that is not current return R3_E_STATE.
+ *                                The listed slots' index_capacity is kept as a floor of the invocation bound that sizes the culling
+ *                                buffers, so a remesh back up to capacity never outgrows them.  Counts in force before the first remesh
+ *                                read 0.
+ *   r3_remesh_meshes             host streams: counts (n_meshes x {vertex_count, index_count}), positions (3 floats per vertex), indices,
+ *                                and normals (3), tangents (3), uv0 (2) and color0 (one 4-byte word) per vertex.  Every vertex stream is
+ *                                laid out at capacity strides: mesh i starts at the sum of the earlier meshes' vertex_capacity;
+ *                                indices likewise by index_capacity.  n_vertices and n_indices must be the set's total capacities.  A
+ *                                mesh's normals are read when it has a normal range and does not recompute them (R3_DEFORM_NORMALS
+ *                                unset), tangents likewise, uv0 and color0 whenever it has those ranges; a null stream that some mesh
+ *                                reads is R3_E_INVALID.  Mesh::validate (rend3-types/src/lib.rs:533-567) on every mesh: a count above
+ *                                its capacity, index_count % 3 != 0 or an index >= vertex_count rejects the whole call with
+ *                                R3_E_INVALID, nothing written.  One copy per stream, the kernels, one drain.
+ *   r3_remesh_meshes_device      the same from DEVICE memory (4-byte aligned), enqueue only; legal between r3_frame_begin and
+ *                                r3_frame_end, producer ordering as for r3_set_object_transforms_device.  The counts vary on the device
+ *                                while every launch keeps its grid, so a frame graph keeps its topology.  Validation cannot return an
+ *                                error here: a failing mesh and its objects are left exactly as they were (what a failed build leaves),
+ *                                its status word records the first reason (R3_REMESH_*), and the other meshes are applied.
+ *   r3_readback_remesh_status    blocking: status words of meshes [first, first + n) from the last remesh and, when counts_or_null is
+ *                                given, the counts in force (n x {vertex_count, index_count}).  R3_E_INVALID past the set.
+ * R3_E_STATE from both remesh calls: before a set exists; after r3_set_mesh_buffer; while the object buffer is borrowed; while
+ * r3_set_object_mesh_spheres does not cover every listed slot; while a listed slot is at or past the slot count.  An
+ * r3_update_mesh_buffer into the set's ranges invalidates nothing.  Both calls start a new frame epoch.  A later r3_update_objects of a
+ * listed slot writes the host's index_count until the next remesh.  Remeshed meshes are not skinning bases: a skeleton whose ranges lie in
+ * the set reads stale vertices. */
+int r3_set_remeshable_meshes(r3_ctx*, const r3_remeshable_mesh* meshes, uint32_t n_meshes,
+                             const uint32_t* object_slots, const uint32_t* object_meshes, uint32_t n_objects);
+int r3_remesh_meshes(r3_ctx*, const uint32_t* counts, const float* positions, const uint32_t* indices, const float* normals,
+                     const float* tangents, const float* uv0, const uint32_t* color0, uint64_t n_vertices, uint64_t n_indices);
+int r3_remesh_meshes_device(r3_ctx*, const uint32_t* d_counts, const float* d_positions, const uint32_t* d_indices, const float* d_normals,
+                            const float* d_tangents, const float* d_uv0, const uint32_t* d_color0, uint64_t n_vertices, uint64_t n_indices);
+int r3_readback_remesh_status(r3_ctx*, uint32_t* status, uint32_t* counts_or_null /* n x 2 */, uint32_t first, uint32_t n);
+/* Test hook: the invocation bound the culling buffers are sized with, computed now if stale: out[0] = sum over the slots of
+ * round_up(max(index_count, floor) / 3, 256), out[1] = the largest term; the floor is a listed slot's index_capacity while a remeshable
+ * set exists, else 0. */
+int r3_debug_invocation_bound(r3_ctx*, uint64_t out[2]);
 /* MeshManager::add (mesh.rs:123-184): write nbytes at byte_offset of the megabuffer (both multiples of 4).  A write past the end extends it;
  * words between the old end and byte_offset read 0.  The allocation grows to the next power of two, keeping its contents (also what
  * r3_skin wrote) — MeshManager::reallocate_buffers (mesh.rs:264-308). */

@@ -103,6 +103,15 @@ struct EvalOutput {
     // the context's stream); applied first at the skinning node, so that a move wins the location and skinning reads the new positions
     const float* deform_positions = nullptr; uint64_t n_deform_floats = 0;
     const float* d_deform_positions = nullptr; uint64_t n_d_deform_floats = 0;
+    // meshes whose topology changes this frame (the set of r3_set_remeshable_meshes rebuilt from new vertices and indices, its objects
+    // re-added): the streams of r3_remesh_meshes at capacity strides, in HOST memory (blocking) or in DEVICE memory (enqueue only, 4-byte
+    // aligned, producer ordered on the context's stream); applied where the deform is (a context holds one of the two sets), when
+    // `counts` is set
+    struct RemeshStreams {
+        const uint32_t* counts = nullptr; const float* positions = nullptr; const uint32_t* indices = nullptr; const float* normals = nullptr;
+        const float* tangents = nullptr; const float* uv0 = nullptr; const uint32_t* color0 = nullptr; uint64_t n_vertices = 0, n_indices = 0;
+    };
+    RemeshStreams remesh, d_remesh;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -170,6 +179,10 @@ public:
     void add_skinning_to_graph(Renderer& r, const EvalOutput& ev) const {
         if (ev.n_deform_floats) r.check(r3_deform_meshes(r.raw(), ev.deform_positions, ev.n_deform_floats));
         if (ev.n_d_deform_floats) r.check(r3_deform_meshes_device(r.raw(), ev.d_deform_positions, ev.n_d_deform_floats));
+        if (const EvalOutput::RemeshStreams& s = ev.remesh; s.counts)
+            r.check(r3_remesh_meshes(r.raw(), s.counts, s.positions, s.indices, s.normals, s.tangents, s.uv0, s.color0, s.n_vertices, s.n_indices));
+        if (const EvalOutput::RemeshStreams& s = ev.d_remesh; s.counts)
+            r.check(r3_remesh_meshes_device(r.raw(), s.counts, s.positions, s.indices, s.normals, s.tangents, s.uv0, s.color0, s.n_vertices, s.n_indices));
         if (ev.n_skeletons) r.check(r3_skin(r.raw(), ev.skinning_inputs, ev.n_skeletons, ev.joint_matrices, ev.n_joints));
         if (ev.n_presence) r.check(r3_set_objects_enabled_device(r.raw(), ev.d_presence_slots, ev.d_presence, ev.n_presence));
         if (ev.n_moved) r.check(r3_set_object_transforms_device(r.raw(), ev.d_moved_slots, ev.d_moved_transforms, ev.n_moved));

@@ -48,6 +48,7 @@ ENTRY_POINTS = [
     "update_materials", "update_materials_device", "readback_materials",
     "set_joint_matrices", "set_joint_matrices_device",
     "set_deformable_meshes", "deform_meshes", "deform_meshes_device", "readback_deformable_mesh_spheres",
+    "set_remeshable_meshes", "remesh_meshes", "remesh_meshes_device", "readback_remesh_status", "debug_invocation_bound",
 ]
 
 
@@ -518,6 +519,71 @@ class Backend:
         out = np.zeros((max(n, 1), 4), dtype=np.float32)
         self._call("readback_deformable_mesh_spheres", _ptr(out), C.c_uint32(first), C.c_uint32(n))
         return out[:n]
+
+    # ---- meshes whose topology changes every frame (rebuild of the mesh from new vertices and indices + re-add of its objects, on the device)
+    def set_remeshable_meshes(self, meshes, object_slots=None, object_meshes=None):
+        """REMESHABLE_MESH_DTYPE records and the (slot, mesh) pairs of the objects that draw them.  Blocking."""
+        from .layouts import REMESHABLE_MESH_DTYPE
+
+        m = np.asarray(meshes)
+        assert m.ndim == 1 and m.dtype == REMESHABLE_MESH_DTYPE, "meshes: a 1-d REMESHABLE_MESH_DTYPE array"
+        m = np.ascontiguousarray(m)
+        s = np.ascontiguousarray(np.zeros(0) if object_slots is None else object_slots, dtype=np.uint32).reshape(-1)
+        o = np.ascontiguousarray(np.zeros(0) if object_meshes is None else object_meshes, dtype=np.uint32).reshape(-1)
+        assert len(s) == len(o), "object_slots and object_meshes: one mesh per slot"
+        self._call("set_remeshable_meshes", _ptr(m) if len(m) else None, C.c_uint32(len(m)), _ptr(s) if len(s) else None,
+                   _ptr(o) if len(o) else None, C.c_uint32(len(s)))
+
+    _REMESH_STREAMS = (("counts", "uint32", 2), ("positions", "float32", 3), ("indices", "uint32", None), ("normals", "float32", 3),
+                       ("tangents", "float32", 3), ("uv0", "float32", 2), ("color0", "uint32", None))
+
+    @staticmethod
+    def _remesh_arrays(arrays, dtype_of, is_ok):
+        """checks each stream's shape and dtype: counts (n_meshes, 2) uint32, positions / normals / tangents (n_vertices, 3) float32, uv0
+        (n_vertices, 2) float32, indices and color0 1-d uint32 (color0 one packed word per vertex); int32 is taken for uint32 (a negative
+        value fails validation); returns (n_vertices, n_indices)"""
+        n_v = n_i = None
+        for (name, dt, cols), a in zip(Backend._REMESH_STREAMS, arrays):
+            if a is None:
+                assert name not in ("counts", "positions", "indices"), f"{name}: required"
+                continue
+            shape = tuple(a.shape)
+            assert is_ok(a) and dtype_of(a) in ((dt, "int32") if dt == "uint32" else (dt,)) and (len(shape) == 1 if cols is None else (len(shape) == 2 and shape[1] == cols)), \
+                f"{name}: a contiguous {dt} array of shape {'(n,)' if cols is None else f'(n, {cols})'}"
+            if name == "indices":
+                n_i = shape[0]
+            elif name != "counts":
+                assert n_v is None or n_v == shape[0], f"{name}: one row per vertex, as positions"
+                n_v = shape[0]
+        return n_v, n_i
+
+    def remesh_meshes(self, counts, positions, indices, normals=None, tangents=None, uv0=None, color0=None):
+        """New counts, vertices and indices of every mesh of the set from host memory, at capacity strides (see r3_remesh_meshes).
+        Blocking; R3_E_INVALID, nothing written, when a mesh fails Mesh::validate."""
+        arrays = [None if a is None else np.ascontiguousarray(a) for a in (counts, positions, indices, normals, tangents, uv0, color0)]
+        n_v, n_i = self._remesh_arrays(arrays, lambda a: str(a.dtype), lambda a: True)
+        self._call("remesh_meshes", *[None if a is None or a.size == 0 else _ptr(a) for a in arrays], C.c_uint64(n_v), C.c_uint64(n_i))
+
+    def remesh_meshes_device(self, counts, positions, indices, normals=None, tangents=None, uv0=None, color0=None):
+        """The same from device memory, enqueue only: contiguous CUDA tensors (4-byte aligned) of the host form's shapes and dtypes; the
+        caller keeps them alive and orders their producer on stream().  A mesh that fails Mesh::validate is left as it was and reported
+        by readback_remesh_status."""
+        arrays = (counts, positions, indices, normals, tangents, uv0, color0)
+        n_v, n_i = self._remesh_arrays(arrays, lambda a: str(a.dtype).replace("torch.", ""),
+                                       lambda a: getattr(a, "is_cuda", False) and a.is_contiguous() and a.data_ptr() % 4 == 0)
+        self._call("remesh_meshes_device", *[C.c_void_p(None if a is None else a.data_ptr()) for a in arrays], C.c_uint64(n_v), C.c_uint64(n_i))
+
+    def readback_remesh_status(self, first: int, n: int):
+        """(status (n,) uint32: REMESH_* of the last remesh, counts (n, 2) uint32: the {vertex_count, index_count} in force)"""
+        status, counts = np.zeros(max(n, 1), np.uint32), np.zeros((max(n, 1), 2), np.uint32)
+        self._call("readback_remesh_status", _ptr(status), _ptr(counts), C.c_uint32(first), C.c_uint32(n))
+        return status[:n], counts[:n]
+
+    def debug_invocation_bound(self):
+        """Test hook: (sum, largest) of the per-slot invocation terms the culling buffers are sized with"""
+        out = (C.c_uint64 * 2)()
+        self._call("debug_invocation_bound", out)
+        return int(out[0]), int(out[1])
 
     # ---- object animation (the object-transform half of pose_animation_frame, posed on the device)
     def set_object_animations(self, nodes: np.ndarray, clips: np.ndarray, channels: np.ndarray, keys: np.ndarray, left_handed: bool):

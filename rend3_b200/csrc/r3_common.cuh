@@ -91,7 +91,7 @@ struct r3_camera {
 };
 
 struct r3_anim_state;                        // skeletal animation + resident skinning data (r3_animation.cu)
-struct r3_deform_state;                      // the deformable mesh set (r3_mesh_deform.cu)
+struct r3_deform_state;                      // the dynamic-mesh set: deformable or remeshable (r3_mesh_deform.cu)
 
 struct r3_tri_record { float xyw[3][3]; uint32_t object_id; uint32_t vid[3]; uint32_t _pad[3]; };   // 64 B
 static_assert(sizeof(r3_tri_record) == 64, "triangle record");
@@ -126,6 +126,9 @@ struct r3_ctx {
     uint32_t* d_gsort_header = nullptr; int gsort_src = 0; uint32_t gsort_n = 0; bool gsort_valid = false; float gsort_loc[3] = {0, 0, 0};
     uint64_t gsort_epoch = 0, gsort_sorted_epoch = ~0ull; uint32_t gsort_cameras_this_epoch = 0, gsort_cameras_last_epoch = 0;
     uint64_t max_total_invocations = 0, max_object_invocations = 0; bool max_invocations_valid = false;   // sum / max over all slots of round_up(tris, 256)
+    // per-slot floor of the index_count those bounds take (a remeshable set's index_capacity; r3_mesh_deform.cu), only while such a set
+    // exists: a remesh can grow a record's index_count back up to it without the host seeing the records
+    uint32_t* d_invocation_floor = nullptr; uint32_t n_invocation_floor = 0, invocation_floor_cap = 0;
     uint32_t* d_mesh = nullptr; uint64_t mesh_words = 0, mesh_cap = 0;
     r3_material* d_materials = nullptr; uint32_t n_materials = 0, materials_cap = 0;
     bool has_skybox = false; r3_texture_desc sky_desc{}; uint8_t* d_sky_texels = nullptr; uint64_t sky_cap = 0;   // cube map of the skybox routine
@@ -169,7 +172,7 @@ struct r3_ctx {
     r3_peer_state peer;
     uint32_t tri_shard_index = 0, tri_shard_count = 1;   // r3_set_cull_shard
     r3_anim_state* anim = nullptr;            // created by the first r3_set_animations / r3_set_skeletons
-    r3_deform_state* deform = nullptr;        // created by the first r3_set_deformable_meshes
+    r3_deform_state* deform = nullptr;        // created by the first r3_set_deformable_meshes or r3_set_remeshable_meshes
     // frame graph
     bool capturing = false;                   // between r3_frame_begin and the submission (or an early flush)
     cudaGraphExec_t frame_exec[2] = {nullptr, nullptr};   // instantiated graphs of even / odd frames (the culling buffers ping-pong), updated in place
@@ -264,6 +267,7 @@ int r3_reserve_point_buffer(r3_ctx* c, uint32_t n_lights);   // r3_lights.cu: ro
 // every byte; r3_update_mesh_buffer: [offset, offset + nbytes), which matters when it meets one of the set's index ranges)
 void r3_deform_destroy(r3_ctx* c);
 void r3_deform_note_mesh_write(r3_ctx* c, bool whole_buffer, uint64_t byte_offset, uint64_t nbytes);
+int r3_deform_grow_floors(r3_ctx* c, uint32_t n);   // r3_resize_objects: zero invocation floors for the new slots, while they exist
 
 #ifdef __CUDACC__
 // Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine

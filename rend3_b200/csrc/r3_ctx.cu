@@ -653,6 +653,7 @@ R3_EXPORT int r3_resize_objects(r3_ctx* c, uint32_t n) {
     R3_CUDA(c, cudaMemsetAsync(c->d_objects + old_n, 0, (size_t)(n - old_n) * sizeof(r3_object), c->stream));
     R3_TRY(r3_grow_hot(c, old_n, n));
     R3_TRY(r3_grow_mesh_spheres(c, n));
+    R3_TRY(r3_deform_grow_floors(c, n));
     c->n_slots = n;   // zero records have no triangles: the cached invocation bounds stay valid
     const size_t sorted = c->sort_key.size();
     if (c->have_live && sorted < n) {

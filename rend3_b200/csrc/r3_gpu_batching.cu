@@ -26,13 +26,11 @@
 #include <cuda/atomic>
 
 #include "r3_common.cuh"
+#include "r3_radix.cuh"
 #include "r3_scan.cuh"
 
 namespace {
 
-constexpr int SORT_THREADS = 256;
-constexpr int SORT_KEYS_PER_THREAD = 8;
-constexpr int SORT_TILE = SORT_THREADS * SORT_KEYS_PER_THREAD;   // 2048 keys per block
 constexpr int KEY_SHIFT0 = 24, SORT_PASSES = 5;
 
 // order-preserving map of OrderedFloat's total order (batching.rs:37): every NaN is one value above +inf, -0.0 == +0.0
@@ -141,79 +139,9 @@ __global__ void keygen_kernel(const uint32_t* __restrict__ visible, const uint32
     keys[j] = make_sort_key(visible, key8, loc, vx, vy, vz, j);
 }
 
-// Digit histogram of the tile of SORT_TILE keys at `base`, stored digit-major into hist[digit * n_tiles + tile]: a flat
-// exclusive scan of that table gives every tile's scatter bases.  SORT_THREADS threads, one digit each.
-__device__ __forceinline__ void radix_tile_hist(const unsigned long long* keys, uint32_t nv, int shift, uint32_t* hist, uint32_t tile, uint32_t n_tiles) {
-    __shared__ uint32_t s_hist[256];
-    s_hist[threadIdx.x] = 0;
-    __syncthreads();
-    const uint32_t base = tile * SORT_TILE;
-#pragma unroll
-    for (int r = 0; r < SORT_KEYS_PER_THREAD; ++r) {
-        const uint32_t i = base + r * SORT_THREADS + threadIdx.x;
-        if (i < nv) atomicAdd(&s_hist[(uint32_t)(keys[i] >> shift) & 0xFFu], 1u);
-    }
-    __syncthreads();
-    hist[threadIdx.x * n_tiles + tile] = s_hist[threadIdx.x];
-}
-
-// Stable scatter of the tile at `base`, 256 keys per round: a key goes to s_gbase[digit] (the tile's first position of that
-// digit, in shared memory) + the keys of its digit in earlier rounds + those in lower warps of this round + its rank among the
-// warp's peers (__match_any_sync).  SORT_THREADS threads, one digit each.
-__device__ __forceinline__ void radix_tile_scatter(const unsigned long long* keys_in, unsigned long long* keys_out, uint32_t nv, int shift, uint32_t base,
-                                                   const uint32_t* s_gbase) {
-    __shared__ uint32_t s_cnt[SORT_THREADS / 32][256];   // per-warp digit counts of the current round
-    __shared__ uint32_t s_run[256];                       // digits already emitted by this tile in earlier rounds
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    s_run[threadIdx.x] = 0;
-#pragma unroll 1
-    for (int r = 0; r < SORT_KEYS_PER_THREAD; ++r) {
-#pragma unroll
-        for (int w = 0; w < SORT_THREADS / 32; ++w) s_cnt[w][threadIdx.x] = 0;
-        __syncthreads();
-        const uint32_t i = base + r * SORT_THREADS + threadIdx.x;
-        const bool valid = i < nv;
-        const unsigned long long key = valid ? keys_in[i] : 0ull;
-        const uint32_t d = valid ? ((uint32_t)(key >> shift) & 0xFFu) : 0x100u;     // invalid lanes form their own group
-        const uint32_t peers = __match_any_sync(0xFFFFFFFFu, d);
-        const uint32_t rank_in_warp = __popc(peers & ((1u << lane) - 1u));
-        if (valid && rank_in_warp == 0) s_cnt[warp][d] = __popc(peers);              // one writer per (warp, digit)
-        __syncthreads();
-        // digit t: exclusive prefix over the warps, then advance the tile's running count
-        uint32_t acc = 0;
-#pragma unroll
-        for (int w = 0; w < SORT_THREADS / 32; ++w) { const uint32_t c = s_cnt[w][threadIdx.x]; s_cnt[w][threadIdx.x] = acc; acc += c; }
-        __syncthreads();
-        if (valid) keys_out[s_gbase[d] + s_run[d] + s_cnt[warp][d] + rank_in_warp] = key;
-        __syncthreads();
-        s_run[threadIdx.x] += acc;
-        __syncthreads();
-    }
-}
-
 __global__ void __launch_bounds__(SORT_THREADS) radix_hist_kernel(const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ header,
                                                                   int shift, uint32_t* __restrict__ hist) {
     radix_tile_hist(keys, header[0], shift, hist, blockIdx.x, gridDim.x);
-}
-
-// in-place exclusive scan by one block: every thread owns a contiguous run (serial sum, one block scan of the 1024 run totals,
-// serial write-back) — three barriers in all instead of four per 1024 elements
-__global__ void __launch_bounds__(1024) scan_u32_kernel(uint32_t* __restrict__ data, uint32_t n) {
-    __shared__ uint32_t s_warp[1024 / 32 + 1];
-    const uint32_t per = (((n + 1023u) / 1024u) + 3u) & ~3u;          // multiple of 4: runs start 16-byte aligned
-    const uint32_t lo = min(threadIdx.x * per, n), hi = min(lo + per, n);
-    uint32_t sum = 0;
-    uint32_t i = lo;
-    for (; i + 4 <= hi; i += 4) { const uint4 v = *reinterpret_cast<const uint4*>(data + i); sum += v.x + v.y + v.z + v.w; }
-    for (; i < hi; ++i) sum += data[i];
-    uint32_t run = block_scan_excl<1024>(sum, s_warp);
-    for (i = lo; i + 4 <= hi; i += 4) {
-        const uint4 v = *reinterpret_cast<const uint4*>(data + i);
-        uint4 o;
-        o.x = run; o.y = o.x + v.x; o.z = o.y + v.y; o.w = o.z + v.z; run = o.w + v.w;
-        *reinterpret_cast<uint4*>(data + i) = o;
-    }
-    for (; i < hi; ++i) { const uint32_t v = data[i]; data[i] = run; run += v; }
 }
 
 __global__ void __launch_bounds__(SORT_THREADS) radix_scatter_kernel(const unsigned long long* __restrict__ keys_in, unsigned long long* __restrict__ keys_out,
@@ -531,11 +459,14 @@ __global__ void __launch_bounds__(1024) partition_scatter_kernel(const __grid_co
     }
 }
 
-// out[0] = sum over the slots of round_up(triangles, 256), out[1] = the largest such term
-__global__ void max_invocations_kernel(const r3_object* __restrict__ objects, uint32_t n, unsigned long long* __restrict__ out) {
+// out[0] = sum over the slots of round_up(triangles, 256), out[1] = the largest such term; a slot's index_count counts as at least its
+// floor (slots below n_floor)
+__global__ void max_invocations_kernel(const r3_object* __restrict__ objects, uint32_t n, const uint32_t* __restrict__ floor, uint32_t n_floor,
+                                       unsigned long long* __restrict__ out) {
     unsigned long long acc = 0, big = 0;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const unsigned long long v = ((objects[i].index_count / 3u) + 255u) & ~255u;
+        const uint32_t ic = i < n_floor ? max(objects[i].index_count, floor[i]) : objects[i].index_count;
+        const unsigned long long v = ((ic / 3u) + 255u) & ~255u;
         acc += v; big = max(big, v);
     }
     acc = warp_reduce(acc);
@@ -545,14 +476,14 @@ __global__ void max_invocations_kernel(const r3_object* __restrict__ objects, ui
 
 }  // namespace
 
-// sum over every slot of round_up(index_count / 3, 256): the bound the culling buffers are sized with when the per-frame
+// sum over every slot of round_up(max(index_count, floor) / 3, 256): the bound the culling buffers are sized with when the per-frame
 // totals stay on the device.  One small reduction + 8-byte readback at upload time, never per frame.
 int r3_compute_max_invocations(r3_ctx* c) {
     if (c->max_invocations_valid) return R3_OK;
     c->max_total_invocations = 0; c->max_object_invocations = 0;
     if (c->n_slots) {
         R3_CUDA(c, cudaMemsetAsync(c->d_stats + 4, 0, 16, c->stream));
-        max_invocations_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(c->d_objects, c->n_slots, c->d_stats + 4);
+        max_invocations_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(c->d_objects, c->n_slots, c->d_invocation_floor, c->n_invocation_floor, c->d_stats + 4);
         R3_CHECK_LAUNCH(c, "max_invocations_kernel");
         unsigned long long v[2] = {0, 0};
         R3_CUDA(c, cudaMemcpyAsync(v, c->d_stats + 4, 16, cudaMemcpyDeviceToHost, c->stream));
@@ -560,6 +491,14 @@ int r3_compute_max_invocations(r3_ctx* c) {
         c->max_total_invocations = v[0]; c->max_object_invocations = v[1];
     }
     c->max_invocations_valid = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_debug_invocation_bound(r3_ctx* c, uint64_t out[2]) {
+    if (!c || !out) return R3_E_INVALID;
+    cudaSetDevice(c->device);
+    R3_TRY(r3_compute_max_invocations(c));
+    out[0] = c->max_total_invocations; out[1] = c->max_object_invocations;
     return R3_OK;
 }
 

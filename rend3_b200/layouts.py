@@ -209,6 +209,12 @@ JOINT_WRITE_DTYPE = _dt([("joint_matrix_base_offset", u4, 0), ("joint_count", u4
 DEFORMABLE_MESH_DTYPE = _dt([("position_offset", u4, 0), ("normal_offset", u4, 4), ("tangent_offset", u4, 8), ("uv0_offset", u4, 12),
                              ("first_index", u4, 16), ("index_count", u4, 20), ("vertex_count", u4, 24), ("flags", u4, 28)], 32)
 DEFORM_LEFT_HANDED, DEFORM_NORMALS, DEFORM_TANGENTS = 0x1, 0x2, 0x4
+# r3_set_remeshable_meshes: one mesh's capacity-sized ranges and how MeshBuilder::build made it (DEFORM_* flags)
+REMESHABLE_MESH_DTYPE = _dt([("position_offset", u4, 0), ("normal_offset", u4, 4), ("tangent_offset", u4, 8), ("uv0_offset", u4, 12),
+                             ("color0_offset", u4, 16), ("first_index", u4, 20), ("index_capacity", u4, 24), ("vertex_capacity", u4, 28),
+                             ("flags", u4, 32)], 48)
+# r3_readback_remesh_status: Mesh::validate's reasons, the first that applies
+REMESH_APPLIED, REMESH_OVER_CAPACITY, REMESH_NOT_TRIANGLES, REMESH_INDEX_OUT_OF_RANGE = 0, 1, 2, 3
 # object animation (r3_set_object_animations / r3_set_object_pose_jobs); jobs are POSE_JOB_DTYPE records
 ANIM_NODE_DTYPE = _dt([("bind_translation", (f4, 3), 0), ("bind_rotation", (f4, 4), 16), ("bind_scale", (f4, 3), 32)], 48)
 ANIM_NODE_CHANNEL_DTYPE = _dt([("translation", ANIM_TRACK_DTYPE, 0), ("rotation", ANIM_TRACK_DTYPE, 16), ("scale", ANIM_TRACK_DTYPE, 32),

@@ -143,7 +143,7 @@ class BaseRenderGraph:
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
                      movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None,
-                     material_updates=None, joint_matrices=None, mesh_deforms=None):
+                     material_updates=None, joint_matrices=None, mesh_deforms=None, remeshes=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -184,7 +184,12 @@ class BaseRenderGraph:
         `object_transforms`, `posed_objects` and the skeletons, so that a move in the same frame wins the location (set_object_transform
         after add) and a deformed skinning base is skinned from the new positions.  A CUDA tensor goes through r3_deform_meshes_device —
         enqueue only, its producer ordered on the context's stream — and a host array through r3_deform_meshes, which waits for the
-        stream."""
+        stream.
+        `remeshes` = dict(counts=, positions=, indices=, and normals= / tangents= / uv0= / color0= where the set reads them) remeshes the set
+        made by r3_set_remeshable_meshes (the rebuild of each mesh from new vertices and indices and the re-add of its objects) in the
+        place of `mesh_deforms`; a context holds one of the two sets, so the two arguments are exclusive.  CUDA tensors go through
+        r3_remesh_meshes_device (enqueue only; a mesh that fails validation is left as it was, see readback_remesh_status) and host arrays
+        through r3_remesh_meshes, which waits for the stream."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -223,6 +228,12 @@ class BaseRenderGraph:
                 b.deform_meshes_device(mesh_deforms)
             else:
                 b.deform_meshes(mesh_deforms)
+        if remeshes is not None:                                                  # :145 meshes rebuilt from new vertices and indices
+            assert mesh_deforms is None, "remeshes and mesh_deforms: a context holds one dynamic-mesh set"
+            if getattr(remeshes["counts"], "is_cuda", False):
+                b.remesh_meshes_device(**remeshes)
+            else:
+                b.remesh_meshes(**remeshes)
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
         if material_updates is not None:                                          # :145 materials that change, before the shadow passes
