@@ -346,6 +346,29 @@ R3_STATIC_ASSERT(sizeof(r3_remeshable_mesh) == 48, "r3_remeshable_mesh");
 R3_STATIC_ASSERT(offsetof(r3_remeshable_mesh, color0_offset) == 16, "color0_offset");
 R3_STATIC_ASSERT(offsetof(r3_remeshable_mesh, first_index) == 20, "first_index");
 R3_STATIC_ASSERT(offsetof(r3_remeshable_mesh, flags) == 32, "flags");
+
+/* One prepared mesh + material of an object (r3_set_object_variants): what ObjectManager::add takes from the mesh kind and the material
+ * (object.rs:267-284).  A switch writes these fields into the slot's record, moves mesh_sphere by the slot's transform and, when sort
+ * info is set, takes material_key and sort_flags as the slot's key and flags bits 1-2. */
+typedef struct r3_object_variant {
+    uint32_t first_index;         /* @0  as r3_object (object.rs:279): word index of the mesh's indices */
+    uint32_t index_count;         /* @4 */
+    uint32_t material_index;      /* @8 */
+    uint32_t attr_offset[6];      /* @12 byte offsets, R3_ATTR_ABSENT if missing */
+    uint32_t sort_flags;          /* @36 bits 1-2 of r3_set_object_sort_info's flags (atomic, back to front); bit 0 (live) must be 0 */
+    uint64_t material_key;        /* @40 Material::key */
+    float mesh_sphere[4];         /* @48 InternalObject::mesh_bounding_sphere (centre, radius) */
+} r3_object_variant;
+R3_STATIC_ASSERT(sizeof(r3_object_variant) == 64, "r3_object_variant");
+R3_STATIC_ASSERT(offsetof(r3_object_variant, index_count) == 4, "index_count");
+R3_STATIC_ASSERT(offsetof(r3_object_variant, material_index) == 8, "material_index");
+R3_STATIC_ASSERT(offsetof(r3_object_variant, attr_offset) == 12, "attr_offset");
+R3_STATIC_ASSERT(offsetof(r3_object_variant, sort_flags) == 36, "sort_flags");
+R3_STATIC_ASSERT(offsetof(r3_object_variant, material_key) == 40, "material_key");
+R3_STATIC_ASSERT(offsetof(r3_object_variant, mesh_sphere) == 48, "mesh_sphere");
+/* a run of variants a slot chooses from, e.g. one LOD chain: variants first .. first + count - 1 */
+typedef struct r3_variant_group { uint32_t first, count; } r3_variant_group;
+R3_STATIC_ASSERT(sizeof(r3_variant_group) == 8, "r3_variant_group");
 /* per-mesh status of the last remesh (r3_readback_remesh_status): Mesh::validate's reasons (rend3-types/src/lib.rs:533-567), the first
  * that applies */
 #define R3_REMESH_APPLIED 0u

@@ -21,7 +21,7 @@
  *     `data_core` mutex of the reference, rend3/src/graph/graph.rs:265).  The per-frame entry points
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
- *     r3_update_materials_device, r3_set_joint_matrices_device, r3_deform_meshes_device, r3_remesh_meshes_device, r3_evaluate_shadow_cameras,
+ *     r3_switch_object_variants_device, r3_update_materials_device, r3_set_joint_matrices_device, r3_deform_meshes_device, r3_remesh_meshes_device, r3_evaluate_shadow_cameras,
  *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
@@ -30,7 +30,8 @@
  *     uploads that borrow a HOST pointer — r3_set_objects, r3_update_objects, r3_set_object_sort_info,
  *     r3_set_mesh_buffer, r3_set_materials, r3_update_materials, r3_set_textures, r3_set_skybox, r3_set_*_lights, r3_skin's joint upload,
  *     r3_set_animations, r3_set_skeletons, r3_set_pose_jobs, r3_set_joint_matrices, r3_readback_joint_matrices, r3_set_object_animations,
- *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_deformable_meshes,
+ *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_object_variants,
+ *     r3_switch_object_variants, r3_set_deformable_meshes,
  *     r3_deform_meshes, r3_set_remeshable_meshes, r3_remesh_meshes, r3_readback_remesh_status, r3_set_directional_light_sources,
  *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
@@ -176,6 +177,52 @@ int r3_set_object_transforms_device(r3_ctx*, const uint32_t* d_slots_or_null, co
  * draws nothing); the batch records of that one frame differ. */
 int r3_set_objects_enabled(r3_ctx*, const uint32_t* slots_or_null, const uint8_t* enabled, uint32_t n);
 int r3_set_objects_enabled_device(r3_ctx*, const uint32_t* d_slots_or_null, const uint8_t* d_enabled, uint32_t n);
+/* Objects that change mesh or material: re-adding an object with another mesh kind or material (ObjectManager::add, object.rs:122-160,
+ * 267-284; duplicate_object with an ObjectChange, object.rs:201-218, 318) for n slots in one kernel, from host or device memory — LOD
+ * chains, damage states, team or selection material swaps, impostors.  The host prepares a table of variants once (r3_object_variant:
+ * mesh range, attribute offsets, material, key, flags bits 1-2, mesh sphere) and groups of consecutive variants (r3_variant_group, e.g.
+ * one LOD chain); each listed slot chooses from one group, and many slots may share a group.  A switch of slot s to variant v writes what
+ * re-adding the object with v's mesh and material at its current transform writes: the record's first_index, index_count,
+ * material_index and attr_offset[6]; the world sphere (BoundingSphere::apply_transform of v's mesh sphere by the slot's transform, rule
+ * R12) into the record and the cull + bake's copies and centre bit; the slot's mesh sphere; and, when sort info is set, key and flags bits
+ * 1-2 and the sort location = the world sphere's centre (add's location).  `enabled`, the live bit, the transform, its rows and the affine
+ * bit stay: a switched absent slot stays absent.
+ *   r3_set_object_variants           blocking, once per set: n_variants variants, n_groups groups and n_listed (slot, group) pairs.  Records
+ *                                    are not changed.  Checks everything before it writes anything; R3_E_INVALID, the context unchanged,
+ *                                    for: a null pointer with a non-zero count; a variant whose index range lies outside the mesh buffer,
+ *                                    whose index_count % 3 != 0, with an offset that is neither a multiple of 4 nor R3_ATTR_ABSENT, without
+ *                                    a position, or with a flag bit other than 1-2; an empty group or one reaching past the variants; a slot
+ *                                    at or past the slot count or named twice; a group index >= n_groups; a slot also listed by the current
+ *                                    deformable or remeshable set (r3_set_deformable_meshes / r3_set_remeshable_meshes reject the reverse).
+ *                                    R3_E_STATE before r3_set_objects, while the object buffer is borrowed and while
+ *                                    r3_set_object_mesh_spheres does not cover every slot.  Each listed slot's invocation floor becomes the
+ *                                    largest index_count of its group, so a switch to the largest level never outgrows the culling buffers
+ *                                    (r3_debug_invocation_bound).  n_variants == 0 removes the set and its floors.  r3_resize_objects grows
+ *                                    the per-slot arrays (new slots unlisted).
+ *   r3_switch_object_variants        host pointers, blocking: one copy, one kernel, one drain.  Entry i gives slot slots[i] variant
+ *                                    group.first + choices[i] of its group; slots == NULL is the dense form over slots 0 .. n-1.
+ *                                    R3_E_INVALID, nothing written, for an unlisted slot, a slot named twice or choices[i] >= group.count.
+ *                                    The host's mirrors of keys and flags stay exact (the blend routine and the host batching follow them).
+ *   r3_switch_object_variants_device the same from DEVICE memory, enqueue only; legal between r3_frame_begin and r3_frame_end.  Producer
+ *                                    ordering as for r3_set_object_transforms_device.  Unlisted slots and out-of-range choices are dropped;
+ *                                    distinct slots are a precondition.  Until the next r3_set_object_sort_info or host switch the host
+ *                                    cannot know the switched keys: the blend routine runs whenever some slot or some variant of the set
+ *                                    has material key 2, and the device batching is only used while no variant key is >= 64.  The host
+ *                                    batching reads the slots' current variants back in the drain it makes anyway and stays exact.
+ *   r3_readback_object_variants      blocking: the current variant (an index into the table) of slots [first, first + n); 0xFFFFFFFF for a
+ *                                    slot that is unlisted or was not switched since the set was made.
+ * R3_E_STATE from both switch calls: before a set exists; after an r3_set_mesh_buffer that left the mesh buffer shorter than the set's
+ * largest index end; before r3_set_objects; while the object buffer is borrowed; while r3_set_object_mesh_spheres does not cover every
+ * slot.  n == 0 is R3_OK.  Each call starts a new frame epoch.  Ordering: r3_update_objects, r3_set_objects and
+ * r3_update_object_sort_info of a listed slot overwrite a switch, and the reverse (the floor still bounds the slot's index_count);
+ * r3_set_object_transforms* after a switch in the same frame gives the move's location with the new mesh sphere, a switch after a move
+ * gives the add's location; r3_pose_objects carries its own mesh spheres, so on a slot both posed and switched the later call wins for
+ * the sphere. */
+int r3_set_object_variants(r3_ctx*, const r3_object_variant* variants, uint32_t n_variants, const r3_variant_group* groups, uint32_t n_groups,
+                           const uint32_t* slots, const uint32_t* slot_groups, uint32_t n_listed);
+int r3_switch_object_variants(r3_ctx*, const uint32_t* slots_or_null, const uint32_t* choices, uint32_t n);
+int r3_switch_object_variants_device(r3_ctx*, const uint32_t* d_slots_or_null, const uint32_t* d_choices, uint32_t n);
+int r3_readback_object_variants(r3_ctx*, uint32_t* out, uint32_t first, uint32_t n);
 int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);               /* eval_output.mesh_buffer (mesh.rs:99) */
 /* Meshes that deform every frame (cloth, flags, a water grid, soft bodies, blend shapes evaluated by a CUDA kernel), from host or device
  * memory.  rend3's meshes are immutable: the reference rebuilds such a mesh each frame (MeshBuilder::build recomputes smooth normals and
@@ -196,7 +243,8 @@ int r3_set_mesh_buffer(r3_ctx*, const void* bytes, uint64_t nbytes);            
  *                                       the set; written ranges (positions, and normals / tangents when recomputed) that overlap each other
  *                                       or a read range of the set (indices, uv0 and authored normals when tangents are recomputed); an
  *                                       object mesh >= n_meshes; a slot named twice or at or past the slot count; a slot whose record does
- *                                       not draw its mesh (first_index, index_count and attr_offset[POSITION] differ).  R3_E_STATE before
+ *                                       not draw its mesh (first_index, index_count and attr_offset[POSITION] differ); a slot listed by
+ *                                       the object-variant set (r3_set_object_variants).  R3_E_STATE before
  *                                       r3_set_objects and while the object buffer is borrowed.  n_meshes == 0 removes the set.  A context
  *                                       holds one dynamic-mesh set: this call replaces a set of r3_set_remeshable_meshes, and the reverse.
  *   r3_deform_meshes                    host positions: sum(vertex_count) x 3 floats, mesh after mesh in set order (n_floats must be that
@@ -231,7 +279,8 @@ int r3_readback_deformable_mesh_spheres(r3_ctx*, float* out /* n x 4 */, uint32_
  *                                ranges (every present attribute, and the indices) that overlap; more than 2^31 - 1 vertices or 2^32 - 2^11
  *                                indices of capacity in the set; an object mesh >= n_meshes; a slot named twice or at or past the slot
  *                                count; a listed record that does not draw its mesh (first_index, the position, normal, tangent, uv0 and
- *                                color0 offsets differ, or index_count > index_capacity).  R3_E_STATE before r3_set_objects and while the
+ *                                color0 offsets differ, or index_count > index_capacity); a slot listed by the object-variant set.
+ *                                R3_E_STATE before r3_set_objects and while the
  *                                object buffer is borrowed.  n_meshes == 0 removes the set.  The set replaces a set of
  *                                r3_set_deformable_meshes, and the reverse; the calls of the set that is not current return R3_E_STATE.
  *                                The listed slots' index_capacity is kept as a floor of the invocation bound that sizes the culling
@@ -267,7 +316,7 @@ int r3_remesh_meshes_device(r3_ctx*, const uint32_t* d_counts, const float* d_po
 int r3_readback_remesh_status(r3_ctx*, uint32_t* status, uint32_t* counts_or_null /* n x 2 */, uint32_t first, uint32_t n);
 /* Test hook: the invocation bound the culling buffers are sized with, computed now if stale: out[0] = sum over the slots of
  * round_up(max(index_count, floor) / 3, 256), out[1] = the largest term; the floor is a listed slot's index_capacity while a remeshable
- * set exists, else 0. */
+ * set exists, the largest index_count of a listed slot's group while an object-variant set exists, else 0. */
 int r3_debug_invocation_bound(r3_ctx*, uint64_t out[2]);
 /* MeshManager::add (mesh.rs:123-184): write nbytes at byte_offset of the megabuffer (both multiples of 4).  A write past the end extends it;
  * words between the old end and byte_offset read 0.  The allocation grows to the next power of two, keeping its contents (also what

@@ -86,6 +86,11 @@ struct EvalOutput {
     // objects that appear or disappear this frame (ObjectManager::add into a prepared slot / remove): presence bytes (and slots, null =
     // slots 0 .. n-1) in DEVICE memory, their producer ordered on the context's stream; applied at the skinning node before the moves
     const uint32_t* d_presence_slots = nullptr; const uint8_t* d_presence = nullptr; uint32_t n_presence = 0;
+    // objects that change mesh or material this frame (ObjectManager::add with another mesh kind or material, within the set of
+    // r3_set_object_variants made before the frame): choices (and slots, null = slots 0 .. n-1) in HOST memory (blocking) or in DEVICE
+    // memory (enqueue only, producer ordered on the context's stream); applied at the skinning node before the presence and the moves
+    const uint32_t* variant_slots = nullptr; const uint32_t* variant_choices = nullptr; uint32_t n_variant_switches = 0;
+    const uint32_t* d_variant_slots = nullptr; const uint32_t* d_variant_choices = nullptr; uint32_t n_d_variant_switches = 0;
     // materials that change this frame (MaterialManager::update + evaluate's scatter of the stale records): records (and indices, null =
     // materials 0 .. n-1) in HOST memory (blocking, an index past the table grows it) or in DEVICE memory (enqueue only, records 16-byte
     // aligned, producer ordered on the context's stream); applied at the skinning node, before the shadow passes read the materials
@@ -184,6 +189,8 @@ public:
         if (const EvalOutput::RemeshStreams& s = ev.d_remesh; s.counts)
             r.check(r3_remesh_meshes_device(r.raw(), s.counts, s.positions, s.indices, s.normals, s.tangents, s.uv0, s.color0, s.n_vertices, s.n_indices));
         if (ev.n_skeletons) r.check(r3_skin(r.raw(), ev.skinning_inputs, ev.n_skeletons, ev.joint_matrices, ev.n_joints));
+        if (ev.n_variant_switches) r.check(r3_switch_object_variants(r.raw(), ev.variant_slots, ev.variant_choices, ev.n_variant_switches));
+        if (ev.n_d_variant_switches) r.check(r3_switch_object_variants_device(r.raw(), ev.d_variant_slots, ev.d_variant_choices, ev.n_d_variant_switches));
         if (ev.n_presence) r.check(r3_set_objects_enabled_device(r.raw(), ev.d_presence_slots, ev.d_presence, ev.n_presence));
         if (ev.n_moved) r.check(r3_set_object_transforms_device(r.raw(), ev.d_moved_slots, ev.d_moved_transforms, ev.n_moved));
         if (ev.posed_objects) r.check(r3_pose_objects(r.raw()));

@@ -49,6 +49,7 @@ ENTRY_POINTS = [
     "set_joint_matrices", "set_joint_matrices_device",
     "set_deformable_meshes", "deform_meshes", "deform_meshes_device", "readback_deformable_mesh_spheres",
     "set_remeshable_meshes", "remesh_meshes", "remesh_meshes_device", "readback_remesh_status", "debug_invocation_bound",
+    "set_object_variants", "switch_object_variants", "switch_object_variants_device", "readback_object_variants",
 ]
 
 
@@ -73,6 +74,14 @@ class R3Error(RuntimeError):
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _u32_list(a, what: str) -> np.ndarray:
+    """A 1-d integer array inside the uint32 range, as contiguous uint32."""
+    a = np.asarray(a)
+    assert a.ndim == 1 and a.dtype.kind in "iu", f"{what}: a 1-d integer array"
+    assert not len(a) or (a.min() >= 0 and a.max() <= 0xFFFFFFFF), f"{what}: out of the uint32 range"
+    return np.ascontiguousarray(a, dtype=np.uint32)
 
 
 class Backend:
@@ -518,6 +527,50 @@ class Backend:
         """(n, 4) mesh spheres (centre, radius) of the set's meshes [first, first + n) from the last deform"""
         out = np.zeros((max(n, 1), 4), dtype=np.float32)
         self._call("readback_deformable_mesh_spheres", _ptr(out), C.c_uint32(first), C.c_uint32(n))
+        return out[:n]
+
+    # ---- objects that change mesh or material (ObjectManager::add with another mesh kind or material)
+    def set_object_variants(self, variants, groups, slots=None, slot_groups=None):
+        """OBJECT_VARIANT_DTYPE records, VARIANT_GROUP_DTYPE groups (runs of variants) and the (slot, group) pairs of the listed slots.
+        Blocking; an empty `variants` removes the set."""
+        from .layouts import OBJECT_VARIANT_DTYPE, VARIANT_GROUP_DTYPE
+
+        v, g = np.asarray(variants), np.asarray(groups)
+        assert v.ndim == 1 and v.dtype == OBJECT_VARIANT_DTYPE, "variants: a 1-d OBJECT_VARIANT_DTYPE array"
+        assert g.ndim == 1 and g.dtype == VARIANT_GROUP_DTYPE, "groups: a 1-d VARIANT_GROUP_DTYPE array"
+        s = _u32_list(np.zeros(0, np.uint32) if slots is None else slots, "slots")
+        sg = _u32_list(np.zeros(0, np.uint32) if slot_groups is None else slot_groups, "slot_groups")
+        assert len(s) == len(sg), "slots and slot_groups: one group per slot"
+        v, g = np.ascontiguousarray(v), np.ascontiguousarray(g)
+        self._call("set_object_variants", _ptr(v) if len(v) else None, C.c_uint32(len(v)), _ptr(g) if len(g) else None, C.c_uint32(len(g)),
+                   _ptr(s) if len(s) else None, _ptr(sg) if len(sg) else None, C.c_uint32(len(s)))
+
+    def switch_object_variants(self, choices, slots=None):
+        """Slots 0 .. n-1, or the listed slots, to variant group.first + choices[i] of their group, from host memory.  Blocking."""
+        c = _u32_list(choices, "choices")
+        s = None if slots is None else _u32_list(slots, "slots")
+        assert s is None or len(s) == len(c), "slots: as long as choices"
+        self._call("switch_object_variants", _ptr(s) if s is not None and len(s) else None, _ptr(c) if len(c) else None, C.c_uint32(len(c)))
+
+    def switch_object_variants_device(self, choices, slots=None, n: Optional[int] = None):
+        """The same from device memory, enqueue only.  `choices` and `slots` (None: slots 0 .. n-1) are contiguous 1-d CUDA tensors of
+        4-byte integers, or raw device pointers with `n` given; the caller keeps them alive and orders their producer on stream()."""
+        def pointer(x, what):
+            if x is None or isinstance(x, int):
+                return x, None
+            assert getattr(x, "is_cuda", False) and x.is_contiguous() and x.dim() == 1 and x.element_size() == 4 \
+                and not x.is_floating_point(), f"{what}: a contiguous 1-d CUDA tensor of 4-byte integers"
+            return x.data_ptr(), x.numel()
+        cp, cn = pointer(choices, "choices")
+        sp, sn = pointer(slots, "slots")
+        n = cn if n is None else n
+        assert n is not None and (sn is None or sn == n) and (cn is None or cn == n), "choices and slots differ in length"
+        self._call("switch_object_variants_device", C.c_void_p(sp), C.c_void_p(cp), C.c_uint32(n))
+
+    def readback_object_variants(self, first: int, n: int) -> np.ndarray:
+        """The current variant of slots [first, first + n): an index into the table, VARIANT_NONE when unlisted or never switched"""
+        out = np.zeros(max(n, 1), dtype=np.uint32)
+        self._call("readback_object_variants", _ptr(out), C.c_uint32(first), C.c_uint32(n))
         return out[:n]
 
     # ---- meshes whose topology changes every frame (rebuild of the mesh from new vertices and indices + re-add of its objects, on the device)

@@ -92,6 +92,7 @@ struct r3_camera {
 
 struct r3_anim_state;                        // skeletal animation + resident skinning data (r3_animation.cu)
 struct r3_deform_state;                      // the dynamic-mesh set: deformable or remeshable (r3_mesh_deform.cu)
+struct r3_variant_state;                     // the object-variant set (r3_object_transforms.cu)
 
 struct r3_tri_record { float xyw[3][3]; uint32_t object_id; uint32_t vid[3]; uint32_t _pad[3]; };   // 64 B
 static_assert(sizeof(r3_tri_record) == 64, "triangle record");
@@ -121,6 +122,9 @@ struct r3_ctx {
     uint32_t sort_live_blend = 0, sort_wide_keys = 0;   // live slots with material key 2 (any_blend), slots with a key >= 64 (host batching)
     uint32_t sort_blend_slots = 0;            // slots with material key 2, live or not (any_blend while presence_on_device)
     bool presence_on_device = false;          // r3_set_objects_enabled_device ran since r3_set_object_sort_info: the host's live bits are stale
+    // r3_switch_object_variants_device ran since the host last read the slots' current variants: its key and flag mirrors are stale.
+    // variant_key2 / variant_wide_key: some variant of the set has material key 2 / a key >= 64
+    bool variants_on_device = false, variant_key2 = false, variant_wide_key = false;
     // frame-wide sort shared by the cameras of one frame (r3_gpu_batching.cu)
     unsigned long long* d_gsort_keys[2] = {nullptr, nullptr}; uint64_t gsort_cap[2] = {0, 0}; uint32_t* d_gsort_hist = nullptr; uint64_t gsort_hist_cap = 0;
     uint32_t* d_gsort_header = nullptr; int gsort_src = 0; uint32_t gsort_n = 0; bool gsort_valid = false; float gsort_loc[3] = {0, 0, 0};
@@ -173,6 +177,7 @@ struct r3_ctx {
     uint32_t tri_shard_index = 0, tri_shard_count = 1;   // r3_set_cull_shard
     r3_anim_state* anim = nullptr;            // created by the first r3_set_animations / r3_set_skeletons
     r3_deform_state* deform = nullptr;        // created by the first r3_set_deformable_meshes or r3_set_remeshable_meshes
+    r3_variant_state* variants = nullptr;     // created by the first r3_set_object_variants
     // frame graph
     bool capturing = false;                   // between r3_frame_begin and the submission (or an early flush)
     cudaGraphExec_t frame_exec[2] = {nullptr, nullptr};   // instantiated graphs of even / odd frames (the culling buffers ping-pong), updated in place
@@ -268,6 +273,25 @@ int r3_reserve_point_buffer(r3_ctx* c, uint32_t n_lights);   // r3_lights.cu: ro
 void r3_deform_destroy(r3_ctx* c);
 void r3_deform_note_mesh_write(r3_ctx* c, bool whole_buffer, uint64_t byte_offset, uint64_t nbytes);
 int r3_deform_grow_floors(r3_ctx* c, uint32_t n);   // r3_resize_objects: zero invocation floors for the new slots, while they exist
+// r3_mesh_deform.cu: c->d_invocation_floor from both of its sources, a remeshable set's index capacities and the object-variant set's
+// group maxima (their slots are disjoint); freed when neither set exists.  Invalidates the cached invocation bound.
+int r3_rebuild_invocation_floors(r3_ctx* c);
+const std::vector<uint32_t>* r3_deform_listed_slots(r3_ctx* c);   // the current deformable / remeshable set's slots, nullptr without one
+// r3_object_transforms.cu: the object-variant set (r3_set_object_variants)
+void r3_variants_destroy(r3_ctx* c);
+int r3_variants_grow(r3_ctx* c, uint32_t n);          // r3_resize_objects: the per-slot arrays grow, new slots unlisted
+bool r3_variants_have_set(const r3_ctx* c);
+bool r3_variants_list(const r3_ctx* c, uint32_t slot);   // the set lists the slot
+int r3_variants_scatter_floors(r3_ctx* c);            // the listed slots' floors into c->d_invocation_floor (zeroed by the caller)
+// After r3_switch_object_variants_device the host's key / flag mirrors are behind the device's.  stage enqueues a copy of the listed slots'
+// current-variant words to the host and marks them seen on the device (*staged = true when it did); once the caller has drained the
+// stream, apply rebuilds the mirrors of the slots switched since.  sync is stage + drain + apply.
+int r3_variants_stage(r3_ctx* c, bool* staged);
+void r3_variants_apply(r3_ctx* c);
+int r3_variants_sync_host(r3_ctx* c);
+// r3_ctx.cu: slot s's material key and flags bits 1-2 into the host mirrors, with the counts any_blend and gpu_batching_ok follow (the
+// caller re-derives them with r3_presence_derive)
+void r3_sort_set_key_flags(r3_ctx* c, uint32_t s, uint64_t key, uint8_t flags12);
 
 #ifdef __CUDACC__
 // Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine

@@ -81,6 +81,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     r3_peer_destroy(c);
     r3_anim_destroy(c);
     r3_deform_destroy(c);
+    r3_variants_destroy(c);
     if (!c->objects_borrowed) cudaFree(c->d_objects);
     cudaFree(c->d_hot_xyz); cudaFree(c->d_hot_w); cudaFree(c->d_hot_sphere); cudaFree(c->d_enabled_bits); cudaFree(c->d_affine_bits); cudaFree(c->d_hot_radius); cudaFree(c->d_centre_bits); cudaFree(c->d_tex_descs); cudaFree(c->d_texels); cudaFree(c->d_sky_texels);
     cudaFree(c->d_sort_key8); cudaFree(c->d_sort_loc); cudaFree(c->d_gsort_keys[0]); cudaFree(c->d_gsort_keys[1]); cudaFree(c->d_gsort_hist); cudaFree(c->d_gsort_header);
@@ -306,14 +307,26 @@ static inline uint32_t sort_wide_key(uint64_t key) { return key >= 64 ? 1u : 0u;
 static inline uint32_t sort_blend_slot(uint64_t key) { return key == 2 ? 1u : 0u; }                                  // live or not
 static void sort_derive(r3_ctx* c) {
     // after r3_set_objects_enabled_device only the device knows which slots are live: then any slot with key 2 runs the blend routine
-    // (over no fragments when none of them is present, which leaves the image as it is)
-    c->any_blend = (c->presence_on_device ? c->sort_blend_slots : c->sort_live_blend) != 0;
-    c->gpu_batching_ok = c->sort_wide_keys == 0 && c->sort_key.size() < (1u << 24) && !getenv("R3_HOST_BATCHING");
+    // (over no fragments when none of them is present, which leaves the image as it is).  After r3_switch_object_variants_device only
+    // the device knows the switched slots' keys: then any slot or variant with key 2 runs it, and a variant key >= 64 (which the device
+    // batching's 6-bit keys cannot hold) keeps the batching on the host, which reads the current variants back.
+    const bool conservative = c->presence_on_device || c->variants_on_device;
+    c->any_blend = (conservative ? c->sort_blend_slots : c->sort_live_blend) != 0 || (c->variants_on_device && c->variant_key2);
+    c->gpu_batching_ok = c->sort_wide_keys == 0 && c->sort_key.size() < (1u << 24) && !getenv("R3_HOST_BATCHING") &&
+                         !(c->variants_on_device && c->variant_wide_key);
+}
+void r3_sort_set_key_flags(r3_ctx* c, uint32_t s, uint64_t key, uint8_t flags12) {
+    const uint8_t was = c->sort_flags[s], now = (uint8_t)((was & 1u) | (flags12 & 6u));
+    c->sort_wide_keys += sort_wide_key(key) - sort_wide_key(c->sort_key[s]);
+    c->sort_blend_slots += sort_blend_slot(key) - sort_blend_slot(c->sort_key[s]);
+    c->sort_live_blend += sort_live_blend(key, now) - sort_live_blend(c->sort_key[s], was);
+    c->sort_key[s] = key; c->sort_flags[s] = now;
 }
 
 R3_EXPORT int r3_set_object_sort_info(r3_ctx* c, const uint64_t* key, const uint8_t* flags, const float* loc, uint32_t n) {
     if (!c || !key || !flags || !loc) return r3_fail(c, R3_E_INVALID, "set_object_sort_info: null");
     cudaSetDevice(c->device);
+    R3_TRY(r3_variants_sync_host(c));   // device switches the host has not seen are settled before the mirrors are replaced
     c->sort_key.assign(key, key + n);
     c->sort_flags.assign(flags, flags + n);
     c->sort_loc.assign(loc, loc + 3 * (size_t)n);
@@ -584,6 +597,7 @@ R3_EXPORT int r3_update_object_sort_info(r3_ctx* c, const uint32_t* slots, const
     for (uint32_t i = 0; i < n; ++i)
         if (slots[i] >= count) return r3_fail(c, R3_E_INVALID, "update_object_sort_info: slot beyond the sort info");
     cudaSetDevice(c->device);
+    R3_TRY(r3_variants_sync_host(c));   // a device switch before this call must not be replayed over its entries later
     // the host mirrors (read by the host batching) take the entries in order: of a slot listed twice, the later entry wins
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t s = slots[i];
@@ -654,6 +668,7 @@ R3_EXPORT int r3_resize_objects(r3_ctx* c, uint32_t n) {
     R3_TRY(r3_grow_hot(c, old_n, n));
     R3_TRY(r3_grow_mesh_spheres(c, n));
     R3_TRY(r3_deform_grow_floors(c, n));
+    R3_TRY(r3_variants_grow(c, n));
     c->n_slots = n;   // zero records have no triangles: the cached invocation bounds stay valid
     const size_t sorted = c->sort_key.size();
     if (c->have_live && sorted < n) {

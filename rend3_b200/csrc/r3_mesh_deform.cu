@@ -368,13 +368,6 @@ remesh_copy_kernel(const deform_mesh_dev* __restrict__ meshes, const uint32_t* _
     if (md.color0_offset != R3_ATTR_ABSENT) mesh[md.color0_offset / 4 + (uint64_t)v] = __ldg(color0 + g);
 }
 
-// the invocation floor of every listed slot: its mesh's index_capacity
-__global__ void floor_scatter_kernel(const deform_mesh_dev* __restrict__ meshes, const uint32_t* __restrict__ slots, const uint32_t* __restrict__ object_mesh,
-                                     uint32_t n, uint32_t* __restrict__ floor) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) floor[slots[i]] = meshes[object_mesh[i]].index_capacity;
-}
-
 }  // namespace
 
 struct r3_deform_state {
@@ -397,6 +390,7 @@ struct r3_deform_state {
     unsigned long long* d_keys[2] = {nullptr, nullptr}; uint64_t keys_cap[2] = {0, 0};
     uint32_t* d_hist = nullptr; uint64_t hist_cap = 0;
     uint32_t* d_status = nullptr; uint32_t status_cap = 0;
+    std::vector<uint32_t> listed;             // host copy of the listed slots (r3_set_object_variants must not list them)
 };
 
 namespace {
@@ -405,7 +399,7 @@ namespace {
 constexpr uint64_t MAX_SET_INDICES = (1ull << 32) - SORT_TILE;
 constexpr uint32_t READS_NORMALS = 1, READS_TANGENTS = 2, READS_UV0 = 4, READS_COLOR0 = 8;
 
-// the invocation floors exist only while a remesh set does; dropping them changes the bound
+// the invocation floors exist only while a remesh set or an object-variant set does; dropping them changes the bound
 void drop_floors(r3_ctx* c) {
     if (!c->d_invocation_floor) return;
     cudaFree(c->d_invocation_floor);
@@ -413,14 +407,41 @@ void drop_floors(r3_ctx* c) {
     c->max_invocations_valid = false;
 }
 
-void remove_set(r3_ctx* c) {
-    drop_floors(c);
+int remove_set(r3_ctx* c) {
     r3_deform_state* d = c->deform;
-    if (!d) return;
-    d->valid = false; d->remesh = false; d->n_meshes = 0;
-    d->meshes.clear(); d->remeshes.clear();
+    if (d) {
+        d->valid = false; d->remesh = false; d->n_meshes = 0;
+        d->meshes.clear(); d->remeshes.clear(); d->listed.clear();
+    }
+    return r3_rebuild_invocation_floors(c);   // the object-variant set's floors stay
+}
+
+// the invocation floor of every listed slot of a remesh set: its mesh's index_capacity
+__global__ void floor_scatter_kernel(const deform_mesh_dev* __restrict__ meshes, const uint32_t* __restrict__ slots, const uint32_t* __restrict__ object_mesh,
+                                     uint32_t n, uint32_t* __restrict__ floor) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) floor[slots[i]] = meshes[object_mesh[i]].index_capacity;
 }
 }  // namespace
+
+int r3_rebuild_invocation_floors(r3_ctx* c) {
+    const r3_deform_state* d = c->deform;
+    const bool remesh = d && d->remesh && d->n_meshes;
+    c->max_invocations_valid = false;
+    if (!remesh && !r3_variants_have_set(c)) { drop_floors(c); return R3_OK; }
+    const uint32_t n = std::max(c->n_slots, 1u);
+    R3_TRY(r3_reserve_t(c, &c->d_invocation_floor, &c->invocation_floor_cap, n));
+    R3_CUDA(c, cudaMemsetAsync(c->d_invocation_floor, 0, (size_t)n * 4, c->stream));
+    c->n_invocation_floor = c->n_slots;
+    if (remesh && d->n_objects) {
+        floor_scatter_kernel<<<(d->n_objects + DF_THREADS - 1) / DF_THREADS, DF_THREADS, 0, c->stream>>>(d->d_meshes, d->d_slots, d->d_object_mesh,
+                                                                                                       d->n_objects, c->d_invocation_floor);
+        R3_CHECK_LAUNCH(c, "floor_scatter_kernel");
+    }
+    return r3_variants_scatter_floors(c);
+}
+
+const std::vector<uint32_t>* r3_deform_listed_slots(r3_ctx* c) { return c->deform && c->deform->n_meshes ? &c->deform->listed : nullptr; }
 
 void r3_deform_destroy(r3_ctx* c) {
     drop_floors(c);
@@ -485,6 +506,7 @@ int check_objects(r3_ctx* c, const char* who, const uint32_t* object_slots, cons
         if (object_meshes[i] >= n_meshes) return fail_s(c, R3_E_INVALID, std::string(who) + ": object mesh out of range");
         if (s >= c->n_slots) return fail_s(c, R3_E_INVALID, std::string(who) + ": slot beyond the object buffer");
         if (seen[s >> 6] & (1ull << (s & 63u))) return fail_s(c, R3_E_INVALID, std::string(who) + ": one slot named twice");
+        if (r3_variants_list(c, s)) return fail_s(c, R3_E_INVALID, std::string(who) + ": a slot listed by the object-variant set");
         seen[s >> 6] |= 1ull << (s & 63u);
         *lo = std::min(*lo, s); *hi = std::max(*hi, s);
     }
@@ -656,8 +678,7 @@ R3_EXPORT int r3_set_deformable_meshes(r3_ctx* c, const r3_deformable_mesh* mesh
     if ((!meshes && n_meshes) || ((!object_slots || !object_meshes) && n_objects)) return r3_fail(c, R3_E_INVALID, "set_deformable_meshes: null");
     if (n_meshes == 0) {
         if (n_objects) return r3_fail(c, R3_E_INVALID, "set_deformable_meshes: objects without meshes");
-        remove_set(c);
-        return R3_OK;
+        return remove_set(c);
     }
     if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, "set_deformable_meshes before set_objects");
     if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_deformable_meshes: the object buffer is borrowed (r3_set_objects_device)");
@@ -735,11 +756,12 @@ R3_EXPORT int r3_set_deformable_meshes(r3_ctx* c, const r3_deformable_mesh* mesh
         block_mesh.insert(block_mesh.end(), nb, i);
         vb += m.vertex_count; ib += m.index_count; blocks += nb;
     }
-    remove_set(c);
+    R3_TRY(remove_set(c));
     R3_TRY(reserve_set(c, n_meshes, blocks, n_vertices, n_indices, n_objects));
     R3_TRY(upload_set(c, dev, block_mesh, index_base, object_slots, object_meshes, n_objects));
     commit_set(c, false, n_meshes, n_objects, blocks, n_vertices, n_indices, n_objects ? slot_hi : 0);
     c->deform->meshes.assign(meshes, meshes + n_meshes);
+    c->deform->listed.assign(object_slots, object_slots + n_objects);
     R3_TRY(build_corner_lists(c, nullptr));
     R3_CUDA(c, r3_stream_sync(c));   // host pointers are only borrowed for the call
     free_sort_scratch(c->deform);    // a deformable set sorts only here; a remesh set sorts in every call
@@ -785,8 +807,7 @@ R3_EXPORT int r3_set_remeshable_meshes(r3_ctx* c, const r3_remeshable_mesh* mesh
     if ((!meshes && n_meshes) || ((!object_slots || !object_meshes) && n_objects)) return r3_fail(c, R3_E_INVALID, "set_remeshable_meshes: null");
     if (n_meshes == 0) {
         if (n_objects) return r3_fail(c, R3_E_INVALID, "set_remeshable_meshes: objects without meshes");
-        remove_set(c);
-        return R3_OK;
+        return remove_set(c);
     }
     if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, "set_remeshable_meshes before set_objects");
     if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_remeshable_meshes: the object buffer is borrowed (r3_set_objects_device)");
@@ -853,20 +874,13 @@ R3_EXPORT int r3_set_remeshable_meshes(r3_ctx* c, const r3_remeshable_mesh* mesh
         block_mesh.insert(block_mesh.end(), nb, i);
         vb += m.vertex_capacity; ib += m.index_capacity; blocks += nb;
     }
-    remove_set(c);
+    R3_TRY(remove_set(c));
     R3_TRY(reserve_set(c, n_meshes, blocks, n_vertices, n_indices, n_objects));
     R3_TRY(upload_set(c, dev, block_mesh, index_base, object_slots, object_meshes, n_objects));
-    // the invocation floors: the listed slots' index_capacity, zero elsewhere
-    R3_TRY(r3_reserve_t(c, &c->d_invocation_floor, &c->invocation_floor_cap, std::max(c->n_slots, 1u)));
-    R3_CUDA(c, cudaMemsetAsync(c->d_invocation_floor, 0, (size_t)std::max(c->n_slots, 1u) * 4, c->stream));
-    c->n_invocation_floor = c->n_slots;
-    c->max_invocations_valid = false;
-    if (n_objects) {
-        floor_scatter_kernel<<<(n_objects + DF_THREADS - 1) / DF_THREADS, DF_THREADS, 0, c->stream>>>(c->deform->d_meshes, c->deform->d_slots,
-                                                                                                     c->deform->d_object_mesh, n_objects, c->d_invocation_floor);
-        R3_CHECK_LAUNCH(c, "floor_scatter_kernel");
-    }
     commit_set(c, true, n_meshes, n_objects, blocks, n_vertices, n_indices, n_objects ? slot_hi : 0);
+    c->deform->listed.assign(object_slots, object_slots + n_objects);
+    // the invocation floors: the listed slots' index_capacity (and the object-variant set's), zero elsewhere
+    R3_TRY(r3_rebuild_invocation_floors(c));
     c->deform->reads = reads;
     c->deform->remeshes.assign(meshes, meshes + n_meshes);
     R3_CUDA(c, r3_stream_sync(c));   // host pointers are only borrowed for the call

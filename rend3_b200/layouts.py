@@ -213,6 +213,12 @@ DEFORM_LEFT_HANDED, DEFORM_NORMALS, DEFORM_TANGENTS = 0x1, 0x2, 0x4
 REMESHABLE_MESH_DTYPE = _dt([("position_offset", u4, 0), ("normal_offset", u4, 4), ("tangent_offset", u4, 8), ("uv0_offset", u4, 12),
                              ("color0_offset", u4, 16), ("first_index", u4, 20), ("index_capacity", u4, 24), ("vertex_capacity", u4, 28),
                              ("flags", u4, 32)], 48)
+# r3_set_object_variants: one prepared mesh + material of an object (what ObjectManager::add takes from the mesh kind and the material)
+OBJECT_VARIANT_DTYPE = _dt([("first_index", u4, 0), ("index_count", u4, 4), ("material_index", u4, 8), ("attr_offset", (u4, 6), 12),
+                            ("sort_flags", u4, 36), ("material_key", "<u8", 40), ("mesh_sphere", (f4, 4), 48)], 64)
+VARIANT_GROUP_DTYPE = _dt([("first", u4, 0), ("count", u4, 4)], 8)
+# r3_readback_object_variants: a slot the set does not list, or one not switched since the set was made
+VARIANT_NONE = 0xFFFFFFFF
 # r3_readback_remesh_status: Mesh::validate's reasons, the first that applies
 REMESH_APPLIED, REMESH_OVER_CAPACITY, REMESH_NOT_TRIANGLES, REMESH_INDEX_OUT_OF_RANGE = 0, 1, 2, 3
 # object animation (r3_set_object_animations / r3_set_object_pose_jobs); jobs are POSE_JOB_DTYPE records

@@ -143,7 +143,7 @@ class BaseRenderGraph:
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
                      movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None,
-                     material_updates=None, joint_matrices=None, mesh_deforms=None, remeshes=None):
+                     material_updates=None, joint_matrices=None, mesh_deforms=None, remeshes=None, object_variants=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -189,7 +189,11 @@ class BaseRenderGraph:
         made by r3_set_remeshable_meshes (the rebuild of each mesh from new vertices and indices and the re-add of its objects) in the
         place of `mesh_deforms`; a context holds one of the two sets, so the two arguments are exclusive.  CUDA tensors go through
         r3_remesh_meshes_device (enqueue only; a mesh that fails validation is left as it was, see readback_remesh_status) and host arrays
-        through r3_remesh_meshes, which waits for the stream."""
+        through r3_remesh_meshes, which waits for the stream.
+        `object_variants` = (slots or None, choices) switches objects between the prepared mesh and material variants of the set made by
+        r3_set_object_variants (ObjectManager::add with another mesh kind or material) at the skinning node, before `object_presence` and
+        `object_transforms`: CUDA tensors through r3_switch_object_variants_device — enqueue only, their producer ordered on the
+        context's stream — and host arrays through r3_switch_object_variants, which waits for the stream."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -242,6 +246,12 @@ class BaseRenderGraph:
                 b.update_materials_device(records, indices)
             else:
                 b.update_materials(records, indices)
+        if object_variants is not None:                                           # :145 objects re-added with another mesh or material
+            slots, choices = object_variants
+            if getattr(choices, "is_cuda", False):
+                b.switch_object_variants_device(choices, slots)
+            else:
+                b.switch_object_variants(choices, slots)
         if object_presence is not None:                                           # :145 objects that appear or disappear this frame
             slots, enabled = object_presence
             if getattr(enabled, "is_cuda", False):

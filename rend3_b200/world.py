@@ -660,6 +660,21 @@ class Renderer:
 
     def add_object(self, obj: Object) -> int:
         h = self._alloc_object_handle()
+        self._place_object(h, obj)
+        return h
+
+    def readd_object(self, h: int, mesh: int, material: int):
+        """ObjectManager::add of handle h's object again, with another mesh and material, at its current transform and into the same
+        handle (object.rs:122-160, 267-284; duplicate_object with an ObjectChange, object.rs:201-218): the record's mesh range,
+        material and attribute offsets, the world sphere, the mesh sphere and the sort location (the world sphere's centre) are the
+        add's.  `enabled` stays as it is: presence is switched on its own (remove_object).  The expected state of
+        r3_switch_object_variants."""
+        e = self.objects[h]
+        enabled = int(e["rec"]["enabled"])
+        self._place_object(h, Object(mesh, material, e["obj"].transform))
+        self.objects[h]["rec"]["enabled"] = enabled
+
+    def _place_object(self, h: int, obj: Object):
         mesh = self.meshes[obj.mesh]
         rec = np.zeros((), dtype=OBJECT_DTYPE)
         t = np.asarray(obj.transform, dtype=f32)
@@ -674,7 +689,6 @@ class Renderer:
         rec["enabled"] = 1
         self.objects[h] = dict(rec=rec, obj=obj, mesh_center=mesh["center"], mesh_radius=mesh["radius"], location=c)
         self._use_index(h)
-        return h
 
     def duplicate_object(self, src: int, transform=None, material=None) -> int:
         o = self.objects[src]["obj"]
