@@ -610,7 +610,17 @@ class Renderer:
 
     def set_skybox(self, faces, srgb: bool = True, mips: str = "generated"):
         """SkyboxRoutine::set_background_texture with a cube texture (rend3-routine/src/skybox.rs:47-60): six square RGBA faces
-        in the order +X, -X, +Y, -Y, +Z, -Z; None removes it."""
+        in the order +X, -X, +Y, -Y, +Z, -Z; None removes it.  Like wgpu's cube textures, the faces must be equal squares of one
+        texel type — (n, n, 4) uint8 or float32 — because the library reads them at offsets computed from one face width."""
+        if faces is not None:
+            faces = [np.asarray(f) for f in faces]
+            if len(faces) != 6:
+                raise ValueError(f"set_skybox: six faces, got {len(faces)}")
+            shape, dtype = faces[0].shape, faces[0].dtype
+            if len(shape) != 3 or shape[0] != shape[1] or shape[0] == 0 or shape[2] != 4 or dtype not in (np.uint8, np.float32):
+                raise ValueError(f"set_skybox: faces must be (n, n, 4) uint8 or float32, got {shape} {dtype}")
+            if any(f.shape != shape or f.dtype != dtype for f in faces):
+                raise ValueError("set_skybox: the six faces must have the same shape and dtype")
         self.skybox = None if faces is None else [Texture(np.ascontiguousarray(f), srgb=srgb, mips=mips) for f in faces]
 
     def _skybox_blob(self):

@@ -159,28 +159,46 @@ def test_tile_culling_layouts(cuda, name):
 
 def test_scissor_rows(cuda):
     """A second frame shaded only in rows [13, 37) (the row split of the multi-GPU forward pass, begin not a multiple of 8):
-    the rows inside equal a full frame of the new lights and the reference, the rows outside keep the first frame."""
-    scene = scenes.grid_with_lights(40, 1)
-    orc = load_oracle_backend()
-    runners = {id(b): scenes.build(b, scene) for b in (cuda, orc)}
-    for b in (cuda, orc):
-        scenes.draw(runners[id(b)], scene, 1)
-    first = cuda.readback_hdr_f32()
-    moved = scenes.grid_with_lights(40, 1)
-    moved.point_lights = scenes.random_point_lights(40, seed=7)
-    for b in (cuda, orc):
-        runners[id(b)].renderer.point_lights = moved.point_lights
-        scenes.draw(runners[id(b)], scene, 1, scissor_rows=(13, 37))
-    inside = np.zeros((scene.height, scene.width), dtype=bool)
-    inside[13:37] = True
-    c = Case(cuda, moved)
-    c.exp = scenes.expected(moved, runners[id(cuda)].last_eval, atlas(cuda, runners[id(cuda)]))
-    a = c.check(1, "scissored frame", mask=inside, orc=orc)
-    assert np.array_equal(a[~inside], first[~inside].astype(np.float64)), "rows outside the scissor were written"
-    fresh = load_cuda_backend(0, parity_target=True)
-    scenes.render(fresh, moved, 1)
-    assert np.array_equal(a[inside], fresh.readback_hdr_f32()[inside].astype(np.float64)), "rows inside differ from the full frame"
-    fresh.close()
+    the rows inside equal a full frame of the new lights and the reference, the rows outside keep the first frame.  Once without
+    and once with a skybox behind the grid, so that skybox_kernel's rows are scissored too."""
+    import skybox_case
+
+    sky_faces = skybox_case.random_faces(16, "rgba8_srgb", seed=13)
+    for sky in (False, True):
+        scene = scenes.grid_with_lights(40, 1)
+
+        def build(b, scene):
+            r = scenes.build(b, scene)
+            if sky:
+                r.renderer.set_skybox(sky_faces, srgb=True)
+            return r
+
+        orc = load_oracle_backend()
+        runners = {id(b): build(b, scene) for b in (cuda, orc)}
+        for b in (cuda, orc):
+            scenes.draw(runners[id(b)], scene, 1)
+        first = cuda.readback_hdr_f32()
+        moved = scenes.grid_with_lights(40, 1)
+        moved.point_lights = scenes.random_point_lights(40, seed=7)
+        for b in (cuda, orc):
+            runners[id(b)].renderer.point_lights = moved.point_lights
+            scenes.draw(runners[id(b)], scene, 1, scissor_rows=(13, 37))
+        inside = np.zeros((scene.height, scene.width), dtype=bool)
+        inside[13:37] = True
+        c = Case(cuda, moved)
+        c.exp = scenes.expected(moved, runners[id(cuda)].last_eval, atlas(cuda, runners[id(cuda)]))
+        a = c.check(1, f"scissored frame, sky {sky}", mask=inside, orc=orc)
+        assert np.array_equal(a[~inside], first[~inside].astype(np.float64)), "rows outside the scissor were written"
+        fresh = load_cuda_backend(0, parity_target=True)
+        scenes.draw(build(fresh, moved), moved, 1)
+        assert np.array_equal(a[inside], fresh.readback_hdr_f32()[inside].astype(np.float64)), "rows inside differ from the full frame"
+        fresh.close()
+        if sky:
+            import skybox_reference
+
+            sky_px = inside & ~c.exp.f.mask
+            assert np.count_nonzero(sky_px) > 100, "no sky inside the rows"
+            skybox_reference.compare(a, skybox_case.reference(runners[id(cuda)], (scene.width, scene.height)), "scissored sky", mask=sky_px)
 
 
 def peak_mask(scene):
