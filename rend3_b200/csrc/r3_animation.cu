@@ -31,8 +31,6 @@ struct anim_skin_dev {                            // r3_anim_skin + its level ta
     uint64_t first_level, first_sched;
 };
 
-__device__ __forceinline__ float sqrt_rn(float a) { return __fsqrt_rn(a); }
-
 // sample_at_time (lib.rs:165-176): next = first key with time > t (the last key if none), prev = max(next - 1, 0),
 // s = clamp((t - t_prev) / (t_next - t_prev), 0, 1) with f32::clamp's compares (NaN stays NaN)
 __device__ __forceinline__ float key_factor(const float* __restrict__ keys, const r3_anim_track& tr, float t, uint32_t* prev, uint32_t* next) {
@@ -271,22 +269,17 @@ __global__ void __launch_bounds__(R3_OBJ_POSE_THREADS) pose_objects_kernel(const
     if (left_handed) sc.z = __uint_as_float(__float_as_uint(sc.z) ^ 0x80000000u);   // scale.z = -scale.z (lib.rs:201-203): a sign flip
     float m[16];
     from_srt(sc, q, tr, m);
-    // BoundingSphere::apply_transform (util/frustum.rs:22-32): Vec3::length_squared of each axis, f32::max (a NaN operand is ignored,
-    // as fmaxf ignores it), sqrt; centre = matrix * (c, 1) in mul_vec4's order; radius = max_scale * r
-    float ls[3];
+    float x[4], y[4], z[4];   // xyz of the four columns
 #pragma unroll
-    for (int a = 0; a < 3; ++a) ls[a] = add_rn(add_rn(mul_rn(m[4 * a], m[4 * a]), mul_rn(m[4 * a + 1], m[4 * a + 1])), mul_rn(m[4 * a + 2], m[4 * a + 2]));
-    const float max_scale = sqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
-    const float4 c = mat_vec_rn(m, tg.mesh_sphere_center[0], tg.mesh_sphere_center[1], tg.mesh_sphere_center[2], 1.0f);
+    for (int j = 0; j < 4; ++j) { x[j] = m[4 * j]; y[j] = m[4 * j + 1]; z[j] = m[4 * j + 2]; }
+    const float4 sph = sphere_apply_transform_rn(x, y, z, make_float4(tg.mesh_sphere_center[0], tg.mesh_sphere_center[1], tg.mesh_sphere_center[2], tg.mesh_sphere_radius));
     float4* rec = objects + (size_t)tg.slot * 8;
     rec[0] = make_float4(m[0], m[1], m[2], m[3]); rec[1] = make_float4(m[4], m[5], m[6], m[7]);
     rec[2] = make_float4(m[8], m[9], m[10], m[11]); rec[3] = make_float4(m[12], m[13], m[14], m[15]);
-    rec[4] = make_float4(c.x, c.y, c.z, mul_rn(max_scale, tg.mesh_sphere_radius));
-    // location = transform_point3a(Vec3A::ZERO): w + ((x * 0 + y * 0) + z * 0) per component — the translation for finite axes
+    rec[4] = sph;
     if (sort_loc && tg.slot < sort_n) {
         float* l = sort_loc + 3 * (size_t)tg.slot;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) l[k] = add_rn(m[12 + k], add_rn(add_rn(mul_rn(m[k], 0.0f), mul_rn(m[4 + k], 0.0f)), mul_rn(m[8 + k], 0.0f)));
+        l[0] = sort_location_rn(x); l[1] = sort_location_rn(y); l[2] = sort_location_rn(z);
     }
 }
 
@@ -592,7 +585,7 @@ int r3_anim_stage_posed_locations(r3_ctx* c, bool* staged) {
     *staged = false;
     r3_anim_state* a = c->anim;
     if (!a || !a->locations_pending) return R3_OK;
-    const uint32_t n = a->n_obj_items, sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    const uint32_t n = a->n_obj_items, sort_n = r3_sort_extent(c);
     if (n == 0 || sort_n == 0 || !c->d_sort_loc) { a->locations_pending = false; return R3_OK; }
     gather_locations_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(a->d_obj_slots, n, c->d_sort_loc, sort_n, a->d_loc_stage);
     R3_CHECK_LAUNCH(c, "gather_locations_kernel");
@@ -603,6 +596,7 @@ int r3_anim_stage_posed_locations(r3_ctx* c, bool* staged) {
 }
 void r3_anim_apply_posed_locations(r3_ctx* c) {
     r3_anim_state* a = c->anim;
+    if (!a || !a->locations_pending) return;   // stage enqueued nothing: it clears the flag unless it did
     const size_t sort_n = c->sort_key.size();
     for (size_t i = 0; i < a->obj_slots.size(); ++i)
         if (a->obj_slots[i] < sort_n) memcpy(&c->sort_loc[3 * (size_t)a->obj_slots[i]], &a->loc_stage[3 * i], 12);
@@ -622,7 +616,7 @@ R3_EXPORT int r3_set_object_animations(r3_ctx* c, const r3_anim_object_library* 
     if (!c) return R3_E_INVALID;
     const char* msg = "";
     if (r3_anim_check_object_library(L, &msg) != R3_OK) return r3_fail(c, R3_E_INVALID, msg);
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_object_animations: the object buffer is borrowed (r3_set_objects_device)");
+    R3_TRY(r3_check_object_writer(c, "set_object_animations", R3_NEED_OWNED));
     cudaSetDevice(c->device);
     R3_TRY(anim_state(c));
     r3_anim_state* a = c->anim;
@@ -649,7 +643,7 @@ R3_EXPORT int r3_set_object_pose_jobs(r3_ctx* c, const r3_pose_job* jobs, uint32
     if (!c) return R3_E_INVALID;
     r3_anim_state* a = c->anim;
     if (!a || !a->has_obj_library) return r3_fail(c, R3_E_STATE, "set_object_pose_jobs before set_object_animations");
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_object_pose_jobs: the object buffer is borrowed (r3_set_objects_device)");
+    R3_TRY(r3_check_object_writer(c, "set_object_pose_jobs", R3_NEED_OWNED));
     const char* msg = "";
     uint32_t* listed = nullptr;
     uint64_t n_items = 0;
@@ -687,11 +681,10 @@ R3_EXPORT int r3_pose_objects(r3_ctx* c) {
     if (!c) return R3_E_INVALID;
     r3_anim_state* a = c->anim;
     if (!a || !a->has_obj_jobs) return r3_fail(c, R3_E_STATE, "pose_objects before set_object_animations + set_object_pose_jobs");
-    if (!c->d_objects) return r3_fail(c, R3_E_STATE, "pose_objects before set_objects");
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "pose_objects: the object buffer is borrowed (r3_set_objects_device)");
+    R3_TRY(r3_check_object_writer(c, "pose_objects", R3_NEED_OBJECTS | R3_NEED_OWNED));
     if (a->n_obj_items == 0) return R3_OK;
     cudaSetDevice(c->device);
-    const uint32_t n = a->n_obj_items, sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    const uint32_t n = a->n_obj_items, sort_n = r3_sort_extent(c);
     pose_objects_kernel<<<(n + R3_OBJ_POSE_THREADS - 1) / R3_OBJ_POSE_THREADS, R3_OBJ_POSE_THREADS, 0, c->stream>>>(
         a->d_obj_items, n, a->d_obj_jobs, a->d_obj_targets, a->d_node_clips, a->d_node_channels, a->d_nodes, a->d_obj_keys, a->left_handed,
         reinterpret_cast<float4*>(c->d_objects), c->n_slots, c->d_sort_loc, sort_n);
@@ -706,7 +699,7 @@ R3_EXPORT int r3_readback_objects(r3_ctx* c, r3_object* out, float* locations, u
     if (!c) return R3_E_INVALID;
     if (!out && n) return r3_fail(c, R3_E_INVALID, "readback_objects: null");
     if ((uint64_t)first + n > c->n_slots) return r3_fail(c, R3_E_INVALID, "readback_objects: range outside the object buffer");
-    if (locations && (uint64_t)first + n > (c->have_live ? c->sort_key.size() : 0u))
+    if (locations && (uint64_t)first + n > r3_sort_extent(c))
         return r3_fail(c, R3_E_INVALID, "readback_objects: range outside the sort info");
     if (n == 0) return R3_OK;
     cudaSetDevice(c->device);

@@ -49,16 +49,13 @@ int r3_host_batch_objects(r3_ctx* c, r3_camera* cam, const float vp_loc[3], uint
     // every location (12 B per slot: the host does not know which slots a device list named), so that no extra drain is needed
     uint32_t nv = 0;
     // and, after r3_switch_object_variants_device, the listed slots' current variants (4 B per slot), from which the key mirrors follow
-    bool staged = false, moved = false, switched = false;
-    R3_TRY(r3_stage_moved_locations(c, &moved));
-    R3_TRY(r3_anim_stage_posed_locations(c, &staged));
-    R3_TRY(r3_variants_stage(c, &switched));
-    if (cam->d_visible_count || staged || moved || switched) {
+    bool mirrors = false;
+    R3_TRY(r3_stage_sort_mirrors(c, &mirrors));
+    if (cam->d_visible_count || mirrors) {
         if (cam->d_visible_count) R3_CUDA(c, cudaMemcpyAsync(&nv, cam->d_visible_count, 4, cudaMemcpyDeviceToHost, c->stream));
         R3_CUDA(c, r3_stream_sync(c));
     }
-    if (staged) r3_anim_apply_posed_locations(c);
-    if (switched) r3_variants_apply(c);
+    if (mirrors) r3_apply_sort_mirrors(c);
     cam->visible_count_host = (int)nv;
     std::vector<uint32_t> visible(nv), index_count(nv);
     if (nv) {

@@ -255,13 +255,11 @@ int r3_iobuf_swap(r3_ctx* c, r3_iobuf* b, uint64_t new_elems);
 int r3_launch_skinning(r3_ctx* c, const r3_skinning_input* d_inputs, const uint32_t* d_chunk_prefix, uint32_t n_skeletons, uint32_t total_chunks,
                        const float* d_joints, uint32_t n_joints);
 void r3_anim_destroy(r3_ctx* c);             // r3_animation.cu: frees c->anim (r3_ctx_destroy)
-// r3_animation.cu: after r3_pose_objects the host mirror c->sort_loc is behind the device's.  stage enqueues a copy of the posed slots'
-// locations to the host (*staged = true when it did); once the caller has drained the stream, apply writes them into c->sort_loc.
-int r3_anim_stage_posed_locations(r3_ctx* c, bool* staged);
-void r3_anim_apply_posed_locations(r3_ctx* c);
-// r3_object_transforms.cu: the same after r3_set_object_transforms / _device, whose moved slots the host may not know: stage enqueues a
-// copy of every location into c->sort_loc, complete once the caller has drained the stream
-int r3_stage_moved_locations(r3_ctx* c, bool* staged);
+// r3_object_transforms.cu: after device-side moves, poses and variant switches the host batching's sort mirrors (c->sort_loc, the key and
+// flag mirrors) are behind the device's.  stage enqueues the copies that bring them up to date (*pending = true when it enqueued any);
+// once the caller has drained the stream, apply writes what they brought into the mirrors.
+int r3_stage_sort_mirrors(r3_ctx* c, bool* pending);
+void r3_apply_sort_mirrors(r3_ctx* c);
 int r3_grow_mesh_spheres(r3_ctx* c, uint32_t n);   // r3_resize_objects: zero spheres for the new slots, once spheres are set
 // r3_ctx.cu: the host bookkeeping of r3_set_objects_enabled (exact: live bits of c->sort_flags, live key-2 count, any_blend) and, after
 // the device form has set c->presence_on_device, any_blend's conservative rule
@@ -283,15 +281,22 @@ int r3_variants_grow(r3_ctx* c, uint32_t n);          // r3_resize_objects: the 
 bool r3_variants_have_set(const r3_ctx* c);
 bool r3_variants_list(const r3_ctx* c, uint32_t slot);   // the set lists the slot
 int r3_variants_scatter_floors(r3_ctx* c);            // the listed slots' floors into c->d_invocation_floor (zeroed by the caller)
-// After r3_switch_object_variants_device the host's key / flag mirrors are behind the device's.  stage enqueues a copy of the listed slots'
-// current-variant words to the host and marks them seen on the device (*staged = true when it did); once the caller has drained the
-// stream, apply rebuilds the mirrors of the slots switched since.  sync is stage + drain + apply.
-int r3_variants_stage(r3_ctx* c, bool* staged);
-void r3_variants_apply(r3_ctx* c);
+// after r3_switch_object_variants_device: bring the host's key / flag mirrors up to date, blocking
 int r3_variants_sync_host(r3_ctx* c);
 // r3_ctx.cu: slot s's material key and flags bits 1-2 into the host mirrors, with the counts any_blend and gpu_batching_ok follow (the
 // caller re-derives them with r3_presence_derive)
 void r3_sort_set_key_flags(r3_ctx* c, uint32_t s, uint64_t key, uint8_t flags12);
+// slots with host sort facts (r3_set_object_sort_info): the device's key, location and live arrays cover [0, extent)
+static inline uint32_t r3_sort_extent(const r3_ctx* c) { return c->have_live ? (uint32_t)c->sort_key.size() : 0u; }
+// r3_ctx.cu: the preconditions of a call that writes object records.  Each failed one is R3_E_STATE with a message that starts with
+// `who`; they are checked in the order of the flags.
+enum : uint32_t {
+    R3_NEED_OBJECTS = 1u,   // an object buffer exists: "<who> before set_objects"
+    R3_NEED_HOT = 2u,       // ... and its cull + bake copies are valid (same message)
+    R3_NEED_OWNED = 4u,     // the buffer is not borrowed (r3_set_objects_device)
+    R3_NEED_SPHERES = 8u,   // r3_set_object_mesh_spheres covers every slot
+};
+int r3_check_object_writer(r3_ctx* c, const char* who, uint32_t needs);
 
 #ifdef __CUDACC__
 // Bit pattern of row 3 of an affine transform, column j: (+0, +0, +0, 1).  Bits, not floats: -0.0 and NaN are not affine
@@ -307,20 +312,37 @@ __device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, 
 __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
 __device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
 __device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ float sqrt_rn(float a) { return __fsqrt_rn(a); }
+// Slot s's bit of a bit-word array, set or cleared by an atomic: other slots of the word may be written by other threads
+__device__ __forceinline__ void slot_bit_assign(uint32_t* words, uint32_t s, bool on) {
+    const uint32_t bit = 1u << (s & 31u);
+    if (on) atomicOr(&words[s >> 5], bit);
+    else atomicAnd(&words[s >> 5], ~bit);
+}
+// *word = (*word & ~mask) | (bits & mask): a plain store when the warp owns the whole word, atomics when slots past the range share it
+__device__ __forceinline__ void store_bits(uint32_t* word, uint32_t bits, uint32_t mask) {
+    if (mask == 0xFFFFFFFFu) *word = bits;
+    else if (mask) { atomicAnd(word, ~mask | bits); atomicOr(word, bits & mask); }
+}
 // BoundingSphere::apply_transform (util/frustum.rs:22-32), rule R12's object half: Vec3::length_squared of each axis, f32::max (fmaxf
 // ignores a NaN operand as it does), sqrt; centre = matrix * (c, 1) in mul_vec4's order; radius = max_scale * r.  x, y, z: the xyz of the
-// matrix's four columns; ms: the mesh sphere (centre, radius).  Shared by r3_set_object_transforms and r3_deform_meshes.
+// matrix's four columns; ms: the mesh sphere (centre, radius).  Every writer of a world sphere uses it: moves, poses, deforms, variants.
 __device__ __forceinline__ float4 sphere_apply_transform_rn(const float (&x)[4], const float (&y)[4], const float (&z)[4], const float4& ms) {
     float ls[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) ls[c] = add_rn(add_rn(mul_rn(x[c], x[c]), mul_rn(y[c], y[c])), mul_rn(z[c], z[c]));
-    const float max_scale = __fsqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
+    const float max_scale = sqrt_rn(fmaxf(ls[0], fmaxf(ls[1], ls[2])));
     float4 sph;
     sph.x = add_rn(add_rn(add_rn(mul_rn(x[0], ms.x), mul_rn(x[1], ms.y)), mul_rn(x[2], ms.z)), mul_rn(x[3], 1.0f));
     sph.y = add_rn(add_rn(add_rn(mul_rn(y[0], ms.x), mul_rn(y[1], ms.y)), mul_rn(y[2], ms.z)), mul_rn(y[3], 1.0f));
     sph.z = add_rn(add_rn(add_rn(mul_rn(z[0], ms.x), mul_rn(z[1], ms.y)), mul_rn(z[2], ms.z)), mul_rn(z[3], 1.0f));
     sph.w = mul_rn(max_scale, ms.w);
     return sph;
+}
+// The sort location of a moved object, transform_point3a(Vec3A::ZERO), one component from one row r of the matrix (x, y or z as for
+// sphere_apply_transform_rn): w + ((x * 0 + y * 0) + z * 0) — the translation for finite axes, NaN for an infinite one
+__device__ __forceinline__ float sort_location_rn(const float (&r)[4]) {
+    return add_rn(r[3], add_rn(add_rn(mul_rn(r[0], 0.0f), mul_rn(r[1], 0.0f)), mul_rn(r[2], 0.0f)));
 }
 // M * (x, y, z, w): column-major, accumulated x,y,z,w like WGSL's mat4x4*vec4
 __device__ __forceinline__ float4 mat_vec_rn(const float* __restrict__ m, float x, float y, float z, float w) {

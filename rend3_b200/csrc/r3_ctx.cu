@@ -19,6 +19,15 @@ int r3_cuda_fail(r3_ctx* c, cudaError_t e, const char* where) {
     cudaGetLastError();   // clear the sticky-less error so later calls report their own
     return e == cudaErrorMemoryAllocation ? R3_E_OOM : R3_E_CUDA;
 }
+int r3_check_object_writer(r3_ctx* c, const char* who, uint32_t needs) {
+    const bool no_objects = !c->d_objects || ((needs & R3_NEED_HOT) && !c->hot_valid);
+    if ((needs & (R3_NEED_OBJECTS | R3_NEED_HOT)) && no_objects) return r3_fail(c, R3_E_STATE, (std::string(who) + " before set_objects").c_str());
+    if ((needs & R3_NEED_OWNED) && c->objects_borrowed)
+        return r3_fail(c, R3_E_STATE, (std::string(who) + ": the object buffer is borrowed (r3_set_objects_device)").c_str());
+    if ((needs & R3_NEED_SPHERES) && c->n_mesh_spheres < c->n_slots)
+        return r3_fail(c, R3_E_STATE, (std::string(who) + ": r3_set_object_mesh_spheres does not cover every slot").c_str());
+    return R3_OK;
+}
 
 int r3_reserve(r3_ctx* c, void** ptr, uint64_t* cap, uint64_t need, size_t elem, bool keep, bool zero_new) {
     if (*ptr && *cap >= need) return R3_OK;
@@ -582,9 +591,7 @@ __global__ void scatter_sort_info_kernel(const uint32_t* __restrict__ upd, uint3
     key8[s] = (uint8_t)(kl & 255u);
     const uint32_t* l = upd + 2 * (size_t)m + 3 * (size_t)i;
     loc[3 * (size_t)s] = __uint_as_float(l[0]); loc[3 * (size_t)s + 1] = __uint_as_float(l[1]); loc[3 * (size_t)s + 2] = __uint_as_float(l[2]);
-    const uint32_t bit = 1u << (s & 31u);   // slots of one word are written by different threads: as split_slots_kernel does
-    if (kl & 256u) atomicOr(&live_bits[s >> 5], bit);
-    else atomicAnd(&live_bits[s >> 5], ~bit);
+    slot_bit_assign(live_bits, s, kl & 256u);
 }
 
 // FreelistDerivedBuffer::apply's scatter of the stale entries (util/freelist/buffer.rs:85-97) for the facts batch_objects reads

@@ -123,13 +123,9 @@ __global__ void __launch_bounds__(256) split_slots_kernel(const float4* __restri
     const float tx = __shfl_up_sync(0xFFFFFFFFu, r.x, 1), ty = __shfl_up_sync(0xFFFFFFFFu, r.y, 1), tz = __shfl_up_sync(0xFFFFFFFFu, r.z, 1);   // column 3
     const uint32_t cb = __ballot_sync(0xFFFFFFFFu, ok && k == 4 && centre_is_translation(r.x, r.y, r.z, tx, ty, tz));
     if (ok && k == 7) {
-        const uint32_t bit = 1u << (s & 31u);
-        if (__float_as_uint(r.y) != 0u) atomicOr(&enabled_bits[s >> 5], bit);
-        else atomicAnd(&enabled_bits[s >> 5], ~bit);
-        if (((a >> (threadIdx.x & 24u)) & 0xFu) == 0xFu) atomicOr(&affine_bits[s >> 5], bit);
-        else atomicAnd(&affine_bits[s >> 5], ~bit);
-        if ((cb >> ((threadIdx.x & 24u) + 4u)) & 1u) atomicOr(&centre_bits[s >> 5], bit);
-        else atomicAnd(&centre_bits[s >> 5], ~bit);
+        slot_bit_assign(enabled_bits, s, __float_as_uint(r.y) != 0u);
+        slot_bit_assign(affine_bits, s, ((a >> (threadIdx.x & 24u)) & 0xFu) == 0xFu);
+        slot_bit_assign(centre_bits, s, (cb >> ((threadIdx.x & 24u) + 4u)) & 1u);
     }
 }
 

@@ -247,9 +247,7 @@ deform_objects_kernel(const deform_mesh_dev* __restrict__ meshes, const uint32_t
     objects[(size_t)s * 8 + 4] = sph;
     hot_spheres[s] = sph;
     radii[s] = sph.w;
-    const uint32_t bit = 1u << (s & 31u);
-    if (centre_is_translation(sph.x, sph.y, sph.z, x[3], y[3], z[3])) atomicOr(&centre_bits[s >> 5], bit);
-    else atomicAnd(&centre_bits[s >> 5], ~bit);
+    slot_bit_assign(centre_bits, s, centre_is_translation(sph.x, sph.y, sph.z, x[3], y[3], z[3]));
     if (sort_loc && s < sort_n) {   // location = the world sphere's centre (object.rs:273)
         float* l = sort_loc + 3 * (size_t)s;
         l[0] = sph.x; l[1] = sph.y; l[2] = sph.z;
@@ -517,7 +515,7 @@ int check_deform_state(r3_ctx* c, bool remesh, const char* who_state) {
     r3_deform_state* d = c->deform;
     if (!d || !d->valid || d->remesh != remesh) return r3_fail(c, R3_E_STATE, who_state);
     const char* who = remesh ? "remesh_meshes" : "deform_meshes";
-    if (c->objects_borrowed) return fail_s(c, R3_E_STATE, std::string(who) + ": the object buffer is borrowed (r3_set_objects_device)");
+    R3_TRY(r3_check_object_writer(c, who, R3_NEED_OWNED));
     if (d->n_objects) {
         if (!c->d_objects || !c->hot_valid || d->max_slot >= c->n_slots) return fail_s(c, R3_E_STATE, std::string(who) + ": a listed slot is past the slot count");
         if (d->max_slot >= c->n_mesh_spheres) return fail_s(c, R3_E_STATE, std::string(who) + ": r3_set_object_mesh_spheres does not cover every listed slot");
@@ -619,7 +617,7 @@ int launch_deform(r3_ctx* c, const float* d_pos) {
         R3_CHECK_LAUNCH(c, "deform_radius_kernel");
     }
     if (d->n_objects) {
-        const uint32_t sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+        const uint32_t sort_n = r3_sort_extent(c);
         deform_objects_kernel<<<(d->n_objects + DF_THREADS - 1) / DF_THREADS, DF_THREADS, 0, c->stream>>>(
             d->d_meshes, d->d_slots, d->d_object_mesh, d->n_objects, c->n_slots, d->remesh ? 1u : 0u, d->d_spheres, c->d_mesh_spheres, reinterpret_cast<float4*>(c->d_objects),
             c->d_hot_sphere, c->d_hot_radius, c->d_centre_bits, sort_n ? c->d_sort_loc : nullptr, sort_n);
@@ -680,8 +678,7 @@ R3_EXPORT int r3_set_deformable_meshes(r3_ctx* c, const r3_deformable_mesh* mesh
         if (n_objects) return r3_fail(c, R3_E_INVALID, "set_deformable_meshes: objects without meshes");
         return remove_set(c);
     }
-    if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, "set_deformable_meshes before set_objects");
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_deformable_meshes: the object buffer is borrowed (r3_set_objects_device)");
+    R3_TRY(r3_check_object_writer(c, "set_deformable_meshes", R3_NEED_HOT | R3_NEED_OWNED));
     // ---- the records, against the mesh buffer as it is
     const uint64_t buf = c->mesh_words * 4;
     uint64_t n_vertices = 0, n_indices = 0, idx_lo = ~0ull, idx_hi = 0;
@@ -809,8 +806,7 @@ R3_EXPORT int r3_set_remeshable_meshes(r3_ctx* c, const r3_remeshable_mesh* mesh
         if (n_objects) return r3_fail(c, R3_E_INVALID, "set_remeshable_meshes: objects without meshes");
         return remove_set(c);
     }
-    if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, "set_remeshable_meshes before set_objects");
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_remeshable_meshes: the object buffer is borrowed (r3_set_objects_device)");
+    R3_TRY(r3_check_object_writer(c, "set_remeshable_meshes", R3_NEED_HOT | R3_NEED_OWNED));
     // ---- the records: every capacity-sized range inside the buffer, and every range (all are written) disjoint from every other
     const uint64_t buf = c->mesh_words * 4;
     uint64_t n_vertices = 0, n_indices = 0;

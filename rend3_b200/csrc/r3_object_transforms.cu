@@ -77,31 +77,20 @@ object_transforms_kernel(const float4* __restrict__ mats, const uint32_t* __rest
             if (k == 0) objects[(size_t)s * 8 + 4] = sph;
             else if (k == 1) { spheres[s] = sph; radii[s] = sph.w; }
             else if (k == 2) {
-                // location = transform_point3a(Vec3A::ZERO): w + ((x * 0 + y * 0) + z * 0) per component — NaN for an inf axis
                 if (sort_loc && s < sort_n) {
                     float* l = sort_loc + 3 * (size_t)s;
-                    l[0] = add_rn(x[3], add_rn(add_rn(mul_rn(x[0], 0.0f), mul_rn(x[1], 0.0f)), mul_rn(x[2], 0.0f)));
-                    l[1] = add_rn(y[3], add_rn(add_rn(mul_rn(y[0], 0.0f), mul_rn(y[1], 0.0f)), mul_rn(y[2], 0.0f)));
-                    l[2] = add_rn(z[3], add_rn(add_rn(mul_rn(z[0], 0.0f), mul_rn(z[1], 0.0f)), mul_rn(z[2], 0.0f)));
+                    l[0] = sort_location_rn(x); l[1] = sort_location_rn(y); l[2] = sort_location_rn(z);
                 }
             } else if (SPARSE) {
-                const uint32_t bit = 1u << (s & 31u);   // other slots of the word may be written by other warps
-                if (affine) atomicOr(&affine_bits[s >> 5], bit);
-                else atomicAnd(&affine_bits[s >> 5], ~bit);
-                if (centred) atomicOr(&centre_bits[s >> 5], bit);
-                else atomicAnd(&centre_bits[s >> 5], ~bit);
+                slot_bit_assign(affine_bits, s, affine);
+                slot_bit_assign(centre_bits, s, centred);
             }
         }
     }
-    if (!SPARSE && lane == 0) {
-        if (n - base >= 32u) { affine_bits[wtile] = abits; centre_bits[wtile] = cbits; }
-        else {   // the last word also holds slots past n: they keep their bits
-            const uint32_t mask = (1u << (n - base)) - 1u;
-            atomicAnd(&affine_bits[wtile], ~mask | abits);
-            atomicOr(&affine_bits[wtile], abits);
-            atomicAnd(&centre_bits[wtile], ~mask | cbits);
-            atomicOr(&centre_bits[wtile], cbits);
-        }
+    if (!SPARSE && lane == 0) {   // the last word also holds slots past n: they keep their bits
+        const uint32_t mask = n - base >= 32u ? 0xFFFFFFFFu : (1u << (n - base)) - 1u;
+        store_bits(&affine_bits[wtile], abits, mask);
+        store_bits(&centre_bits[wtile], cbits, mask);
     }
 }
 
@@ -123,15 +112,13 @@ int check_slots(r3_ctx* c, const uint32_t* slots, uint32_t n, uint32_t limit, co
     return R3_OK;
 }
 
-int check_state(r3_ctx* c) {
-    if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, "set_object_transforms before set_objects");
-    if (c->n_mesh_spheres < c->n_slots) return r3_fail(c, R3_E_STATE, "set_object_transforms: r3_set_object_mesh_spheres does not cover every slot");
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_object_transforms: the object buffer is borrowed (r3_set_objects_device)");
-    return R3_OK;
+int check_state(r3_ctx* c) {   // of two failed preconditions, the mesh spheres' message comes before the borrowed buffer's
+    R3_TRY(r3_check_object_writer(c, "set_object_transforms", R3_NEED_HOT | R3_NEED_SPHERES));
+    return r3_check_object_writer(c, "set_object_transforms", R3_NEED_OWNED);
 }
 
 int launch_transforms(r3_ctx* c, const uint32_t* d_slots, const float* d_mats, uint32_t n) {
-    const uint32_t sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    const uint32_t sort_n = r3_sort_extent(c);
     const uint32_t ctas = (uint32_t)(((uint64_t)n + OT_THREADS - 1) / OT_THREADS);   // a warp walks 32 entries: 256 per CTA
     auto kernel = d_slots ? object_transforms_kernel<true> : object_transforms_kernel<false>;
     kernel<<<ctas, OT_THREADS, 0, c->stream>>>(reinterpret_cast<const float4*>(d_mats), d_slots, n, c->n_slots, c->d_mesh_spheres, reinterpret_cast<float4*>(c->d_objects),
@@ -159,19 +146,8 @@ objects_enabled_sparse_kernel(const uint32_t* __restrict__ slots, const uint8_t*
     if (s >= n_slots) return;   // out-of-range writes are dropped (ScatterCopy's robust access)
     const bool on = __ldg(enabled + i) != 0;
     objects[(size_t)s * 32 + EN_WORD] = on ? 1u : 0u;
-    const uint32_t bit = 1u << (s & 31u);
-    if (on) atomicOr(&enabled_bits[s >> 5], bit);
-    else atomicAnd(&enabled_bits[s >> 5], ~bit);
-    if (s < sort_n) {
-        if (on) atomicOr(&live_bits[s >> 5], bit);
-        else atomicAnd(&live_bits[s >> 5], ~bit);
-    }
-}
-
-// *word = (*word & ~mask) | (bits & mask): a plain store when the warp owns the whole word, atomics when slots past the range share it
-__device__ __forceinline__ void store_bits(uint32_t* word, uint32_t bits, uint32_t mask) {
-    if (mask == 0xFFFFFFFFu) *word = bits;
-    else if (mask) { atomicAnd(word, ~mask | bits); atomicOr(word, bits & mask); }
+    slot_bit_assign(enabled_bits, s, on);
+    if (s < sort_n) slot_bit_assign(live_bits, s, on);
 }
 
 // dense: entry i is slot i; a warp owns one 32-slot word, ballots the 32 flags and stores the bit words whole
@@ -250,11 +226,7 @@ object_variants_kernel(const uint32_t* __restrict__ slots, const uint32_t* __res
         current[s] = v | tag;
     }
     if (SPARSE) {
-        if (ok) {
-            const uint32_t bit = 1u << (s & 31u);
-            if (centred) atomicOr(&centre_bits[s >> 5], bit);
-            else atomicAnd(&centre_bits[s >> 5], ~bit);
-        }
+        if (ok) slot_bit_assign(centre_bits, s, centred);
     } else {
         const uint32_t applied = __ballot_sync(0xFFFFFFFFu, ok), bits = __ballot_sync(0xFFFFFFFFu, ok && centred);
         if ((threadIdx.x & 31u) == 0) store_bits(&centre_bits[i >> 5], bits, applied);
@@ -275,14 +247,8 @@ __global__ void variant_words_seen_kernel(uint32_t* __restrict__ current, uint32
     if (s < n) current[s] &= ~VR_UNSEEN;
 }
 
-int check_presence_state(r3_ctx* c, const char* who) {
-    if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, who);
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_objects_enabled: the object buffer is borrowed (r3_set_objects_device)");
-    return R3_OK;
-}
-
 int launch_enabled(r3_ctx* c, const uint32_t* d_slots, const uint8_t* d_enabled, uint32_t n) {
-    const uint32_t sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    const uint32_t sort_n = r3_sort_extent(c);
     uint32_t* objects = reinterpret_cast<uint32_t*>(c->d_objects);
     uint32_t* live = sort_n ? c->d_live_bits : nullptr;
     const uint32_t ctas = (uint32_t)(((uint64_t)n + EN_THREADS - 1) / EN_THREADS);
@@ -303,7 +269,7 @@ struct r3_variant_state {
     std::vector<r3_object_variant> variants;  // host copies: validation, floors and the key mirrors
     std::vector<r3_variant_group> groups;
     std::vector<uint32_t> slot_group;         // per slot: its group, VR_NONE when unlisted
-    std::vector<uint32_t> staged;             // current words read back by r3_variants_stage
+    std::vector<uint32_t> staged;             // current words read back by variants_stage
     float4* d_variants = nullptr; uint32_t variants_cap = 0;
     uint4* d_groups = nullptr; uint32_t groups_cap = 0;   // first, count, floor, 0
     uint32_t* d_slot_group = nullptr; uint32_t* d_current = nullptr; uint32_t slots_cap = 0;
@@ -314,16 +280,14 @@ namespace {
 int check_variant_state(r3_ctx* c, const char* who) {
     const r3_variant_state* V = c->variants;
     if (!V || !V->n_variants) return r3_fail(c, R3_E_STATE, who);
-    if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, "switch_object_variants before set_objects");
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "switch_object_variants: the object buffer is borrowed (r3_set_objects_device)");
-    if (c->n_mesh_spheres < c->n_slots) return r3_fail(c, R3_E_STATE, "switch_object_variants: r3_set_object_mesh_spheres does not cover every slot");
+    R3_TRY(r3_check_object_writer(c, "switch_object_variants", R3_NEED_HOT | R3_NEED_OWNED | R3_NEED_SPHERES));
     if (c->mesh_words < V->index_end) return r3_fail(c, R3_E_STATE, "switch_object_variants: the mesh buffer ends before a variant's indices");
     return R3_OK;
 }
 
 int launch_variants(r3_ctx* c, const uint32_t* d_slots, const uint32_t* d_choices, uint32_t n, uint32_t tag) {
     const r3_variant_state* V = c->variants;
-    const uint32_t sort_n = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    const uint32_t sort_n = r3_sort_extent(c);
     const uint32_t n_slots = std::min(c->n_slots, V->n_slots);
     const uint32_t ctas = (uint32_t)(((uint64_t)n + VR_THREADS - 1) / VR_THREADS);
     auto kernel = d_slots ? object_variants_kernel<true> : object_variants_kernel<false>;
@@ -382,7 +346,10 @@ int r3_variants_scatter_floors(r3_ctx* c) {
     return R3_OK;
 }
 
-int r3_variants_stage(r3_ctx* c, bool* staged) {
+// After r3_switch_object_variants_device the host's key / flag mirrors are behind the device's.  stage enqueues a copy of the listed slots'
+// current-variant words to the host and marks them seen on the device (*staged = true when it did; c->variants_on_device stays set until
+// apply); once the caller has drained the stream, apply rebuilds the mirrors of the slots switched since.
+static int variants_stage(r3_ctx* c, bool* staged) {
     *staged = false;
     if (!c->variants_on_device) return R3_OK;
     r3_variant_state* V = c->variants;
@@ -399,9 +366,9 @@ int r3_variants_stage(r3_ctx* c, bool* staged) {
     return R3_OK;
 }
 
-void r3_variants_apply(r3_ctx* c) {
+static void variants_apply(r3_ctx* c) {
     const r3_variant_state* V = c->variants;
-    const uint32_t sorted = c->have_live ? (uint32_t)std::min<size_t>(c->sort_key.size(), V->staged.size()) : 0u;
+    const uint32_t sorted = std::min(r3_sort_extent(c), (uint32_t)V->staged.size());
     for (uint32_t s = 0; s < sorted; ++s) {
         const uint32_t w = V->staged[s];
         if (w == VR_NONE || !(w & VR_UNSEEN)) continue;
@@ -414,10 +381,10 @@ void r3_variants_apply(r3_ctx* c) {
 
 int r3_variants_sync_host(r3_ctx* c) {
     bool staged = false;
-    R3_TRY(r3_variants_stage(c, &staged));
+    R3_TRY(variants_stage(c, &staged));
     if (!staged) return R3_OK;
     R3_CUDA(c, r3_stream_sync(c));
-    r3_variants_apply(c);
+    variants_apply(c);
     return R3_OK;
 }
 
@@ -436,9 +403,7 @@ R3_EXPORT int r3_set_object_variants(r3_ctx* c, const r3_object_variant* variant
         r3_presence_derive(c);
         return R3_OK;
     }
-    if (!c->d_objects || !c->hot_valid) return r3_fail(c, R3_E_STATE, "set_object_variants before set_objects");
-    if (c->objects_borrowed) return r3_fail(c, R3_E_STATE, "set_object_variants: the object buffer is borrowed (r3_set_objects_device)");
-    if (c->n_mesh_spheres < c->n_slots) return r3_fail(c, R3_E_STATE, "set_object_variants: r3_set_object_mesh_spheres does not cover every slot");
+    R3_TRY(r3_check_object_writer(c, "set_object_variants", R3_NEED_HOT | R3_NEED_OWNED | R3_NEED_SPHERES));
     // ---- every argument before anything is written
     uint64_t index_end = 0;
     bool key2 = false, wide = false;
@@ -531,7 +496,7 @@ R3_EXPORT int r3_switch_object_variants(r3_ctx* c, const uint32_t* slots, const 
     R3_CUDA(c, r3_stream_sync(c));               // host pointers are only borrowed for the call
     R3_TRY(r3_variants_sync_host(c));            // earlier device switches of other slots: their mirrors too
     // the host sees every entry: its key and flag mirrors stay exact
-    const uint32_t sorted = c->have_live ? (uint32_t)c->sort_key.size() : 0u;
+    const uint32_t sorted = r3_sort_extent(c);
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t s = slots ? slots[i] : i;
         if (s >= sorted) continue;
@@ -573,7 +538,7 @@ R3_EXPORT int r3_set_objects_enabled(r3_ctx* c, const uint32_t* slots, const uin
     if (!c) return R3_E_INVALID;
     if (n == 0) return R3_OK;
     if (!enabled) return r3_fail(c, R3_E_INVALID, "set_objects_enabled: null");
-    R3_TRY(check_presence_state(c, "set_objects_enabled before set_objects"));
+    R3_TRY(r3_check_object_writer(c, "set_objects_enabled", R3_NEED_HOT | R3_NEED_OWNED));
     if (!slots && n > c->n_slots) return r3_fail(c, R3_E_INVALID, "set_objects_enabled: more flags than slots");
     if (slots) R3_TRY(check_slots(c, slots, n, c->n_slots, "set_objects_enabled: slot beyond the object buffer", "set_objects_enabled: one slot named twice"));
     cudaSetDevice(c->device);
@@ -592,7 +557,8 @@ R3_EXPORT int r3_set_objects_enabled_device(r3_ctx* c, const uint32_t* d_slots, 
     if (!c) return R3_E_INVALID;
     if (n == 0) return R3_OK;
     if (!d_enabled || ((uintptr_t)d_slots & 3u)) return r3_fail(c, R3_E_INVALID, "set_objects_enabled_device: null or misaligned pointer (slots: 4 bytes)");
-    R3_TRY(check_presence_state(c, "set_objects_enabled_device before set_objects"));
+    R3_TRY(r3_check_object_writer(c, "set_objects_enabled_device", R3_NEED_HOT));
+    R3_TRY(r3_check_object_writer(c, "set_objects_enabled", R3_NEED_OWNED));   // both forms name the host form here
     if (!d_slots && n > c->n_slots) return r3_fail(c, R3_E_INVALID, "set_objects_enabled_device: more flags than slots");
     cudaSetDevice(c->device);
     R3_TRY(launch_enabled(c, d_slots, d_enabled, n));
@@ -665,13 +631,31 @@ int r3_grow_mesh_spheres(r3_ctx* c, uint32_t n) {
 // Host batching sorts by the host mirror c->sort_loc.  After a move the device's locations are ahead of it, and for the device form the
 // host does not know which slots moved: stage enqueues a copy of the whole array into the mirror (*staged = true when it did); it is
 // complete once the caller has drained the stream, which the host batching does anyway for the visible list.
-int r3_stage_moved_locations(r3_ctx* c, bool* staged) {
+static int stage_moved_locations(r3_ctx* c, bool* staged) {
     *staged = false;
     if (!c->locations_moved) return R3_OK;
     c->locations_moved = false;
-    const size_t sort_n = c->have_live ? c->sort_key.size() : 0u;
+    const size_t sort_n = r3_sort_extent(c);
     if (sort_n == 0 || !c->d_sort_loc) return R3_OK;
     R3_CUDA(c, cudaMemcpyAsync(c->sort_loc.data(), c->d_sort_loc, sort_n * 12, cudaMemcpyDeviceToHost, c->stream));
     *staged = true;
     return R3_OK;
+}
+
+// r3_animation.cu: the posed slots' locations, staged and applied as above (apply does nothing unless stage enqueued a copy)
+int r3_anim_stage_posed_locations(r3_ctx* c, bool* staged);
+void r3_anim_apply_posed_locations(r3_ctx* c);
+
+int r3_stage_sort_mirrors(r3_ctx* c, bool* pending) {
+    bool moved = false, posed = false, switched = false;
+    R3_TRY(stage_moved_locations(c, &moved));
+    R3_TRY(r3_anim_stage_posed_locations(c, &posed));
+    R3_TRY(variants_stage(c, &switched));
+    *pending = moved || posed || switched;
+    return R3_OK;
+}
+
+void r3_apply_sort_mirrors(r3_ctx* c) {
+    r3_anim_apply_posed_locations(c);
+    if (c->variants_on_device) variants_apply(c);   // still set: variants_stage enqueued a copy
 }
