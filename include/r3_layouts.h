@@ -179,6 +179,29 @@ typedef struct r3_directional_light_source {
 R3_STATIC_ASSERT(sizeof(r3_directional_light_source) == 48, "DirectionalLight source");
 R3_STATIC_ASSERT(offsetof(r3_directional_light_source, resolution) == 32, "resolution");
 
+/* One DirectionalLightChange (rend3-types/src/lib.rs:1106-1121, applied field by field by update_from_changes, :232-238) for the light
+ * at shadow index `index` of the current set: r3_update_directional_light_sources[_device].  A field is applied when its bit is in
+ * `mask`.  There is no resolution bit: a new resolution re-packs the shadow atlas, which r3_set_directional_light_sources does. */
+#define R3_DIR_CHANGE_COLOR 0x1u
+#define R3_DIR_CHANGE_INTENSITY 0x2u
+#define R3_DIR_CHANGE_DIRECTION 0x4u
+#define R3_DIR_CHANGE_DISTANCE 0x8u
+typedef struct r3_directional_light_change {
+    uint32_t index;               /* @0  shadow index in the current set */
+    uint32_t mask;                /* @4  R3_DIR_CHANGE_* */
+    float color[3];               /* @8 */
+    float intensity;              /* @20 */
+    float direction[3];           /* @24 */
+    float distance;               /* @36 */
+    uint32_t _pad[2];             /* @40 */
+} r3_directional_light_change;
+R3_STATIC_ASSERT(sizeof(r3_directional_light_change) == 48, "DirectionalLightChange");
+R3_STATIC_ASSERT(offsetof(r3_directional_light_change, mask) == 4, "mask");
+R3_STATIC_ASSERT(offsetof(r3_directional_light_change, color) == 8, "color");
+R3_STATIC_ASSERT(offsetof(r3_directional_light_change, intensity) == 20, "intensity");
+R3_STATIC_ASSERT(offsetof(r3_directional_light_change, direction) == 24, "direction");
+R3_STATIC_ASSERT(offsetof(r3_directional_light_change, distance) == 36, "distance");
+
 /* ShaderPointLight — rend3/src/managers/point.rs:21-26; buffer = u32 count @0, array @16 */
 typedef struct r3_point_light {
     float position[4];

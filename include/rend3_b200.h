@@ -22,7 +22,8 @@
  *     (r3_object_uniform_upload, r3_batch_objects, r3_cull, r3_shadow_pass, r3_forward_*, r3_hiz_build, r3_tonemap,
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
  *     r3_switch_object_variants_device, r3_update_materials_device, r3_set_joint_matrices_device, r3_deform_meshes_device, r3_remesh_meshes_device, r3_evaluate_shadow_cameras,
- *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights,
+ *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights, r3_update_directional_light_sources,
+ *     r3_update_directional_light_sources_device,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
@@ -415,6 +416,32 @@ int r3_set_directional_light_sources(r3_ctx*, const r3_directional_light_source*
 int r3_evaluate_shadow_cameras(r3_ctx*, const float viewport_location[3]);
 int r3_shadow_uniform_upload(r3_ctx*, uint32_t shadow_index, uint32_t object_count, uint32_t mode);
 int r3_readback_shadow_cameras(r3_ctx*, r3_camera_header* out, r3_directional_light* lights_or_null, uint32_t n);
+/* DirectionalLightManager::update (directional.rs:91-93, Renderer::update_directional_light at renderer/mod.rs:369) on the lights of the
+ * current set: entry i applies the fields of changes[i].mask to the light at shadow index changes[i].index, as update_from_changes does.
+ * Entries apply in array order and a later entry's fields override an earlier one's, as consecutive update_directional_light calls queued
+ * in one frame do, so an index named twice is legal.  An empty mask changes nothing.  Nothing is clamped: NaN, inf, a negative intensity,
+ * a zero direction, a direction along +-Y and distance 0 reach R13 as given, with its degenerate results.  One kernel (one thread per
+ * light) rewrites the sources and the light records' colour * intensity (the single multiply of r3_set_directional_light_sources) and
+ * direction; view_proj and the shadow cameras come from the next r3_evaluate_shadow_cameras, which reads distance and direction.
+ *   r3_update_directional_light_sources         HOST memory, enqueue only: legal between r3_frame_begin and r3_frame_end.  Checked first:
+ *                                               a non-null pointer when n > 0, every index < the light count, no mask bit outside
+ *                                               R3_DIR_CHANGE_*; a rejected call returns R3_E_INVALID and enqueues nothing.  The entries
+ *                                               travel as kernel parameters, 64 per launch (n > 64: consecutive launches in array order);
+ *                                               nothing is copied to the device and nothing waits, so `changes` is free on return.
+ *                                               Frames whose n stays within 1 .. 64 launch one kernel each and keep the frame graph's
+ *                                               topology, so the graph is updated in place.  The host copy of the sources follows.
+ *   r3_update_directional_light_sources_device  DEVICE memory (4-byte aligned), enqueue only; producer ordering as for
+ *                                               r3_set_object_transforms_device.  An entry whose index is at or past the light count, or
+ *                                               whose mask has an unknown bit, is dropped whole.  The host copy of colour, intensity,
+ *                                               direction and distance is stale afterwards; the host reads only each light's `size`
+ *                                               (r3_shadow_uniform_upload), which neither form changes.
+ * R3_E_STATE from both unless the lights came from r3_set_directional_light_sources (none yet, or r3_set_directional_lights since).
+ * n == 0 is R3_OK and launches nothing.  After an update, r3_shadow_uniform_upload, r3_readback_shadow_cameras, r3_forward_resolve and
+ * r3_forward_blend return R3_E_STATE until r3_evaluate_shadow_cameras has run.  A later r3_set_directional_light_sources replaces
+ * everything.  Resolution is not a field here: a new resolution, like an added or removed light, re-packs the atlas (shadow_alloc.rs), so
+ * it goes through r3_set_directional_light_sources with the new placements. */
+int r3_update_directional_light_sources(r3_ctx*, const r3_directional_light_change* changes, uint32_t n);
+int r3_update_directional_light_sources_device(r3_ctx*, const r3_directional_light_change* d_changes, uint32_t n);
 int r3_set_frame_uniforms(r3_ctx*, const r3_frame_uniforms* uniforms);             /* uniforms.rs:94-106 */
 
 /* ------------------------------------------------------------------ GPU skinning

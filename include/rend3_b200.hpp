@@ -62,6 +62,10 @@ struct EvalOutput {
     // the same lights as sources + atlas placements, in the light buffer's order, and the handedness: what
     // r3_set_directional_light_sources takes when the shadow cameras are evaluated on the device
     const r3_directional_light_source* directional_sources = nullptr; uint32_t n_directional_sources = 0; bool left_handed = true;
+    // DirectionalLightChanges of this frame (DirectionalLightManager::update) for those sources, applied before their shadow cameras are
+    // evaluated: in HOST memory or in DEVICE memory (producer ordered on the context's stream); both only enqueue work
+    const r3_directional_light_change* directional_changes = nullptr; uint32_t n_directional_changes = 0;
+    const r3_directional_light_change* d_directional_changes = nullptr; uint32_t n_d_directional_changes = 0;
     const void* point_lights = nullptr; uint64_t point_bytes = 0;
     // PointLightManager's handle table behind point_lights (records + live bytes, dead handles included): what
     // r3_set_point_light_sources takes when the point lights are evaluated on the device
@@ -248,6 +252,9 @@ public:
         if (submit_as_graph) r.check(r3_frame_begin(r.raw()));
         r.check(r3_clear_shadow_atlas(r.raw()));                                                     // base.rs:139
         r.check(r3_set_frame_uniforms(r.raw(), &ev.uniforms));                                       // :142
+        if (ev.n_directional_changes) r.check(r3_update_directional_light_sources(r.raw(), ev.directional_changes, ev.n_directional_changes));
+        if (ev.n_d_directional_changes)
+            r.check(r3_update_directional_light_sources_device(r.raw(), ev.d_directional_changes, ev.n_d_directional_changes));
         if (device_shadow_cameras) r.check(r3_evaluate_shadow_cameras(r.raw(), ev.viewport_location));
         if (device_point_lights) r.check(r3_evaluate_point_lights(r.raw()));                       // renderer/eval.rs:180
         if (ev.n_material_updates) r.check(r3_update_materials(r.raw(), ev.material_indices, ev.material_records, ev.n_material_updates));

@@ -50,6 +50,7 @@ ENTRY_POINTS = [
     "set_deformable_meshes", "deform_meshes", "deform_meshes_device", "readback_deformable_mesh_spheres",
     "set_remeshable_meshes", "remesh_meshes", "remesh_meshes_device", "readback_remesh_status", "debug_invocation_bound",
     "set_object_variants", "switch_object_variants", "switch_object_variants_device", "readback_object_variants",
+    "update_directional_light_sources", "update_directional_light_sources_device",
 ]
 
 
@@ -338,6 +339,31 @@ class Backend:
 
     def shadow_uniform_upload(self, shadow_index: int, object_count: int, mode: int = CB_BAKE | CB_CULL):
         self._call("shadow_uniform_upload", C.c_uint32(shadow_index), C.c_uint32(object_count), C.c_uint32(mode))
+
+    def update_directional_light_sources(self, changes):
+        """DirectionalLightChanges from host memory: a contiguous 1-d DIRECTIONAL_LIGHT_CHANGE_DTYPE array.  Enqueue only."""
+        from .layouts import DIRECTIONAL_LIGHT_CHANGE_DTYPE
+
+        c = changes
+        assert isinstance(c, np.ndarray) and c.dtype == DIRECTIONAL_LIGHT_CHANGE_DTYPE and c.ndim == 1 and c.flags.c_contiguous, \
+            "changes: a contiguous 1-d DIRECTIONAL_LIGHT_CHANGE_DTYPE array"
+        self._call("update_directional_light_sources", _ptr(c) if len(c) else None, C.c_uint32(len(c)))
+
+    def update_directional_light_sources_device(self, changes, n: Optional[int] = None):
+        """The same from device memory, enqueue only; entries naming no light or carrying an unknown mask bit are dropped.  `changes` is
+        a contiguous CUDA tensor of 48-byte records (uint8 (n, 48), or int32 / uint32 / float32 (n, 12)), or a raw device pointer with `n`
+        given; the caller keeps it alive and orders its producer on stream()."""
+        if isinstance(changes, int):
+            assert n is not None, "changes: a raw pointer needs n"
+            ptr = changes
+        else:
+            x = changes
+            assert getattr(x, "is_cuda", False) and x.is_contiguous() and x.dim() == 2 and x.element_size() in (1, 4) \
+                and x.shape[1] * x.element_size() == 48 and not (x.element_size() == 1 and x.is_floating_point()) \
+                and x.data_ptr() % 4 == 0, "changes: a contiguous CUDA tensor of 48-byte records (uint8 (n, 48) or 4-byte (n, 12))"
+            assert n is None or n == x.shape[0], "n: the tensor's row count"
+            ptr, n = x.data_ptr(), x.shape[0]
+        self._call("update_directional_light_sources_device", C.c_void_p(ptr), C.c_uint32(n))
 
     def readback_shadow_cameras(self, n: int):
         """(CAMERA_HEADER_DTYPE[n], DIRECTIONAL_LIGHT_DTYPE[n])"""

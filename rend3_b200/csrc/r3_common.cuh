@@ -143,6 +143,8 @@ struct r3_ctx {
     r3_directional_light_source* d_light_src = nullptr; r3_camera_header* d_shadow_cams = nullptr;
     std::vector<r3_directional_light_source> light_src;
     bool light_src_set = false, shadow_cams_evaluated = false; uint32_t light_src_left_handed = 0;
+    // r3_update_directional_light_sources[_device] ran since the last r3_evaluate_shadow_cameras: the cameras and view_proj are stale
+    bool dir_eval_pending = false;
     // ShaderPointLightBuffer as the shading reads it: u32 count @0, r3_point_light array @16 (allocated at context creation, count 0).
     // The count is only known on the device; point_capacity (r3_set_point_lights' count, or the handle table's size) bounds it and sizes
     // the light prep.  point_handles: size of PointLightManager's handle table (r3_lights.cu), sources + live bytes on the device.

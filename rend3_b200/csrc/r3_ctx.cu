@@ -732,6 +732,7 @@ R3_EXPORT int r3_set_directional_lights(r3_ctx* c, const void* bytes, uint64_t n
     if (n) R3_CUDA(c, cudaMemcpyAsync(c->d_dir, (const uint8_t*)bytes + 16, (size_t)n * sizeof(r3_directional_light), cudaMemcpyHostToDevice, c->stream));
     c->n_dir = n;
     c->light_src_set = false;   // replaces r3_set_directional_light_sources
+    c->dir_eval_pending = false;
     if (aw != c->atlas_w || ah != c->atlas_h || !c->d_atlas) {
         R3_CUDA(c, r3_stream_sync(c));
         cudaFree(c->d_atlas);

@@ -8,6 +8,7 @@
 //   r3_evaluate_shadow_cameras        one thread per light writes the light's view_proj and its camera header (view, view_proj, frustum)
 //   r3_shadow_uniform_upload          the cull + bake of Shadow(i) reading that header on the device
 //   r3_readback_shadow_cameras        blocking readback of the headers and light records
+//   r3_update_directional_light_sources[_device]  DirectionalLightChanges applied to the sources and the light records' static fields
 // and PointLightManager's handle table with its evaluate (second half of the file).
 #include <algorithm>
 #include <cmath>
@@ -148,6 +149,61 @@ __global__ void __launch_bounds__(64) shadow_camera_kernel(const r3_directional_
     cams[i] = h;
 }
 
+// ---- DirectionalLightManager::update (directional.rs:91-93): update_from_changes of the masked fields
+constexpr uint32_t DIR_CHANGE_BITS = R3_DIR_CHANGE_COLOR | R3_DIR_CHANGE_INTENSITY | R3_DIR_CHANGE_DIRECTION | R3_DIR_CHANGE_DISTANCE;
+constexpr uint32_t DIR_CHANGE_BATCH = 64;   // entries per launch of the host form: 3 KB of kernel parameters, under the 4 KB limit
+
+// the host mirror and the kernel apply an entry through this one function
+__host__ __device__ __forceinline__ void apply_directional_change(r3_directional_light_source& s, const r3_directional_light_change& e) {
+    const uint32_t m = e.mask;
+    if (m & R3_DIR_CHANGE_COLOR) { s.color[0] = e.color[0]; s.color[1] = e.color[1]; s.color[2] = e.color[2]; }
+    if (m & R3_DIR_CHANGE_INTENSITY) s.intensity = e.intensity;
+    if (m & R3_DIR_CHANGE_DIRECTION) { s.direction[0] = e.direction[0]; s.direction[1] = e.direction[1]; s.direction[2] = e.direction[2]; }
+    if (m & R3_DIR_CHANGE_DISTANCE) s.distance = e.distance;
+}
+
+// where the entries come from: a batch passed by value as kernel parameters (host form) or an array in device memory (device form)
+struct DirChangeParams {
+    r3_directional_light_change e[DIR_CHANGE_BATCH];
+    __device__ const r3_directional_light_change& operator[](uint32_t k) const { return e[k]; }
+};
+struct DirChangeDevice {
+    const r3_directional_light_change* p;
+    __device__ const r3_directional_light_change& operator[](uint32_t k) const { return p[k]; }
+};
+
+// thread i owns light i and walks the entries in array order, so a later entry's fields override an earlier one's.  An entry naming
+// no light of the set or carrying an unknown bit is dropped whole (the host form has rejected those already).  A light that some
+// non-empty mask touched gets its source and the light record's static fields rewritten: colour * intensity with the single multiply of
+// r3_set_directional_light_sources, direction copied.  view_proj and the camera header are the next r3_evaluate_shadow_cameras'.
+template <class Changes>
+__global__ void __launch_bounds__(64) directional_light_change_kernel(const __grid_constant__ Changes changes, uint32_t n, uint32_t n_lights,
+                                                                      r3_directional_light_source* __restrict__ src,
+                                                                      r3_directional_light* __restrict__ lights) {
+    const uint32_t i = threadIdx.x;
+    if (i >= n_lights) return;
+    r3_directional_light_source s = src[i];
+    bool changed = false;
+    for (uint32_t k = 0; k < n; ++k) {
+        const r3_directional_light_change& e = changes[k];
+        if (e.index != i || (e.mask & ~DIR_CHANGE_BITS)) continue;
+        apply_directional_change(s, e);
+        changed |= e.mask != 0;
+    }
+    if (!changed) return;
+    src[i] = s;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { lights[i].color[k] = __fmul_rn(s.color[k], s.intensity); lights[i].direction[k] = s.direction[k]; }
+}
+
+template <class Changes>
+int launch_directional_light_change(r3_ctx* c, const Changes& changes, uint32_t n) {
+    static_assert(R3_MAX_SHADOWS <= 64, "one thread per light");
+    directional_light_change_kernel<Changes><<<1, 64, 0, c->stream>>>(changes, n, (uint32_t)c->light_src.size(), c->d_light_src, c->d_dir);
+    R3_CHECK_LAUNCH(c, "directional_light_change_kernel");
+    return R3_OK;
+}
+
 }  // namespace
 
 R3_EXPORT int r3_set_directional_light_sources(r3_ctx* c, const r3_directional_light_source* lights, uint32_t n, uint32_t aw, uint32_t ah,
@@ -181,6 +237,41 @@ R3_EXPORT int r3_set_directional_light_sources(r3_ctx* c, const r3_directional_l
     c->light_src_left_handed = left_handed ? 1u : 0u;
     c->light_src_set = true;
     c->shadow_cams_evaluated = false;
+    c->dir_eval_pending = false;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_update_directional_light_sources(r3_ctx* c, const r3_directional_light_change* changes, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (!c->light_src_set) return r3_fail(c, R3_E_STATE, "update_directional_light_sources before set_directional_light_sources");
+    if (!changes && n) return r3_fail(c, R3_E_INVALID, "update_directional_light_sources: null changes");
+    for (uint32_t k = 0; k < n; ++k) {
+        if (changes[k].index >= c->light_src.size()) return r3_fail(c, R3_E_INVALID, "update_directional_light_sources: no such light");
+        if (changes[k].mask & ~DIR_CHANGE_BITS) return r3_fail(c, R3_E_INVALID, "update_directional_light_sources: unknown mask bit");
+    }
+    if (n == 0) return R3_OK;
+    cudaSetDevice(c->device);
+    // the entries travel by value: nothing is copied to the device and nothing waits, so `changes` is free on return
+    for (uint32_t first = 0; first < n; first += DIR_CHANGE_BATCH) {
+        DirChangeParams batch;
+        memset(&batch, 0, sizeof batch);
+        const uint32_t m = std::min(n - first, DIR_CHANGE_BATCH);
+        memcpy(batch.e, changes + first, (size_t)m * sizeof *changes);
+        R3_TRY(launch_directional_light_change(c, batch, m));
+    }
+    for (uint32_t k = 0; k < n; ++k) apply_directional_change(c->light_src[changes[k].index], changes[k]);
+    c->dir_eval_pending = true;
+    return R3_OK;
+}
+
+R3_EXPORT int r3_update_directional_light_sources_device(r3_ctx* c, const r3_directional_light_change* d_changes, uint32_t n) {
+    if (!c) return R3_E_INVALID;
+    if (!c->light_src_set) return r3_fail(c, R3_E_STATE, "update_directional_light_sources_device before set_directional_light_sources");
+    if (n == 0) return R3_OK;
+    if (!d_changes) return r3_fail(c, R3_E_INVALID, "update_directional_light_sources_device: null changes");
+    cudaSetDevice(c->device);
+    R3_TRY(launch_directional_light_change(c, DirChangeDevice{d_changes}, n));
+    c->dir_eval_pending = true;
     return R3_OK;
 }
 
@@ -195,12 +286,14 @@ R3_EXPORT int r3_evaluate_shadow_cameras(r3_ctx* c, const float loc[3]) {
         R3_CHECK_LAUNCH(c, "shadow_camera_kernel");
     }
     c->shadow_cams_evaluated = true;
+    c->dir_eval_pending = false;
     return R3_OK;
 }
 
 R3_EXPORT int r3_shadow_uniform_upload(r3_ctx* c, uint32_t shadow_index, uint32_t object_count, uint32_t mode) {
     if (!c) return R3_E_INVALID;
     if (!c->light_src_set || !c->shadow_cams_evaluated) return r3_fail(c, R3_E_STATE, "shadow_uniform_upload before set_directional_light_sources + evaluate_shadow_cameras");
+    if (c->dir_eval_pending) return r3_fail(c, R3_E_STATE, "shadow_uniform_upload: directional lights updated since the last evaluate_shadow_cameras");
     if (shadow_index >= c->light_src.size()) return r3_fail(c, R3_E_INVALID, "shadow_uniform_upload: no such light");
     if (object_count > c->n_slots) return r3_fail(c, R3_E_INVALID, "object_count exceeds the object buffer");
     cudaSetDevice(c->device);
@@ -223,6 +316,7 @@ R3_EXPORT int r3_readback_shadow_cameras(r3_ctx* c, r3_camera_header* out, r3_di
     if (!c) return R3_E_INVALID;
     if (!out && n) return r3_fail(c, R3_E_INVALID, "readback_shadow_cameras: null");
     if (!c->light_src_set || !c->shadow_cams_evaluated) return r3_fail(c, R3_E_STATE, "readback_shadow_cameras before evaluate_shadow_cameras");
+    if (c->dir_eval_pending) return r3_fail(c, R3_E_STATE, "readback_shadow_cameras: directional lights updated since the last evaluate_shadow_cameras");
     if (n > c->light_src.size()) return r3_fail(c, R3_E_INVALID, "readback_shadow_cameras: more cameras than lights");
     cudaSetDevice(c->device);
     if (n) R3_CUDA(c, cudaMemcpyAsync(out, c->d_shadow_cams, (size_t)n * sizeof *out, cudaMemcpyDeviceToHost, c->stream));

@@ -1041,6 +1041,7 @@ R3_EXPORT int r3_forward_resolve(r3_ctx* c) {
     if (!c || !c->d_vis) return r3_fail(c, R3_E_STATE, "forward_resolve before set_render_target");
     if (!c->uniforms_set) return r3_fail(c, R3_E_STATE, "forward_resolve before set_frame_uniforms");
     if (c->point_eval_pending) return r3_fail(c, R3_E_STATE, "forward_resolve: point lights set or updated since the last evaluate_point_lights");
+    if (c->dir_eval_pending) return r3_fail(c, R3_E_STATE, "forward_resolve: directional lights updated since the last evaluate_shadow_cameras");
     cudaSetDevice(c->device);
     const uint64_t need_floats = (uint64_t)c->n_dir * 32 + (uint64_t)c->point_capacity * 8 + 64;
     static_assert(sizeof(DirPrep) == 32 * 4 && sizeof(PointPrep) == 8 * 4, "prep sizes");
@@ -1075,6 +1076,7 @@ R3_EXPORT int r3_forward_blend(r3_ctx* c) {
     if (!c || !c->d_vis) return r3_fail(c, R3_E_STATE, "forward_blend before set_render_target");
     if (!c->uniforms_set) return r3_fail(c, R3_E_STATE, "forward_blend before set_frame_uniforms");
     if (c->point_eval_pending) return r3_fail(c, R3_E_STATE, "forward_blend: point lights set or updated since the last evaluate_point_lights");
+    if (c->dir_eval_pending) return r3_fail(c, R3_E_STATE, "forward_blend: directional lights updated since the last evaluate_shadow_cameras");
     cudaSetDevice(c->device);
     bool ran = false;
     R3_TRY(r3_blend_collect(c, &ran));

@@ -152,6 +152,11 @@ LIGHT_SOURCE_DTYPE = _dt(
     48,
 )
 
+# r3_directional_light_change: one DirectionalLightChange for the light at a shadow index (r3_update_directional_light_sources[_device])
+DIR_CHANGE_COLOR, DIR_CHANGE_INTENSITY, DIR_CHANGE_DIRECTION, DIR_CHANGE_DISTANCE = 1, 2, 4, 8
+DIRECTIONAL_LIGHT_CHANGE_DTYPE = _dt([("index", u4, 0), ("mask", u4, 4), ("color", (f4, 3), 8), ("intensity", f4, 20), ("direction", (f4, 3), 24),
+                                      ("distance", f4, 36)], 48)
+
 MATERIAL_DTYPE = _dt(
     [
         ("textures", (u4, 10), 0),

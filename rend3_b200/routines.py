@@ -143,7 +143,8 @@ class BaseRenderGraph:
                      after_target=None, tonemap: bool = True, skinning=None, frame_graph: Optional[bool] = None, before_resolve=None,
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
                      movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None,
-                     material_updates=None, joint_matrices=None, mesh_deforms=None, remeshes=None, object_variants=None):
+                     material_updates=None, joint_matrices=None, mesh_deforms=None, remeshes=None, object_variants=None,
+                     directional_changes=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -193,7 +194,10 @@ class BaseRenderGraph:
         `object_variants` = (slots or None, choices) switches objects between the prepared mesh and material variants of the set made by
         r3_set_object_variants (ObjectManager::add with another mesh kind or material) at the skinning node, before `object_presence` and
         `object_transforms`: CUDA tensors through r3_switch_object_variants_device — enqueue only, their producer ordered on the
-        context's stream — and host arrays through r3_switch_object_variants, which waits for the stream."""
+        context's stream — and host arrays through r3_switch_object_variants, which waits for the stream.
+        `directional_changes` = DirectionalLightChanges (DIRECTIONAL_LIGHT_CHANGE_DTYPE records) applied to the lights of
+        `device_shadow_cameras` right before their shadow cameras are evaluated (DirectionalLightManager::update): a CUDA tensor through
+        r3_update_directional_light_sources_device, a host array through r3_update_directional_light_sources; both only enqueue work."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -217,6 +221,12 @@ class BaseRenderGraph:
                 if shadow_filter(i):
                     b.clear_shadow_rect(s.offset[0], s.offset[1], s.size, s.size)
         b.set_frame_uniforms(frame_uniforms(ev.camera, settings.ambient_color, resolution))  # :142
+        if directional_changes is not None:                                       # DirectionalLightManager::update
+            assert device_shadow_cameras, "directional_changes: the lights are sources only with device_shadow_cameras"
+            if getattr(directional_changes, "is_cuda", False):
+                b.update_directional_light_sources_device(directional_changes)
+            else:
+                b.update_directional_light_sources(directional_changes)
         if device_shadow_cameras:                                                 # DirectionalLightManager::evaluate around this camera
             b.evaluate_shadow_cameras(ev.camera.location())
         if point_light_updates is not None:                                       # PointLightManager::{add, update, remove}

@@ -20,6 +20,7 @@ Mirrors (names kept so tests read like rend3-test/tests/*.rs):
 """
 from __future__ import annotations
 
+import dataclasses
 from dataclasses import dataclass, field
 from typing import List, Optional, Tuple
 
@@ -51,6 +52,11 @@ from .layouts import (
     MAT_UNLIT,
     MATERIAL_DTYPE,
     OBJECT_DTYPE,
+    DIR_CHANGE_COLOR,
+    DIR_CHANGE_DIRECTION,
+    DIR_CHANGE_DISTANCE,
+    DIR_CHANGE_INTENSITY,
+    DIRECTIONAL_LIGHT_CHANGE_DTYPE,
     DIRECTIONAL_LIGHT_DTYPE,
     LIGHT_SOURCE_DTYPE,
     POINT_LIGHT_DTYPE,
@@ -376,6 +382,16 @@ class DirectionalLight:
     direction: Tuple[float, float, float]
     distance: float
     resolution: int
+
+
+@dataclass
+class DirectionalLightChange:
+    """rend3-types DirectionalLightChange (lib.rs:1106-1121): None leaves the field as it is."""
+    color: Optional[Tuple[float, float, float]] = None
+    intensity: Optional[float] = None
+    direction: Optional[Tuple[float, float, float]] = None
+    distance: Optional[float] = None
+    resolution: Optional[int] = None
 
 
 @dataclass
@@ -724,6 +740,47 @@ class Renderer:
     def add_directional_light(self, light: DirectionalLight) -> int:
         self.dir_lights.append(light)
         return len(self.dir_lights) - 1
+
+    def update_directional_light(self, handle: int, change: DirectionalLightChange):
+        """Renderer::update_directional_light (renderer/mod.rs:369) -> DirectionalLightManager::update (directional.rs:91-93):
+        update_from_changes (rend3-types/src/lib.rs:232-238) sets every field the change carries, so consecutive changes merge field by
+        field and the later one wins.  A new resolution re-packs the shadow atlas at the next evaluate."""
+        fields = {f: getattr(change, f) for f in ("color", "intensity", "direction", "distance", "resolution")}
+        self.dir_lights[handle] = dataclasses.replace(self.dir_lights[handle], **{f: v for f, v in fields.items() if v is not None})
+
+    def remove_directional_light(self, handle: int):
+        """DirectionalLightManager::remove (directional.rs:95-97): data[handle] = None; the other handles keep their index."""
+        self.dir_lights[handle] = None
+
+    def directional_shadow_index(self, handle: int) -> int:
+        """The shadow index of a live light: its position in the light buffer, ShadowDesc list and sources evaluate() builds (the
+        atlas's placement order over the live handles).  What r3_directional_light_change.index names."""
+        live = [(i, l.resolution) for i, l in enumerate(self.dir_lights) if l is not None]
+        atlas = allocate_shadow_atlas(live)
+        order = [] if atlas is None else [h for _, _, _, h in atlas[1]]
+        if handle not in order:
+            raise KeyError(f"directional light {handle} is not live")
+        return order.index(handle)
+
+    def directional_change_records(self, changes) -> np.ndarray:
+        """[(handle, DirectionalLightChange)] as DIRECTIONAL_LIGHT_CHANGE_DTYPE records for r3_update_directional_light_sources[_device],
+        in the same order (a later entry overrides an earlier one's fields there too).  Take them before the set changes (a light added or
+        removed moves the shadow indices).  A change of resolution re-packs the shadow atlas: it has no record and goes through
+        r3_set_directional_light_sources with evaluate()'s new placements (ValueError here)."""
+        out = np.zeros(len(changes), dtype=DIRECTIONAL_LIGHT_CHANGE_DTYPE)
+        for k, (handle, c) in enumerate(changes):
+            if c.resolution is not None:
+                raise ValueError("a resolution change re-packs the shadow atlas: set the lights again (r3_set_directional_light_sources)")
+            out[k]["index"] = self.directional_shadow_index(handle)
+            mask = 0
+            for bit, f in ((DIR_CHANGE_COLOR, "color"), (DIR_CHANGE_INTENSITY, "intensity"), (DIR_CHANGE_DIRECTION, "direction"),
+                           (DIR_CHANGE_DISTANCE, "distance")):
+                v = getattr(c, f)
+                if v is not None:
+                    out[k][f] = v
+                    mask |= bit
+            out[k]["mask"] = mask
+        return out
 
     def add_point_light(self, light: PointLight) -> int:
         self.point_lights.append(light)
