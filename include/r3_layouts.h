@@ -312,6 +312,26 @@ typedef struct r3_texture_desc {
 } r3_texture_desc;
 R3_STATIC_ASSERT(sizeof(r3_texture_desc) == 32, "r3_texture_desc");
 
+/* One rectangle of texels for r3_write_texture_regions[_device]: raw bytes in the target's storage format, copied into one level of one
+ * texture of the table or one face of the skybox.  `texture` is a table index or R3_SKYBOX_FACE(f), f = 0..5 in the order +X -X +Y -Y +Z -Z.
+ * x, y, width, height are texels of that level; the source rows (block rows for BC formats) start at src_offset and src_pitch apart. */
+#define R3_SKYBOX_FACE(f) (0x80000000u | (f))
+typedef struct r3_texture_region {
+    uint64_t src_offset;          /* @0  bytes into the caller's source, a multiple of the element size */
+    uint32_t texture;             /* @8  table index, or R3_SKYBOX_FACE(f) */
+    uint32_t level;               /* @12 mip level of that texture / face */
+    uint32_t x, y, width, height; /* @16 texels of that level */
+    uint32_t src_pitch;           /* @32 bytes between consecutive source rows (block rows for BC formats) */
+    uint32_t _reserved;           /* @36 0 */
+} r3_texture_region;
+R3_STATIC_ASSERT(sizeof(r3_texture_region) == 40, "r3_texture_region");
+R3_STATIC_ASSERT(offsetof(r3_texture_region, texture) == 8, "texture");
+R3_STATIC_ASSERT(offsetof(r3_texture_region, level) == 12, "level");
+R3_STATIC_ASSERT(offsetof(r3_texture_region, x) == 16, "x");
+R3_STATIC_ASSERT(offsetof(r3_texture_region, width) == 24, "width");
+R3_STATIC_ASSERT(offsetof(r3_texture_region, src_pitch) == 32, "src_pitch");
+R3_STATIC_ASSERT(offsetof(r3_texture_region, _reserved) == 36, "_reserved");
+
 /* GpuSkinningInput — rend3-routine/src/skinning.rs:20-45, skinning.wgsl:3-26 (40 bytes, byte offsets into the mesh buffer,
  * R3_ATTR_ABSENT when an attribute is missing) */
 typedef struct r3_skinning_input {

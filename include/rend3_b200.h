@@ -23,7 +23,7 @@
  *     r3_skin's kernel, r3_pose_skeletons, r3_skin_posed, r3_pose_objects, r3_set_object_transforms_device, r3_set_objects_enabled_device,
  *     r3_switch_object_variants_device, r3_update_materials_device, r3_set_joint_matrices_device, r3_deform_meshes_device, r3_remesh_meshes_device, r3_evaluate_shadow_cameras,
  *     r3_shadow_uniform_upload, r3_update_point_light_sources_device, r3_evaluate_point_lights, r3_update_directional_light_sources,
- *     r3_update_directional_light_sources_device,
+ *     r3_update_directional_light_sources_device, r3_write_texture_regions_device,
  *     r3_exchange_merge, r3_peer_*) only enqueue work on the
  *     context's stream and return.
  *     What BLOCKS the calling thread until the stream has drained: r3_sync, every r3_readback_*, r3_visible_count,
@@ -34,7 +34,8 @@
  *     r3_set_object_pose_jobs, r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_objects_enabled, r3_set_object_variants,
  *     r3_switch_object_variants, r3_set_deformable_meshes,
  *     r3_deform_meshes, r3_set_remeshable_meshes, r3_remesh_meshes, r3_readback_remesh_status, r3_set_directional_light_sources,
- *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights —
+ *     r3_readback_shadow_cameras, r3_set_point_light_sources, r3_update_point_light_sources, r3_readback_point_lights,
+ *     r3_write_texture_regions —
  *     because the pointer is only valid for the duration of the call (they are the counterpart of queue.write_buffer,
  *     which copies before it returns).  r3_set_objects_device borrows device memory and does not block.  A buffer that
  *     has to grow (first frame, larger world, new resolution) is reallocated with a stream synchronisation as well.
@@ -362,6 +363,36 @@ int r3_update_textures(r3_ctx*, uint32_t first, const r3_texture_desc* descs, ui
  * still holds its clear value.  desc->width = face size (height is ignored), six faces in the order +X, -X, +Y, -Y, +Z, -Z, each with
  * its `mip_count` levels stored tightly, face after face, from desc->byte_offset.  desc == NULL removes the skybox. */
 int r3_set_skybox(r3_ctx*, const r3_texture_desc* desc, const void* texels, uint64_t nbytes);
+/* Textures that change (a video frame, a simulation's or a painting's output, streamed virtual-texture pages, a time-of-day sky): rend3's
+ * textures are immutable (TextureManager::add, texture.rs:98-251), so there a changed texture is added again and its materials updated.
+ * Here each r3_texture_region copies raw bytes, already in the target's storage format, into one rectangle of one level of a table
+ * texture or a skybox face.  There is no format conversion and no mip regeneration: the other levels keep their bytes.
+ *   - The element is the format's texel (R3_TEXFMT_BPP: 1, 2, 4, 8 or 16 bytes), for BC1-BC5 and BC7 a 4x4 block
+ *     (R3_TEXFMT_BLOCK_BYTES), and a source row is a row of elements (a block row).  A level's bytes start after the earlier levels'
+ *     R3_TEXFMT_LEVEL_BYTES; a skybox face's at sky_desc.byte_offset + f * face_bytes, the layout r3_set_skybox checks.
+ *   - A region is valid when its target exists (an index below the table's count, or a face 0-5 with a skybox set), level < mip_count,
+ *     width and height are above 0 and the rectangle lies inside the level; for block formats x and y are multiples of 4 and width and
+ *     height multiples of 4 or reaching the level's edge (so ragged 6x6, 2x2 and 1x1 tail levels are writable); src_offset and src_pitch
+ *     are multiples of the element size and src_pitch >= the row's bytes; the last source row ends within nbytes; _reserved == 0.
+ *   r3_write_texture_regions         HOST pointers, blocking.  The whole call is checked first against the host's copy of the descriptors
+ *                                    (which r3_set_textures and r3_update_textures keep): an invalid region, two regions of one target and
+ *                                    level whose rectangles meet, or a null pointer returns R3_E_INVALID and leaves the context unchanged.
+ *                                    Otherwise one copy of the regions and one of the texels go into a grow-only scratch, the two kernels
+ *                                    below run and the stream is drained once (inside a frame graph that flushes, as r3_update_materials).
+ *   r3_write_texture_regions_device  DEVICE pointers, enqueue only; legal between r3_frame_begin and r3_frame_end.  Regions 8-byte
+ *                                    aligned; producer ordering as for r3_set_object_transforms_device.  An invalid region is dropped whole
+ *                                    and the others apply.  Regions that do not overlap are a precondition: where two overlap, the bytes
+ *                                    are unspecified.  Writes land in whatever blob the stream holds at that point, so they order with
+ *                                    r3_set_textures / r3_update_textures by stream order.
+ * Both run one planning CTA and one persistent copy grid whose sizes depend on the SM count only, so frames whose n stays above 0 keep
+ * the frame graph's topology; the plan scratch grows with n and never shrinks, so only a call with a larger n than before can flush.
+ * R3_E_STATE from both when there is neither a texture table nor a skybox.  n == 0 is R3_OK and launches nothing.  A later
+ * r3_set_textures or r3_set_skybox replaces everything.
+ * r3_readback_texels copies nbytes at byte_offset of the table's blob (skybox == 0) or the skybox's (skybox != 0, up to the end of face
+ * 5) to the host; R3_E_INVALID for a range outside it.  Blocking. */
+int r3_write_texture_regions(r3_ctx*, const r3_texture_region* regions, uint32_t n, const void* texels, uint64_t nbytes);
+int r3_write_texture_regions_device(r3_ctx*, const r3_texture_region* d_regions, uint32_t n, const void* d_texels, uint64_t nbytes);
+int r3_readback_texels(r3_ctx*, int skybox, uint64_t byte_offset, void* out, uint64_t nbytes);
 int r3_set_directional_lights(r3_ctx*, const void* bytes, uint64_t nbytes,
                               uint32_t atlas_width, uint32_t atlas_height);         /* directional.rs:135-156 */
 int r3_set_point_lights(r3_ctx*, const void* bytes, uint64_t nbytes);              /* point.rs:58-74 */

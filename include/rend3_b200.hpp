@@ -121,6 +121,11 @@ struct EvalOutput {
         const float* tangents = nullptr; const float* uv0 = nullptr; const uint32_t* color0 = nullptr; uint64_t n_vertices = 0, n_indices = 0;
     };
     RemeshStreams remesh, d_remesh;
+    // textures that change this frame (in rend3 added again and their materials updated): rectangles of stored bytes patched into the
+    // table's and the skybox's levels, in HOST memory (blocking) or in DEVICE memory (enqueue only, regions 8-byte aligned, producer
+    // ordered on the context's stream); applied before the first pass that samples them
+    const r3_texture_region* texture_regions = nullptr; uint32_t n_texture_regions = 0; const void* texture_write_texels = nullptr; uint64_t texture_write_bytes = 0;
+    const r3_texture_region* d_texture_regions = nullptr; uint32_t n_d_texture_regions = 0; const void* d_texture_write_texels = nullptr; uint64_t d_texture_write_bytes = 0;
 };
 
 struct BaseRenderGraphSettings {              // base.rs:95-98
@@ -257,6 +262,10 @@ public:
             r.check(r3_update_directional_light_sources_device(r.raw(), ev.d_directional_changes, ev.n_d_directional_changes));
         if (device_shadow_cameras) r.check(r3_evaluate_shadow_cameras(r.raw(), ev.viewport_location));
         if (device_point_lights) r.check(r3_evaluate_point_lights(r.raw()));                       // renderer/eval.rs:180
+        if (ev.n_texture_regions)
+            r.check(r3_write_texture_regions(r.raw(), ev.texture_regions, ev.n_texture_regions, ev.texture_write_texels, ev.texture_write_bytes));
+        if (ev.n_d_texture_regions)
+            r.check(r3_write_texture_regions_device(r.raw(), ev.d_texture_regions, ev.n_d_texture_regions, ev.d_texture_write_texels, ev.d_texture_write_bytes));
         if (ev.n_material_updates) r.check(r3_update_materials(r.raw(), ev.material_indices, ev.material_records, ev.n_material_updates));
         if (ev.n_d_material_updates) r.check(r3_update_materials_device(r.raw(), ev.d_material_indices, ev.d_material_records, ev.n_d_material_updates));
         gpu_skinner.add_skinning_to_graph(r, ev);                                                    // :145 state.skinning — before any camera culls

@@ -51,6 +51,7 @@ ENTRY_POINTS = [
     "set_remeshable_meshes", "remesh_meshes", "remesh_meshes_device", "readback_remesh_status", "debug_invocation_bound",
     "set_object_variants", "switch_object_variants", "switch_object_variants_device", "readback_object_variants",
     "update_directional_light_sources", "update_directional_light_sources_device",
+    "write_texture_regions", "write_texture_regions_device", "readback_texels",
 ]
 
 
@@ -321,6 +322,41 @@ class Backend:
         desc = np.ascontiguousarray(desc).reshape(1)
         texels = np.ascontiguousarray(texels).view(np.uint8).reshape(-1)
         self._call("set_skybox", _ptr(desc), _ptr(texels), C.c_uint64(len(texels)))
+
+    # ---- textures that change (rectangles of texels into the table's levels and the skybox's faces)
+    def write_texture_regions(self, regions, texels):
+        """TEXTURE_REGION_DTYPE regions (a contiguous 1-d array) copying bytes of `texels` (any contiguous host array, taken as its raw
+        bytes) into the table's and the skybox's levels.  Checked as a whole first; blocking."""
+        from .layouts import TEXTURE_REGION_DTYPE
+
+        r = regions
+        assert isinstance(r, np.ndarray) and r.dtype == TEXTURE_REGION_DTYPE and r.ndim == 1 and r.flags.c_contiguous, \
+            "regions: a contiguous 1-d TEXTURE_REGION_DTYPE array"
+        assert isinstance(texels, np.ndarray) and texels.flags.c_contiguous, "texels: a contiguous host array"
+        t = texels.reshape(-1).view(np.uint8)
+        self._call("write_texture_regions", _ptr(r) if len(r) else None, C.c_uint32(len(r)), _ptr(t) if len(t) else None, C.c_uint64(len(t)))
+
+    def write_texture_regions_device(self, regions, texels, n: Optional[int] = None):
+        """The same from device memory, enqueue only; invalid regions are dropped.  `regions` is a contiguous CUDA tensor of 40-byte records
+        (uint8 (n, 40), int32 / uint32 (n, 10) or int64 / uint64 (n, 5)) at an 8-byte aligned address, `texels` a contiguous CUDA tensor
+        taken as its raw bytes; `n` (default: every row) may name fewer regions.  The caller keeps both alive and orders their producer on
+        stream()."""
+        x = regions
+        assert getattr(x, "is_cuda", False) and x.is_contiguous() and x.dim() == 2 and x.element_size() in (1, 4, 8) \
+            and x.shape[1] * x.element_size() == 40 and not x.is_floating_point() and x.data_ptr() % 8 == 0, \
+            "regions: a contiguous, 8-byte aligned CUDA tensor of 40-byte integer rows"
+        assert getattr(texels, "is_cuda", False) and texels.is_contiguous(), "texels: a contiguous CUDA tensor"
+        n = x.shape[0] if n is None else n
+        assert 0 <= n <= x.shape[0], "n: at most the regions' row count"
+        nbytes = texels.numel() * texels.element_size()
+        self._call("write_texture_regions_device", C.c_void_p(x.data_ptr()), C.c_uint32(n), C.c_void_p(texels.data_ptr() if nbytes else None),
+                   C.c_uint64(nbytes))
+
+    def readback_texels(self, skybox: bool, byte_offset: int, nbytes: int) -> np.ndarray:
+        """nbytes of the table's blob (skybox False) or the skybox's, from byte_offset, as uint8.  Blocking."""
+        out = np.zeros(max(nbytes, 1), dtype=np.uint8)
+        self._call("readback_texels", C.c_int(1 if skybox else 0), C.c_uint64(byte_offset), _ptr(out), C.c_uint64(nbytes))
+        return out[:nbytes]
 
     def set_directional_lights(self, data: bytes, atlas_w: int, atlas_h: int):
         self._call("set_directional_lights", C.c_char_p(data), C.c_uint64(len(data)), C.c_uint32(atlas_w), C.c_uint32(atlas_h))

@@ -137,6 +137,9 @@ struct r3_ctx {
     r3_material* d_materials = nullptr; uint32_t n_materials = 0, materials_cap = 0;
     bool has_skybox = false; r3_texture_desc sky_desc{}; uint8_t* d_sky_texels = nullptr; uint64_t sky_cap = 0;   // cube map of the skybox routine
     r3_texture_desc* d_tex_descs = nullptr; uint32_t n_textures = 0, tex_descs_cap = 0; uint8_t* d_texels = nullptr; uint64_t texels_cap = 0, texel_bytes = 0;
+    // host copy of the table's n_textures descriptors (r3_set_textures, r3_update_textures): r3_write_texture_regions checks against it
+    std::vector<r3_texture_desc> tex_desc_host;
+    void* d_texw_plan = nullptr; uint64_t texw_plan_cap = 0;   // r3_texture_write.cu: per-region copy plans + unit scan, grow-only
     r3_directional_light* d_dir = nullptr; uint32_t n_dir = 0, dir_cap = 0;
     // shadow cameras evaluated on the device (r3_lights.cu): the sources of r3_set_directional_light_sources and one camera header per
     // light (view, view_proj, frustum written by the evaluation), both sized R3_MAX_SHADOWS; host copies of the placements

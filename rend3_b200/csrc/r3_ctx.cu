@@ -114,6 +114,7 @@ R3_EXPORT int r3_ctx_destroy(r3_ctx* c) {
     for (float* p : c->d_hiz) cudaFree(p);
     cudaFree(c->d_hiz_ptrs); cudaFree(c->d_hiz_dims);
     cudaFree(c->d_tris[0]); cudaFree(c->d_tris[1]); cudaFree(c->d_tris[2]); cudaFree(c->d_tris[3]); cudaFree(c->d_stats); cudaFree(c->d_scratch);
+    cudaFree(c->d_texw_plan);
     cudaFree(c->d_frag_heads); cudaFree(c->d_frag_nodes);
     for (cudaEvent_t e : c->timer.pool) cudaEventDestroy(e);
     for (auto& x : c->frame_exec) if (x) cudaGraphExecDestroy(x);
@@ -506,6 +507,7 @@ R3_EXPORT int r3_set_textures(r3_ctx* c, const r3_texture_desc* descs, uint32_t 
     R3_CUDA(c, r3_stream_sync(c));
     c->n_textures = n;
     c->texel_bytes = nbytes;
+    c->tex_desc_host.assign(descs, descs + n);
     return R3_OK;
 }
 
@@ -579,6 +581,8 @@ R3_EXPORT int r3_update_textures(r3_ctx* c, uint32_t first, const r3_texture_des
         R3_CUDA(c, cudaMemcpyAsync(c->d_tex_descs + first, descs, (size_t)n * sizeof(r3_texture_desc), cudaMemcpyHostToDevice, c->stream));
         R3_CUDA(c, r3_stream_sync(c));
         if (need > c->n_textures) c->n_textures = (uint32_t)need;
+        c->tex_desc_host.resize(c->n_textures);
+        std::copy(descs, descs + n, c->tex_desc_host.begin() + first);
     }
     return R3_OK;
 }

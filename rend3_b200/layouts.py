@@ -178,11 +178,46 @@ MATERIAL_DTYPE = _dt(
 )
 
 TEXTURE_DESC_DTYPE = _dt([("width", u4, 0), ("height", u4, 4), ("mip_count", u4, 8), ("format", u4, 12), ("byte_offset", np.dtype("<u8"), 16)], 32)
+
 TEXFMT_RGBA8_UNORM, TEXFMT_RGBA8_UNORM_SRGB, TEXFMT_RGBA32_FLOAT, TEXFMT_R8_UNORM, TEXFMT_RG8_UNORM = 0, 1, 2, 3, 4
 (TEXFMT_BC1_RGBA_UNORM, TEXFMT_BC1_RGBA_UNORM_SRGB, TEXFMT_BC2_RGBA_UNORM, TEXFMT_BC2_RGBA_UNORM_SRGB, TEXFMT_BC3_RGBA_UNORM, TEXFMT_BC3_RGBA_UNORM_SRGB,
  TEXFMT_BC4_R_UNORM, TEXFMT_BC4_R_SNORM, TEXFMT_BC5_RG_UNORM, TEXFMT_BC5_RG_SNORM, TEXFMT_BC7_RGBA_UNORM, TEXFMT_BC7_RGBA_UNORM_SRGB) = range(5, 17)   # 4x4 blocks, rule R11 (include/r3_layouts.h)
 (TEXFMT_R8_SNORM, TEXFMT_RG8_SNORM, TEXFMT_RGBA8_SNORM, TEXFMT_BGRA8_UNORM, TEXFMT_BGRA8_UNORM_SRGB, TEXFMT_RGB10A2_UNORM, TEXFMT_R16_FLOAT, TEXFMT_RG16_FLOAT,
  TEXFMT_RGBA16_FLOAT, TEXFMT_R32_FLOAT, TEXFMT_RG32_FLOAT, TEXFMT_R16_UNORM, TEXFMT_RG16_UNORM, TEXFMT_RGBA16_UNORM) = range(17, 31)
+TEXFMT_COUNT = 31
+
+
+def texfmt_is_block(f: int) -> bool:
+    """R3_TEXFMT_IS_BLOCK"""
+    return TEXFMT_BC1_RGBA_UNORM <= f <= TEXFMT_BC7_RGBA_UNORM_SRGB
+
+
+def texfmt_element_bytes(f: int) -> int:
+    """Bytes of one stored element: the 4x4 block of a BC format (R3_TEXFMT_BLOCK_BYTES), else the texel (R3_TEXFMT_BPP)."""
+    if texfmt_is_block(f):
+        return 8 if f <= TEXFMT_BC1_RGBA_UNORM_SRGB or f in (TEXFMT_BC4_R_UNORM, TEXFMT_BC4_R_SNORM) else 16
+    if f == TEXFMT_RGBA32_FLOAT:
+        return 16
+    if f in (TEXFMT_RGBA16_FLOAT, TEXFMT_RG32_FLOAT, TEXFMT_RGBA16_UNORM):
+        return 8
+    if f in (TEXFMT_RG8_UNORM, TEXFMT_RG8_SNORM, TEXFMT_R16_FLOAT, TEXFMT_R16_UNORM):
+        return 2
+    return 1 if f in (TEXFMT_R8_UNORM, TEXFMT_R8_SNORM) else 4
+
+
+def texfmt_level_shape(f: int, width: int, height: int, level: int):
+    """(texels wide, texels high, elements per row, rows) of mip `level` of a width x height texture; a BC row is a row of blocks."""
+    w, h = max(width >> level, 1), max(height >> level, 1)
+    return (w, h, (w + 3) // 4, (h + 3) // 4) if texfmt_is_block(f) else (w, h, w, h)
+
+
+# r3_texture_region: one rectangle of texels for r3_write_texture_regions[_device]; `texture` is a table index or SKYBOX_FACE(f)
+def SKYBOX_FACE(f: int) -> int:
+    return 0x80000000 | int(f)
+
+
+TEXTURE_REGION_DTYPE = _dt([("src_offset", np.dtype("<u8"), 0), ("texture", u4, 8), ("level", u4, 12), ("x", u4, 16), ("y", u4, 20),
+                            ("width", u4, 24), ("height", u4, 28), ("src_pitch", u4, 32), ("_reserved", u4, 36)], 40)
 (TEX_ALBEDO, TEX_NORMAL, TEX_ROUGHNESS, TEX_METALLIC, TEX_REFLECTANCE, TEX_CLEAR_COAT, TEX_CLEAR_COAT_ROUGHNESS, TEX_EMISSIVE, TEX_ANISOTROPY,
  TEX_AMBIENT_OCCLUSION) = range(10)
 

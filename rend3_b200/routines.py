@@ -144,7 +144,7 @@ class BaseRenderGraph:
                      posed_skinning: bool = False, posed_objects: bool = False, device_shadow_cameras: bool = False, object_transforms=None,
                      movable_objects: bool = False, device_point_lights: bool = False, point_light_updates=None, object_presence=None,
                      material_updates=None, joint_matrices=None, mesh_deforms=None, remeshes=None, object_variants=None,
-                     directional_changes=None):
+                     directional_changes=None, texture_writes=None):
         """One frame in the node order of base.rs:135-185.  `scissor_rows` restricts rasterisation and shading
         to a band of pixel rows (the screen-tile split of the multi-GPU forward pass); `shadow_filter(i)` selects the shadow
         maps this rank renders — it then clears only their rects, the others arrive from their owners — and `after_shadows()`
@@ -197,7 +197,11 @@ class BaseRenderGraph:
         context's stream — and host arrays through r3_switch_object_variants, which waits for the stream.
         `directional_changes` = DirectionalLightChanges (DIRECTIONAL_LIGHT_CHANGE_DTYPE records) applied to the lights of
         `device_shadow_cameras` right before their shadow cameras are evaluated (DirectionalLightManager::update): a CUDA tensor through
-        r3_update_directional_light_sources_device, a host array through r3_update_directional_light_sources; both only enqueue work."""
+        r3_update_directional_light_sources_device, a host array through r3_update_directional_light_sources; both only enqueue work.
+        `texture_writes` = (regions, texels) — EvalOutput.texture_writes, or TEXTURE_REGION_DTYPE rows and texel bytes a CUDA producer
+        wrote — patches rectangles of the table's and the skybox's levels before the first pass that samples them (a texture added
+        again each frame, in rend3): CUDA tensors through r3_write_texture_regions_device — enqueue only, their producer ordered on the
+        context's stream — and host arrays through r3_write_texture_regions, which waits for the stream."""
         import os
         if frame_graph is None:
             frame_graph = os.environ.get("R3_FRAME_GRAPH", "0") not in ("", "0")
@@ -250,6 +254,12 @@ class BaseRenderGraph:
                 b.remesh_meshes(**remeshes)
         if skinning is not None:                                                  # :145 state.skinning: (skeleton records, joint matrices)
             b.skin(skinning[0], skinning[1])
+        if texture_writes is not None:                                            # textures that change, before the shadow passes
+            regions, texels = texture_writes
+            if getattr(regions, "is_cuda", False):
+                b.write_texture_regions_device(regions, texels)
+            else:
+                b.write_texture_regions(regions, texels)
         if material_updates is not None:                                          # :145 materials that change, before the shadow passes
             indices, records = material_updates
             if getattr(records, "is_cuda", False):

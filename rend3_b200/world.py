@@ -41,6 +41,11 @@ from .layouts import (
     MAT_SWIZZLED_NORMAL,
     MAT_YDOWN_NORMAL,
     TEXTURE_DESC_DTYPE,
+    TEXTURE_REGION_DTYPE,
+    SKYBOX_FACE,
+    texfmt_element_bytes,
+    texfmt_is_block,
+    texfmt_level_shape,
     TEXFMT_RGBA8_UNORM,
     TEXFMT_RGBA8_UNORM_SRGB,
     TEXFMT_RGBA32_FLOAT,
@@ -570,6 +575,10 @@ class EvalOutput:
     # the material buffer's stale indices since the previous evaluate (MaterialManager::update's use_index, material.rs:163-189), sorted
     # and distinct: what r3_update_materials scatters from material_buffer instead of r3_set_materials uploading all of it
     material_stale: np.ndarray = field(default_factory=lambda: np.zeros(0, dtype=np.uint32))
+    # the texel rectangles written since the previous evaluate (Renderer.write_texture_2d / write_skybox) as (TEXTURE_REGION_DTYPE
+    # regions, uint8 texels): what r3_write_texture_regions[_device] applies to the previous frame's blobs to give texture_texels and
+    # skybox_texels; no two regions of one level meet.  None when nothing was written
+    texture_writes: Optional[Tuple[np.ndarray, np.ndarray]] = None
 
 
 class Renderer:
@@ -585,6 +594,10 @@ class Renderer:
         self.materials: List[PbrMaterial] = []
         self.textures: List[Texture] = []
         self.skybox: Optional[List[Texture]] = None
+        # stored levels (flat uint8) of the textures and skybox faces written since they were added: they replace the generated ones
+        self.texture_levels: dict = {}
+        self.skybox_levels: Optional[List[List[np.ndarray]]] = None
+        self.texture_writes: list = []
         self.objects: List[Optional[dict]] = []
         self.free_objects: List[int] = []
         self.delayed: List[int] = []
@@ -638,6 +651,74 @@ class Renderer:
             if any(f.shape != shape or f.dtype != dtype for f in faces):
                 raise ValueError("set_skybox: the six faces must have the same shape and dtype")
         self.skybox = None if faces is None else [Texture(np.ascontiguousarray(f), srgb=srgb, mips=mips) for f in faces]
+        self.skybox_levels = None   # the new faces replace every write to the old ones
+        self.texture_writes = [w for w in self.texture_writes if not w[0] & 0x80000000]
+
+    # ---- textures that change.  rend3's textures are immutable (TextureManager::add, texture.rs:98-251): there a texture that changes is
+    # added again and its materials updated; here a rectangle of one level is patched (r3_write_texture_regions)
+    def write_texture_2d(self, handle: int, level: int, x: int, y: int, stored):
+        """Replace a rectangle of mip `level` of texture `handle` at texel (x, y) with `stored`, byte for byte.  `stored`'s two leading axes
+        are rows and columns of stored elements — texels, or 4x4 blocks for the BC formats, whose rectangle is then the blocks' texels
+        clipped to the level's edge — and its other axes and dtype hold one element's bytes in the texture's storage format.  Nothing is
+        regenerated: from the first write on the texture's levels are explicit, so generated mips no longer follow level 0.  The next
+        evaluate() carries the patched blob and the pending writes (EvalOutput.texture_writes).  ValueError for a rectangle outside the
+        level or an element size that is not the format's."""
+        t = self.textures[handle]
+        if handle not in self.texture_levels:
+            self.texture_levels[handle] = [np.ascontiguousarray(l).reshape(-1).view(np.uint8).copy() for l in t.stored_levels()]
+        self._write_level(handle, self.texture_levels[handle], t.format(), t.data.shape[1], t.data.shape[0], level, x, y, stored)
+
+    def write_skybox(self, face: int, level: int, x: int, y: int, stored):
+        """write_texture_2d for face `face` (0..5: +X -X +Y -Y +Z -Z) of the skybox: `stored` is (h, w, 4) of the faces' dtype."""
+        if self.skybox is None or not 0 <= face < 6:
+            raise ValueError("write_skybox: no skybox, or a face outside 0..5")
+        if self.skybox_levels is None:
+            self.skybox_levels = [[np.ascontiguousarray(l).reshape(-1).view(np.uint8).copy() for l in f.levels()] for f in self.skybox]
+        n = self.skybox[0].data.shape[0]
+        self._write_level(SKYBOX_FACE(face), self.skybox_levels[face], self.skybox[0].format(), n, n, level, x, y, stored)
+
+    def _write_level(self, target, levels, fmt, width, height, level, x, y, stored):
+        a = np.ascontiguousarray(stored)
+        elem = texfmt_element_bytes(fmt)
+        if not 0 <= level < len(levels) or a.ndim < 2 or a.itemsize * int(np.prod(a.shape[2:], dtype=np.int64)) != elem:
+            raise ValueError(f"write: level {level} of {len(levels)}, or elements of {a.dtype} {a.shape[2:]} for a {elem}-byte element")
+        lw, lh, cols, rows = texfmt_level_shape(fmt, width, height, level)
+        er, ec = a.shape[:2]
+        block = texfmt_is_block(fmt)
+        ex, ey = (x // 4, y // 4) if block else (x, y)
+        if x < 0 or y < 0 or er == 0 or ec == 0 or (block and (x % 4 or y % 4)) or ex + ec > cols or ey + er > rows:
+            raise ValueError(f"write: {ec} x {er} elements at texel ({x}, {y}) do not fit level {level} ({lw} x {lh})")
+        w, h = (min(4 * ec, lw - x), min(4 * er, lh - y)) if block else (ec, er)
+        raw = a.reshape(-1).view(np.uint8).reshape(er, ec * elem)
+        levels[level].reshape(rows, cols * elem)[ey:ey + er, ex * elem:(ex + ec) * elem] = raw
+        self.texture_writes.append((target, level, x, y, w, h, raw.copy(), levels, fmt, width, height))
+
+    def _texture_write_regions(self):
+        """The pending writes as (regions, texels).  Where a rectangle meets an earlier one of the same level, that level goes as one
+        whole-level region of its patched bytes, so the regions never overlap."""
+        writes, self.texture_writes = self.texture_writes, []
+        if not writes:
+            return None
+        by_level = {}
+        for wr in writes:
+            by_level.setdefault((wr[0], wr[1]), []).append(wr)
+        out = []
+        for (target, level), ws in by_level.items():
+            meet = any(a[2] < b[2] + b[4] and b[2] < a[2] + a[4] and a[3] < b[3] + b[5] and b[3] < a[3] + a[5]
+                       for i, a in enumerate(ws) for b in ws[:i])
+            if meet:
+                _, _, _, _, _, _, _, levels, fmt, width, height = ws[-1]
+                lw, lh, cols, rows = texfmt_level_shape(fmt, width, height, level)
+                ws = [(target, level, 0, 0, lw, lh, levels[level].reshape(rows, -1).copy())]
+            out += [wr[:7] for wr in ws]
+        regions = np.zeros(len(out), dtype=TEXTURE_REGION_DTYPE)
+        chunks, cursor = [], 0
+        for k, (target, level, x, y, w, h, raw) in enumerate(out):
+            regions[k] = (cursor, target, level, x, y, w, h, raw.shape[1], 0)
+            pad = (-raw.size) % 16                                    # every source starts 16-byte aligned
+            chunks += [raw.reshape(-1), np.zeros(pad, dtype=np.uint8)]
+            cursor += raw.size + pad
+        return regions, np.concatenate(chunks)
 
     def _skybox_blob(self):
         if self.skybox is None:
@@ -645,6 +726,8 @@ class Renderer:
         lv0 = self.skybox[0].levels()
         desc = np.zeros((), dtype=TEXTURE_DESC_DTYPE)
         desc["width"], desc["height"], desc["mip_count"], desc["format"], desc["byte_offset"] = lv0[0].shape[1], lv0[0].shape[0], len(lv0), self.skybox[0].format(), 0
+        if self.skybox_levels is not None:
+            return desc, np.concatenate([l for f in self.skybox_levels for l in f])
         raw = [np.ascontiguousarray(l).view(np.uint8).reshape(-1) for f in self.skybox for l in f.levels()]
         return desc, np.concatenate(raw)
 
@@ -652,7 +735,7 @@ class Renderer:
         descs = np.zeros(len(self.textures), dtype=TEXTURE_DESC_DTYPE)
         blobs, cursor = [], 0
         for i, t in enumerate(self.textures):
-            lv = t.stored_levels()
+            lv = self.texture_levels[i] if i in self.texture_levels else t.stored_levels()
             descs[i]["width"], descs[i]["height"] = t.data.shape[1], t.data.shape[0]
             descs[i]["mip_count"], descs[i]["format"], descs[i]["byte_offset"] = len(lv), t.format(), cursor
             raw = np.concatenate([np.ascontiguousarray(l).view(np.uint8).reshape(-1) for l in lv])
@@ -894,6 +977,7 @@ class Renderer:
 
         tex_descs, tex_blob = self._texture_table()
         sky_desc, sky_blob = self._skybox_blob()
+        texture_writes = self._texture_write_regions()
         return EvalOutput(
             object_buffer=self.obj_gpu.copy(),
             object_material_key=key,
@@ -916,4 +1000,5 @@ class Renderer:
             camera=self.camera,
             object_mesh_sphere=mesh_sphere,
             material_stale=material_stale,
+            texture_writes=texture_writes,
         )

@@ -37,7 +37,8 @@ def compile_tree(csrc, out):
             raise RuntimeError(f"nvcc failed on {csrc}/{src}:\n{r.stderr}")
         return src, o
     with concurrent.futures.ThreadPoolExecutor(os.cpu_count() or 4) as pool:
-        return dict(pool.map(one, entry.SOURCES))
+        # a source the other tree does not have yet (a new unit) is compiled on one side only: its kernels show as ONLY IN
+        return dict(pool.map(one, [s for s in entry.SOURCES if os.path.exists(os.path.join(csrc, s[0]))]))
 
 
 def unhash(text):
@@ -109,8 +110,8 @@ def main():
         tree = compile_tree(os.path.join(ROOT, "rend3_b200", "csrc"), dirs["tree_obj"])
         same = differ = 0
         for src, _ in entry.SOURCES:
-            a, b = kernels(base[src]), kernels(tree[src])
-            ra, rb = resources(base[src]), resources(tree[src])
+            a, b = (kernels(base[src]) if src in base else {}), kernels(tree[src])
+            ra, rb = (resources(base[src]) if src in base else {}), resources(tree[src])
             for name in sorted(set(a) | set(b)):
                 label = f"{src}: {demangle((a.get(name) or b.get(name))[0])[:140]}"
                 if name not in a or name not in b:
