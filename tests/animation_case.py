@@ -194,3 +194,38 @@ def crowd(n_instances=4096, seed=0, n_keys=60):
     frames = [(0, float(rng.uniform(0, duration)), {0: [(130 * i, 65), (130 * i + 65, 65)]}) for i in range(n_instances)]
     jobs, targets = data.pose_jobs(frames)
     return data, jobs, targets, np.zeros((130 * n_instances, 16), dtype=f32)
+
+
+def _posed_cube_world():
+    """The smoke scene whose cube mesh is skinned in place: its position range is overwritten by r3_skin_posed from a copy appended to
+    the mesh buffer, so every rendered cube shows the pose."""
+    from rend3_b200.layouts import ATTR_ABSENT, SKINNING_INPUT_DTYPE
+    from rend3_b200.scenes import cube_field_scene
+
+    ev = cube_field_scene(n_objects=300, seed=7, resolution=(256, 144))
+    pos_off, nrm_off = (int(x) for x in ev.object_buffer["attr_offset"][0][:2])
+    nv = (nrm_off - pos_off) // 12
+    assert nv > 0
+    rng = np.random.default_rng(11)
+    words = ev.mesh_buffer
+    base = len(words)
+    idx = rng.integers(0, 4, (nv, 4)).astype(np.uint16)
+    w = rng.random((nv, 4)).astype(f32)
+    w = (w / w.sum(axis=1, keepdims=True)).astype(f32)
+    extra = [words[pos_off // 4: pos_off // 4 + 3 * nv], idx.view(np.uint32).reshape(-1), w.view(np.uint32).reshape(-1)]
+    rec = np.zeros(1, dtype=SKINNING_INPUT_DTYPE)
+    rec["base_position_offset"] = 4 * base
+    rec["joint_indices_offset"] = 4 * (base + 3 * nv)
+    rec["joint_weight_offset"] = 4 * (base + 5 * nv)
+    rec["updated_position_offset"] = pos_off
+    for f in ("base_normal_offset", "base_tangent_offset", "updated_normal_offset", "updated_tangent_offset"):
+        rec[f] = ATTR_ABSENT
+    rec["vertex_count"] = nv
+    ev.mesh_buffer = np.concatenate([words] + extra)
+    # a small 4-joint chain whose poses stay near the bind pose
+    nodes = [Node(None)] + [Node(k, (0.0, 0.1, 0.0)) for k in range(3)]
+    tracks = {n: NodeChannels(Track(np.array([0, 1, 2], f32), np.array([[0, 0, 0], [0.1, 0, 0], [0, 0.1, 0]], f32)),
+                              Track(np.array([0, 2], f32), np.array([[0, 0, 0, 1], [0, 0.2, 0, 0.98]], f32) / np.float32(np.linalg.norm([0, 0.2, 0, 0.98]))))
+              for n in range(4)}
+    data = AnimationData(nodes, [Skin([0, 1, 2, 3], np.tile(glam.identity().reshape(16), (4, 1)))], [Animation(tracks, 2.0)])
+    return ev, rec, data

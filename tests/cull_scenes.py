@@ -8,6 +8,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
+import cull_reference as ref
 import raster_scenes
 from rend3_b200 import glam
 from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE
@@ -475,3 +476,251 @@ def high_vertex_id_scene():
     objects["index_count"] = 3
     batches, regions = build_tables([1, 1, 1], atomic=[1, 1, 0], keys=[0, 0, 2])
     return Scene(objects, mesh, batches, regions)
+
+
+def hiz_sizes():
+    return [(1920, 1080), (3840, 2160), (40, 24), (36, 36), (34, 34), (480, 270), (481, 270), (1, 777), (777, 1), (2, 2048), (4096, 2),
+            (1, 1)]
+
+
+HIZ_CASES = [(w, h, 1) for w, h in hiz_sizes()] + [(1920, 1080, 4), (481, 270, 4)]
+
+
+FUSED = {(1920, 1080): 3, (3840, 2160): 3, (40, 24): 3, (36, 36): 2, (34, 34): 1, (480, 270): 1, (481, 270): 0}
+
+
+def hiz_content(w, h, seed):
+    """Occluders for the hi-Z size tests: a far background over all but the top-left quarter and the last row and column (the uncovered
+    pixels read 0), random triangles in front of it, and one-pixel quads along the whole last row and column at depths below the
+    background's.  With odd sizes the unique minimum of a footprint then sits in its extra row or column.  Reverse-Z: the larger depth
+    is the nearer, and the pyramid keeps the smaller.  Returns (triangles in pixels, depth per triangle)."""
+    rng = np.random.default_rng(seed)
+    tris, z = [], []
+    x0, y0 = w // 4, h // 4
+    tris += [((x0, y0), (w - 1, y0), (w - 1, h - 1)), ((x0, y0), (w - 1, h - 1), (x0, h - 1))]
+    z += [0.45, 0.45]
+    for _ in range(40):
+        c = rng.uniform(0, 1, 2) * (w - 1, h - 1)
+        t = np.clip(np.round((c + rng.uniform(-0.3, 0.3, (3, 2)) * (w, h)) * 4) / 4, 0, (w - 1, h - 1))
+        tris.append(tuple(map(tuple, t)))
+        z.append(float(rng.uniform(0.5, 0.9)))
+    for x in range(w):
+        tris += [((x, h - 1), (x + 1, h - 1), (x + 1, h)), ((x, h - 1), (x + 1, h), (x, h))]
+        z += [0.05 + 0.35 * rng.random()] * 2
+    for y in range(h - 1):
+        tris += [((w - 1, y), (w, y), (w, y + 1)), ((w - 1, y), (w, y + 1), (w - 1, y + 1))]
+        z += [0.05 + 0.35 * rng.random()] * 2
+    return tris, np.array(z, F32)
+
+
+def render_hiz(backend, w, h, samples, seed=0):
+    tris, z = hiz_content(w, h, seed)
+    r = raster_scenes.build(backend, w, h, tris, z)
+    raster_scenes.draw(r, w, h, samples)
+    launches = backend.launch_count()
+    backend.hiz_build()
+    launches = backend.launch_count() - launches
+    levels = read_pyramid(backend, len(ref.hiz_dims(w, h)))
+    # level 0 is the min over the samples (resolve_depth_min.wgsl:18-27), which is what the depth resolve keeps as well
+    depth = backend.readback_depth()
+    assert np.array_equal(levels[0].view(np.uint32), depth.view(np.uint32)), f"{w}x{h}x{samples}: level 0 is not the resolved depth"
+    backend.last_hiz_launches = launches
+    return levels
+
+
+def assert_pyramid(levels, w, h, what):
+    want = ref.hiz_pyramid(levels[0])
+    assert [l.shape[::-1] for l in levels] == ref.hiz_dims(w, h), f"{what}: level sizes"
+    for m in range(1, len(levels)):
+        bad = levels[m].view(np.uint32) != want[m].view(np.uint32)
+        assert not bad.any(), f"{what}: level {m} differs from hi_z.wgsl at {np.count_nonzero(bad)} texels, first {np.argwhere(bad)[0]}"
+
+
+def exact_runs(backend, samples):
+    """The exact decision scene under every flag combination and a shadow camera: yields (what, got, want, header)."""
+    pyramid = draw_occluders(backend, samples)
+    tris, z, labels = exact_decision_triangles()
+    s = triangle_scene(tris, z)
+    upload(backend, s)
+    n = len(s.objects)
+    for flags in EXACT_FLAGS:
+        for cam in (CAMERA_VIEWPORT, 0):
+            hdr = ortho_header(256, 256, flags, n, shadow_index=cam)
+            got = run_cull(backend, s, hdr, cam)
+            want = reference_for(got, s, hdr, pyramid if cam == CAMERA_VIEWPORT else None)
+            yield f"flags {flags} camera {cam:#x}", s, got, want, labels, pyramid
+
+
+def check_exact(what, s, got, want, labels):
+    # the f32 path is exact here: float64 decides every triangle the same way
+    diff = np.nonzero(want["pass32"] != want["pass64"])[0]
+    assert not len(diff), f"{what}: f32 and float64 differ on {[labels[i] for i in diff[:5]]}"
+    assert_matches(got, want, s, what)
+
+
+def perspective_runs(backend):
+    tris, labels, proj = perspective_scene()
+    s = world_triangle_scene(tris)
+    backend.set_render_target(64, 64, 1, (0, 0, 0, 0))
+    backend.forward_begin()
+    backend.hiz_build()                                   # an empty depth buffer: a uniform pyramid of 0.0
+    pyramid = read_pyramid(backend, len(ref.hiz_dims(64, 64)))
+    upload(backend, s)
+    for flags in (0, PCU_POSITIVE_AREA_VISIBLE, PCU_MULTISAMPLED):
+        hdr = ortho_header(64, 64, flags, len(s.objects), proj=proj)
+        got = run_cull(backend, s, hdr)
+        yield f"perspective flags {flags}", s, got, reference_for(got, s, hdr, pyramid), labels
+
+
+def check_perspective(what, s, got, want, labels, margin_floor=1.0):
+    """Decisions equal the f32 reference everywhere; float64 is checked where the margin allows.  Returns the excluded labels."""
+    assert_matches(got, want, s, what)
+    m = ref.decision_margin(want["q64"], want["stage64"], want["flags"], want["viewport"])
+    near = m <= margin_floor
+    bad = (want["pass32"] != want["pass64"]) & ~near
+    assert not bad.any(), f"{what}: f32 and float64 differ beyond the margin on {[labels[i] for i in np.nonzero(bad)[0][:5]]}"
+    unit = [i for i, l in enumerate(labels) if l == "unit w"]
+    assert (want["q64"]["clip"][0][unit, 3] == 1).all(), "the unit-w triangles must have w == 1.0 exactly"
+    return sorted(labels[i] for i in np.nonzero(near)[0])
+
+
+def structural_runs(backend):
+    """Yields (what, scene, got, want, census): the ragged scene over two frames (NO_PREVIOUS, then in range / past the partition),
+    superblock-boundary scenes of 4 x 32768 + {-256, 0, 256} invocations, the mesh-end scene in a fresh context and again after a
+    larger mesh left stale words behind the smaller one."""
+    s = ragged_scene()
+    upload(backend, s)
+    n = len(s.objects)
+    hdr = ortho_header(256, 256, 0, n)
+    got = run_cull(backend, s, hdr)
+    yield "ragged frame 0", s, got, reference_for(got, s, hdr, None)
+    first = {}
+    for b in s.batches:
+        for info in b["object_culling_information"][:int(b["total_objects"])]:
+            first[int(info["object_id"])] = int(b["batch_base_invocation"]) + int(info["invocation_start"])
+    total = total_invocations(s.batches)
+    prev = [NO_PREVIOUS if i % 3 == 0 else (first[i] if i % 3 == 1 else total + 4096 * 32 + i) for i in range(n)]
+    counts = [int(c) // 3 for c in s.objects["index_count"]]
+    atomic = [0 if i in (0, 1, 254, 255) else 1 for i in range(n)]
+    keys = [2 if i in (0, 1, 254, 255) else 0 for i in range(n)]
+    b2, r2 = build_tables(counts, atomic=atomic, keys=keys, prev=prev)
+    s2 = Scene(s.objects, s.mesh, b2, r2)
+    got = run_cull(backend, s2, hdr)
+    yield "ragged frame 1", s2, got, reference_for(got, s2, hdr, None)
+    for delta in (0, -256, 256):
+        s = superblock_scene(delta)
+        upload(backend, s)
+        hdr = ortho_header(256, 256, PCU_POSITIVE_AREA_VISIBLE, len(s.objects))
+        got = run_cull(backend, s, hdr)
+        yield f"superblock {delta:+d}", s, got, reference_for(got, s, hdr, None)
+
+
+def mesh_end_runs(make_backend):
+    """The mesh-end scene in a fresh context, and again after a larger mesh buffer whose words past the smaller one's end are stale
+    (the allocation is kept, so the bulk copy of the index runs reads them).  Closes the contexts it makes."""
+    s, end, stale = mesh_end_scene()
+    for with_stale in (False, True):
+        b = make_backend()
+        try:
+            if with_stale:
+                b.set_mesh_buffer(stale)
+            upload(b, s)
+            hdr = ortho_header(256, 256, PCU_MULTISAMPLED, len(s.objects))
+            got = run_cull(b, s, hdr)
+            yield f"mesh end stale={with_stale}", s, got, reference_for(got, s, hdr, None)
+        finally:
+            b.close()
+
+
+def stale_triangles(s, stale, got, hdr):
+    """The decisions of object 2's triangle 37 and object 3's first triangle when robust access is honoured, and when the stale words
+    past mesh_words were read instead."""
+    robust = reference_for(got, s, hdr, None)
+    stale_view = Scene(s.objects, stale, s.batches, s.regions)
+    wrong = reference_for(got, stale_view, hdr, None)
+    picks = []
+    for b in s.batches:
+        for info in b["object_culling_information"][:int(b["total_objects"])]:
+            g = int(b["batch_base_invocation"]) + int(info["invocation_start"])
+            if int(info["object_id"]) == 2:
+                picks.append(g + 37)
+            if int(info["object_id"]) == 3:
+                picks.append(g)
+    return robust["stage"][picks], wrong["stage"][picks]
+
+
+def pingpong_runs(backend):
+    """The three frames of pingpong_frames, each compared as it comes (no second cull): yields (what, scene, got, want)."""
+    s, frames = pingpong_frames()
+    upload(backend, s)
+    hdr = ortho_header(256, 256, 0, len(s.objects))
+    for k, (b, r) in enumerate(frames):
+        fs = Scene(s.objects, s.mesh, b, r)
+        got = run_cull(backend, fs, hdr, settle=False)
+        yield f"ping-pong frame {k}", fs, got, reference_for(got, fs, hdr, None)
+
+
+def pingpong_census(frames):
+    """The index buffer is reallocated for frame 1 (next_pow2 of its elements grows) and frame 1 and 2 read previous bits in range."""
+    inv = [total_invocations(b) for b, _ in frames]
+    pow2 = lambda v: 1 << (int(v) - 1).bit_length()
+    assert inv[0] < inv[1] > inv[2] and pow2(3 * inv[1]) > pow2(3 * inv[0])
+    for b, _ in frames[1:]:
+        prev = [int(i["previous_global_invocation"]) for bb in b for i in bb["object_culling_information"][:int(bb["total_objects"])]]
+        assert sum(p != NO_PREVIOUS for p in prev) >= 20
+
+
+def high_id_run(backend):
+    s = high_vertex_id_scene()
+    upload(backend, s)
+    hdr = ortho_header(256, 256, PCU_MULTISAMPLED, len(s.objects))
+    got = run_cull(backend, s, hdr)
+    return s, got, reference_for(got, s, hdr, None), hdr
+
+
+def check_high_id(s, got, want, hdr, what):
+    assert_matches(got, want, s, what)
+    assert want["pass32"].all(), f"{what}: the triangles behind ids >= 2^24 face the camera"
+    masked = s.mesh.copy()
+    masked[64:70] &= 0xFFFFFF
+    low = reference_for(got, Scene(s.objects, masked, s.batches, s.regions), hdr, None)
+    assert not low["pass32"].any(), "fetching the positions through the masked ids must decide differently"
+    assert want["idx_pred"][:6].tolist() == [0, 1, 2, (1 << 24) | 0, (1 << 24) | 1, (1 << 24) | 2]
+    assert want["idx_resid"][3 * 512:3 * 512 + 3].tolist() == [(2 << 24) | 3, (2 << 24) | 4, (2 << 24) | 5]
+
+
+def big_census(s, ends):
+    """More than two passes of the persistent grid (4224 workgroups at 4 CTAs / SM, 5280 at 5), and the end-of-buffer objects lie in
+    workgroups past the first pass, on both sides of the staging guard."""
+    total = total_invocations(s.batches)
+    assert total // 256 > 2 * WARP_STRIDE
+    end = len(s.mesh)
+    wgs = {}
+    for b in s.batches:
+        for info in b["object_culling_information"][:int(b["total_objects"])]:
+            wgs[int(info["object_id"])] = (int(b["batch_base_invocation"]) + int(info["invocation_start"])) // 256
+    assert min(wgs[o] for o in ends) > 132 * 5 * 8
+    runs = [(int(s.objects[o]["first_index"]) & ~3) + 100 for o in ends]
+    assert (end + 4) in runs and any(r > end + 4 for r in runs) and any(r < end + 4 for r in runs)
+
+
+def batched_frame_runs(backend):
+    """One whole frame of a small cube field through BaseRenderGraph (the batch tables from batch_objects, host- or device-built),
+    then each camera's cull compared with the reference fed the tables, MVPs and pyramid that cull used."""
+    from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings, per_camera_header
+    from rend3_b200.scenes import cube_field_scene
+    res = (480, 270)
+    ev = cube_field_scene(n_objects=1500, seed=5, resolution=res, n_point_lights=0, shadow_resolution=256, pull_back=12.0, extent=30.0)
+    BaseRenderGraph(backend).add_to_graph(ev, res, 1, BaseRenderGraphSettings())
+    pyramid = read_pyramid(backend, len(ref.hiz_dims(*res)))
+    n = len(ev.object_buffer)
+    cams = [(CAMERA_VIEWPORT, per_camera_header(ev.camera, CAMERA_VIEWPORT, res, 1, n), pyramid)]
+    cams += [(i, per_camera_header(sh.camera, i, (sh.size, sh.size), 1, n), None) for i, sh in enumerate(ev.shadows)]
+    for cam, hdr, pyr in cams:
+        batches, regions = backend.readback_batches(cam)
+        s = Scene(ev.object_buffer, np.asarray(ev.mesh_buffer, np.uint32), batches, regions)
+        got = dict(words=backend.readback_culling_results(cam, 0), prev=backend.readback_culling_results(cam, 1),
+                   dc_pred=backend.readback_draw_calls(cam, 0), dc_resid=backend.readback_draw_calls(cam, 1),
+                   idx_pred=backend.readback_indices(cam, 0), idx_resid=backend.readback_indices(cam, 1),
+                   mvps=backend.readback_object_matrices(cam, 0, n)["model_view_proj"].reshape(n, 16))
+        yield f"frame camera {cam:#x}", s, got, reference_for(got, s, hdr, pyr)

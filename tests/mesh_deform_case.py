@@ -191,3 +191,23 @@ def upload(b, ev: EvalOutput):
     b.set_object_sort_info(ev.object_material_key, flags.astype(np.uint8), np.ascontiguousarray(ev.object_location, dtype=f32))
     b.set_object_mesh_spheres(ev.object_mesh_sphere)
     b.set_mesh_buffer(ev.mesh_buffer)
+
+
+def bits(a):
+    return np.ascontiguousarray(a, dtype=f32).view(np.uint32)
+
+
+def canon(a):
+    """float32 bits with every NaN as 0x7FC00000: the bits of a NaN that arithmetic makes are not part of R15 (x86 and the GPU make
+    different default NaNs); copied values keep theirs and are compared as they are"""
+    a = np.array(a, dtype=f32)
+    a[np.isnan(a)] = np.float32(np.nan)
+    return a.view(np.uint32)
+
+
+def canon_records(r):
+    out = np.frombuffer(bytearray(np.ascontiguousarray(r).tobytes()), dtype=r.dtype)
+    for f in ("transform", "sphere_center", "sphere_radius"):
+        v = out[f]
+        v[np.isnan(v)] = np.float32(np.nan)
+    return out.tobytes()

@@ -91,3 +91,16 @@ def single_node(channels=None, translation=(1.0, 2.0, 3.0), rotation=(0.0, 0.0, 
 
 def key_track(times, values):
     return Track(np.array(times, f32), np.array(values, f32))
+
+
+def sort_info(n):
+    return np.zeros(n, np.uint64), np.ones(n, np.uint8)
+
+
+def run(b, data, jobs, targets, records, loc):
+    b.set_objects(records)
+    b.set_object_sort_info(*sort_info(len(records)), loc)
+    data.upload(b)
+    b.set_object_pose_jobs(jobs, targets)
+    b.pose_objects()
+    return b.readback_objects(0, len(records))

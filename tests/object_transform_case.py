@@ -5,6 +5,7 @@ element-wise ufuncs never contract — in the order of tests/object_anim_referen
 bit; so must the oracle and the CUDA kernel."""
 import numpy as np
 
+from harness import to_device
 from rend3_b200.scenes import object_cloud_records, random_unit_quaternions, trs_matrices
 
 f32 = np.float32
@@ -106,3 +107,13 @@ def edge_matrices():
     add("overflowing length squared", m)
     names, mats, spheres = zip(*cases)
     return np.stack(mats), np.stack(spheres), list(names)
+
+
+def apply(b, form, mats, slots):
+    """One move through the host or the device form; returns what must stay alive until the stream has drained."""
+    if form == "host":
+        b.set_object_transforms(mats, slots)
+        return None
+    keep = (to_device(b, mats.reshape(-1, 16)), None if slots is None else to_device(b, np.asarray(slots, dtype=np.uint32).view(np.int32)))
+    b.set_object_transforms_device(keep[0], keep[1])
+    return keep

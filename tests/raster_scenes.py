@@ -15,6 +15,8 @@ from rend3_b200.world import CUTOUT, LEFT, OPAQUE, Camera, DirectionalLight, Mes
 
 CLEAR = (0.1, 0.2, 0.3, 1.0)
 COLOUR = (0.7, 0.2, 0.9, 0.25)   # unlit; its alpha only matters for the blend routine
+# a quad twice across the target in both directions would not be clipped; this one reaches 400x past the guard band
+GUARD_QUAD = [((-1.0e5, -1.0e5), (1.0e5, -1.0e5), (1.0e5, 1.0e5)), ((-1.0e5, -1.0e5), (1.0e5, 1.0e5), (-1.0e5, 1.0e5))]
 
 
 def ortho_camera(width, height):

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from rend3_b200.layouts import CAMERA_HEADER_DTYPE, DIRECTIONAL_LIGHT_DTYPE, PCU_POSITIVE_AREA_VISIBLE
+from rend3_b200.layouts import CAMERA_HEADER_DTYPE, DIRECTIONAL_LIGHT_DTYPE, LIGHT_SOURCE_DTYPE, PCU_POSITIVE_AREA_VISIBLE
 
 f32 = np.float32
 ONE, ZERO, HALF = f32(1.0), f32(0.0), f32(0.5)
@@ -134,3 +134,11 @@ def evaluate(sources: np.ndarray, atlas_w: int, atlas_h: int, location, left_han
             lights[i]["atlas_offset"] = (f32(int(s["offset"][0])) / w, f32(int(s["offset"][1])) / h)
             lights[i]["atlas_size"] = (f32(int(s["size"])) / w, f32(int(s["size"])) / h)
     return heads, lights
+
+
+def sources(rows):
+    """rows: (direction, distance, resolution); placements packed along the atlas' first row, 64 texels each."""
+    s = np.zeros(len(rows), dtype=LIGHT_SOURCE_DTYPE)
+    for i, (d, dist, res) in enumerate(rows):
+        s[i] = ((1.0, 0.9, 0.8), 1.0 + 0.5 * i, d, dist, res, (64 * i, 0), 64)
+    return s

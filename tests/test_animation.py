@@ -355,41 +355,6 @@ def test_gpu_skin_posed_equals_skin_of_the_posed_matrices(cuda_backend):
     assert not np.array_equal(mesh_c, words)
 
 
-def _posed_cube_world():
-    """The smoke scene whose cube mesh is skinned in place: its position range is overwritten by r3_skin_posed from a copy appended to
-    the mesh buffer, so every rendered cube shows the pose."""
-    from rend3_b200.layouts import ATTR_ABSENT
-    from rend3_b200.scenes import cube_field_scene
-
-    ev = cube_field_scene(n_objects=300, seed=7, resolution=(256, 144))
-    pos_off, nrm_off = (int(x) for x in ev.object_buffer["attr_offset"][0][:2])
-    nv = (nrm_off - pos_off) // 12
-    assert nv > 0
-    rng = np.random.default_rng(11)
-    words = ev.mesh_buffer
-    base = len(words)
-    idx = rng.integers(0, 4, (nv, 4)).astype(np.uint16)
-    w = rng.random((nv, 4)).astype(f32)
-    w = (w / w.sum(axis=1, keepdims=True)).astype(f32)
-    extra = [words[pos_off // 4: pos_off // 4 + 3 * nv], idx.view(np.uint32).reshape(-1), w.view(np.uint32).reshape(-1)]
-    rec = np.zeros(1, dtype=SKINNING_INPUT_DTYPE)
-    rec["base_position_offset"] = 4 * base
-    rec["joint_indices_offset"] = 4 * (base + 3 * nv)
-    rec["joint_weight_offset"] = 4 * (base + 5 * nv)
-    rec["updated_position_offset"] = pos_off
-    for f in ("base_normal_offset", "base_tangent_offset", "updated_normal_offset", "updated_tangent_offset"):
-        rec[f] = ATTR_ABSENT
-    rec["vertex_count"] = nv
-    ev.mesh_buffer = np.concatenate([words] + extra)
-    # a small 4-joint chain whose poses stay near the bind pose
-    nodes = [Node(None)] + [Node(k, (0.0, 0.1, 0.0)) for k in range(3)]
-    tracks = {n: NodeChannels(Track(np.array([0, 1, 2], f32), np.array([[0, 0, 0], [0.1, 0, 0], [0, 0.1, 0]], f32)),
-                              Track(np.array([0, 2], f32), np.array([[0, 0, 0, 1], [0, 0.2, 0, 0.98]], f32) / np.float32(np.linalg.norm([0, 0.2, 0, 0.98]))))
-              for n in range(4)}
-    data = AnimationData(nodes, [Skin([0, 1, 2, 3], np.tile(glam.identity().reshape(16), (4, 1)))], [Animation(tracks, 2.0)])
-    return ev, rec, data
-
-
 @pytest.mark.gpu
 def test_gpu_posed_frames_stay_one_graph(cuda_backend):
     """Six frames through add_to_graph(posed_skinning=True) with the frame graph on and the time changing per frame: no early flush,
@@ -398,7 +363,7 @@ def test_gpu_posed_frames_stay_one_graph(cuda_backend):
     from rend3_b200.backend import load_cuda_backend
     from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings
 
-    ev, rec, data = _posed_cube_world()
+    ev, rec, data = cases._posed_cube_world()
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
     graph_b, eager_b, orc = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True), load_anim_oracle_backend()
     runs = [(graph_b, True), (eager_b, False), (orc, False)]

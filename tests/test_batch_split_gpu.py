@@ -12,7 +12,7 @@ from rend3_b200.scenes import cloud_camera, cube_field_scene, object_cloud_recor
 
 from batch_split_cases import CASES, assert_same_tables, expected_tables, load
 from oracle import load_oracle_backend
-from test_gpu_parity import compare_frame_state
+from harness import compare_frame_state
 
 pytestmark = pytest.mark.gpu
 LIMITS = [0, 1, 2, 3, 255, 256, 65535]

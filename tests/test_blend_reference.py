@@ -406,11 +406,9 @@ def test_alpha_invariants(samples):
 def test_clipped_transparent_quad(cuda, samples):
     """A blended quad reaching 400x past the guard band: every sample is blended exactly once although its clipped sub-triangles
     share one record."""
-    from test_raster_paths import GUARD_QUAD
-
-    r = rscenes.build(cuda, 256, 256, GUARD_QUAD, [0.5, 0.5], transparency=BLEND)
+    r = rscenes.build(cuda, 256, 256, rscenes.GUARD_QUAD, [0.5, 0.5], transparency=BLEND)
     orc = load_oracle_backend()
-    ro = rscenes.build(orc, 256, 256, GUARD_QUAD, [0.5, 0.5], transparency=BLEND)
+    ro = rscenes.build(orc, 256, 256, rscenes.GUARD_QUAD, [0.5, 0.5], transparency=BLEND)
     for frame in range(2):
         rscenes.draw(r, 256, 256, samples)
         rscenes.draw(ro, 256, 256, samples)

@@ -7,10 +7,10 @@ sphere_center := translation.  Compared with the oracle word for word: the visib
 import numpy as np
 import pytest
 
+from harness import assert_same_bake
 from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE, CB_CULL, load_cuda_backend
 from rend3_b200.routines import per_camera_header
 from rend3_b200.scenes import cloud_camera, object_cloud_records
-from test_cull_bake_row3 import assert_same_bake
 
 from oracle import load_oracle_backend
 
@@ -172,7 +172,7 @@ def test_off_centre_slots_match_oracle(cuda):
 def test_shadow_camera_off_centre_slots_match_oracle(cuda):
     """The device-camera instantiation (r3_shadow_uniform_upload after r3_evaluate_shadow_cameras)."""
     from oracle.lights import load_lights_oracle_backend
-    from test_shadow_cameras import sources
+    from shadow_camera_reference import sources
 
     src = sources([((-1.0, -4.0, 2.0), 40.0, 512)])
     loc = np.array([1.5, 2.0, -3.0], dtype=f32)
@@ -249,7 +249,6 @@ def test_set_object_transforms_moves_between_paths(cuda, form):
     """r3_set_object_transforms (host and device memory, dense and sparse): mesh spheres centred at the origin give centred world spheres,
     off-centre ones do not; slots cross between the two paths both ways over three steps."""
     import object_transform_case as cases
-    from test_object_transforms import apply
 
     from oracle.objtransforms import load_objtransforms_oracle_backend
 
@@ -280,7 +279,7 @@ def test_set_object_transforms_moves_between_paths(cuda, form):
             for b in (cuda, orc):
                 b.set_object_mesh_spheres(ms[slots], slots)
         cur_r, cur_l = cases.moved_records(cur_r, cur_l, ms, mats, slots)
-        keep.append(apply(cuda, form, mats, slots))
+        keep.append(cases.apply(cuda, form, mats, slots))
         orc.set_object_transforms(mats, slots)
         for b in (cuda, orc):
             upload(b, CAMERA_VIEWPORT, header, n)
@@ -303,14 +302,13 @@ def test_animation_posing_moves_between_paths(cuda):
     out with off-centre world spheres (the nodes' mesh spheres are off the origin); the cull + bake after the pose equals the oracle's
     on the same records, and some posed slots would flip with their centre taken from the translation."""
     import object_animation_case as anim_cases
-    from test_object_animation import run
 
     data, jobs, targets, records, loc = anim_cases.case(seed=4, instances=64)
     n = len(records)
     records = records.copy()
     records["sphere_center"] = records["transform"][:, TRANSLATION]
     header = per_camera_header(cloud_camera(pull_back=1.0), CAMERA_VIEWPORT, (640, 360), 1, n)   # side planes cut the crowd
-    got_r, _ = run(cuda, data, jobs, targets, records, loc)
+    got_r, _ = anim_cases.run(cuda, data, jobs, targets, records, loc)
     posed = np.zeros(n, bool)
     posed[targets["slot"]] = True
     c = centred(got_r)

@@ -7,6 +7,7 @@ r3_update_objects moves between affine and non-affine."""
 import numpy as np
 import pytest
 
+from harness import assert_same_bake
 from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE, CB_CULL, load_cuda_backend
 from rend3_b200.routines import per_camera_header
 from rend3_b200.scenes import cloud_camera, object_cloud_records
@@ -54,20 +55,6 @@ def non_affine_records(n):
     rec["enabled"][[40, 66, 100, 101, n - 1]] = 1
     rec["enabled"][[5, 20]] = [0, 0]                                         # disabled slots in the non-affine tile
     return rec
-
-
-def assert_same_bake(cuda, orc, rec, what, culled=True):
-    n = len(rec)
-    if culled:
-        assert np.array_equal(cuda.readback_visible(CAMERA_VIEWPORT), orc.readback_visible(CAMERA_VIEWPORT)), f"{what}: visible list"
-    en = rec["enabled"] != 0
-    a = cuda.readback_object_matrices(CAMERA_VIEWPORT, 0, n).view(np.uint32).reshape(n, 32)[en]
-    o = orc.readback_object_matrices(CAMERA_VIEWPORT, 0, n).view(np.uint32).reshape(n, 32)[en]
-    # NaN payloads may differ between x86 and the GPU: NaN == NaN, every other word bit for bit
-    an, on = np.isnan(a.view(np.float32)), np.isnan(o.view(np.float32))
-    assert np.array_equal(an, on), f"{what}: NaN positions differ"
-    bad = (a != o) & ~an
-    assert not bad.any(), f"{what}: MV/MVP words differ in slots {np.nonzero(en)[0][bad.any(axis=1)][:16]}"
 
 
 def test_non_affine_row3_matches_oracle(cuda):

@@ -10,7 +10,6 @@ import pytest
 
 import cull_reference as ref
 import cull_scenes as scenes
-import test_cull_reference as cpu
 from rend3_b200.backend import load_cuda_backend
 
 from oracle import load_oracle_backend
@@ -33,41 +32,41 @@ def assert_same(got, have, what):
     assert np.array_equal(got["mvps"].view(np.uint32), have["mvps"].view(np.uint32)), f"{what}: baked MVPs differ from the oracle"
 
 
-@pytest.mark.parametrize("w,h,samples", cpu.HIZ_CASES)
+@pytest.mark.parametrize("w,h,samples", scenes.HIZ_CASES)
 def test_hiz_levels_match_reference_and_oracle(cuda, w, h, samples):
     fused, down, tail = ref.hiz_fused_levels(w, h)
-    if (w, h) in cpu.FUSED:
-        assert fused == cpu.FUSED[(w, h)]
+    if (w, h) in scenes.FUSED:
+        assert fused == scenes.FUSED[(w, h)]
     if (w, h) == (1920, 1080):
         assert down >= 1 and tail
     if (w, h) == (3840, 2160):
         assert down == 2 and tail
-    levels = cpu.render_hiz(cuda, w, h, samples)
+    levels = scenes.render_hiz(cuda, w, h, samples)
     # what ran: the head kernel, one downsample launch per large level, the tail kernel if levels are left (r3_hiz_build)
     assert cuda.last_hiz_launches == 1 + down + int(tail), (cuda.last_hiz_launches, fused, down, tail)
-    cpu.assert_pyramid(levels, w, h, f"cuda {w}x{h}x{samples}")
-    orc = cpu.render_hiz(load_oracle_backend(), w, h, samples)
+    scenes.assert_pyramid(levels, w, h, f"cuda {w}x{h}x{samples}")
+    orc = scenes.render_hiz(load_oracle_backend(), w, h, samples)
     for m, (a, b) in enumerate(zip(levels, orc)):
         assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), f"{w}x{h}x{samples}: level {m} differs from the oracle"
 
 
 @pytest.mark.parametrize("samples", [1, 4])
 def test_exact_decisions(cuda, samples):
-    orc = {what: (got, want) for what, _, got, want, _, _ in cpu.exact_runs(load_oracle_backend(), samples)}
+    orc = {what: (got, want) for what, _, got, want, _, _ in scenes.exact_runs(load_oracle_backend(), samples)}
     stages = set()
-    for what, s, got, want, labels, pyramid in cpu.exact_runs(cuda, samples):
-        cpu.assert_pyramid(pyramid, 256, 256, "occluders")
-        cpu.check_exact(what, s, got, want, labels)
+    for what, s, got, want, labels, pyramid in scenes.exact_runs(cuda, samples):
+        scenes.assert_pyramid(pyramid, 256, 256, "occluders")
+        scenes.check_exact(what, s, got, want, labels)
         assert_same(got, orc[what][0], what)
         stages |= set(want["stage"][want["invocations"]].tolist())
     assert stages == {ref.BACKFACE, ref.PIXEL_CENTRE, ref.OCCLUDED, ref.PASS}, stages
 
 
 def test_perspective_edges(cuda):
-    orc = {what: got for what, _, got, _, _ in cpu.perspective_runs(load_oracle_backend())}
+    orc = {what: got for what, _, got, _, _ in scenes.perspective_runs(load_oracle_backend())}
     report = []
-    for what, s, got, want, labels in cpu.perspective_runs(cuda):
-        excluded = cpu.check_perspective(what, s, got, want, labels)
+    for what, s, got, want, labels in scenes.perspective_runs(cuda):
+        excluded = scenes.check_perspective(what, s, got, want, labels)
         assert_same(got, orc[what], what)
         report.append(f"{what}: {len(excluded)} of {len(labels)} excluded from the float64 check")
         assert len(excluded) < len(labels) // 4, report[-1]
@@ -75,8 +74,8 @@ def test_perspective_edges(cuda):
 
 
 def test_structural_scenes(cuda):
-    orc = {what: got for what, _, got, _ in cpu.structural_runs(load_oracle_backend())}
-    for what, s, got, want in cpu.structural_runs(cuda):
+    orc = {what: got for what, _, got, _ in scenes.structural_runs(load_oracle_backend())}
+    for what, s, got, want in scenes.structural_runs(cuda):
         scenes.assert_matches(got, want, s, what)
         assert_same(got, orc[what], what)
         if what == "ragged frame 1":
@@ -87,16 +86,16 @@ def test_structural_scenes(cuda):
             first = [int(b["batch_base_invocation"]) + int(i["invocation_start"]) for b in s.batches
                      for i in b["object_culling_information"][:int(b["total_objects"])]]
             assert first == [0, scenes.SB_INVOCATIONS, 3 * scenes.SB_INVOCATIONS // 2, 5 * scenes.SB_INVOCATIONS // 2], first
-    for what, s, got, want in cpu.mesh_end_runs(lambda: load_cuda_backend(0)):
+    for what, s, got, want in scenes.mesh_end_runs(lambda: load_cuda_backend(0)):
         scenes.assert_matches(got, want, s, what)
         assert want["pass32"][:2].all(), f"{what}: the triangles at the end of the allocation must survive to be compared"
-    for what, s, got, want in cpu.pingpong_runs(cuda):
+    for what, s, got, want in scenes.pingpong_runs(cuda):
         scenes.assert_matches(got, want, s, what)
 
 
 def test_high_vertex_ids(cuda):
-    s, got, want, hdr = cpu.high_id_run(cuda)
-    cpu.check_high_id(s, got, want, hdr, "cuda, ids >= 2^24")
+    s, got, want, hdr = scenes.high_id_run(cuda)
+    scenes.check_high_id(s, got, want, hdr, "cuda, ids >= 2^24")
 
 
 @pytest.mark.parametrize("host", [False, True])
@@ -107,14 +106,14 @@ def test_batched_frame(cuda, monkeypatch, host):
         monkeypatch.setenv("R3_HOST_BATCHING", "1")
     else:
         monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
-    for what, s, got, want in cpu.batched_frame_runs(cuda):
+    for what, s, got, want in scenes.batched_frame_runs(cuda):
         scenes.assert_matches(got, want, s, what)
     assert cuda.batching_info(0xFFFFFFFF)["path"].startswith("host" if host else "device"), cuda.batching_info(0xFFFFFFFF)
 
 
 def test_big_scene(cuda):
     s, ends = scenes.big_scene()
-    cpu.big_census(s, ends)
+    scenes.big_census(s, ends)
     hdr = scenes.ortho_header(256, 256, 0, len(s.objects))
     scenes.upload(cuda, s)
     got = scenes.run_cull(cuda, s, hdr)

@@ -5,9 +5,7 @@ import pytest
 
 import cull_reference as ref
 import cull_scenes as scenes
-import raster_scenes
-from rend3_b200.backend import CAMERA_VIEWPORT
-from rend3_b200.layouts import NO_PREVIOUS, PCU_MULTISAMPLED, PCU_POSITIVE_AREA_VISIBLE
+from rend3_b200.layouts import PCU_MULTISAMPLED, PCU_POSITIVE_AREA_VISIBLE
 
 from oracle import load_oracle_backend
 
@@ -107,103 +105,25 @@ def test_packed_index_order():
 
 
 # ------------------------------------------------------------------ the oracle against the reference
-def hiz_sizes():
-    return [(1920, 1080), (3840, 2160), (40, 24), (36, 36), (34, 34), (480, 270), (481, 270), (1, 777), (777, 1), (2, 2048), (4096, 2),
-            (1, 1)]
-
-
-HIZ_CASES = [(w, h, 1) for w, h in hiz_sizes()] + [(1920, 1080, 4), (481, 270, 4)]
-FUSED = {(1920, 1080): 3, (3840, 2160): 3, (40, 24): 3, (36, 36): 2, (34, 34): 1, (480, 270): 1, (481, 270): 0}
-
-
-def hiz_content(w, h, seed):
-    """Occluders for the hi-Z size tests: a far background over all but the top-left quarter and the last row and column (the uncovered
-    pixels read 0), random triangles in front of it, and one-pixel quads along the whole last row and column at depths below the
-    background's.  With odd sizes the unique minimum of a footprint then sits in its extra row or column.  Reverse-Z: the larger depth
-    is the nearer, and the pyramid keeps the smaller.  Returns (triangles in pixels, depth per triangle)."""
-    rng = np.random.default_rng(seed)
-    tris, z = [], []
-    x0, y0 = w // 4, h // 4
-    tris += [((x0, y0), (w - 1, y0), (w - 1, h - 1)), ((x0, y0), (w - 1, h - 1), (x0, h - 1))]
-    z += [0.45, 0.45]
-    for _ in range(40):
-        c = rng.uniform(0, 1, 2) * (w - 1, h - 1)
-        t = np.clip(np.round((c + rng.uniform(-0.3, 0.3, (3, 2)) * (w, h)) * 4) / 4, 0, (w - 1, h - 1))
-        tris.append(tuple(map(tuple, t)))
-        z.append(float(rng.uniform(0.5, 0.9)))
-    for x in range(w):
-        tris += [((x, h - 1), (x + 1, h - 1), (x + 1, h)), ((x, h - 1), (x + 1, h), (x, h))]
-        z += [0.05 + 0.35 * rng.random()] * 2
-    for y in range(h - 1):
-        tris += [((w - 1, y), (w, y), (w, y + 1)), ((w - 1, y), (w, y + 1), (w - 1, y + 1))]
-        z += [0.05 + 0.35 * rng.random()] * 2
-    return tris, np.array(z, F32)
-
-
-def render_hiz(backend, w, h, samples, seed=0):
-    tris, z = hiz_content(w, h, seed)
-    r = raster_scenes.build(backend, w, h, tris, z)
-    raster_scenes.draw(r, w, h, samples)
-    launches = backend.launch_count()
-    backend.hiz_build()
-    launches = backend.launch_count() - launches
-    levels = scenes.read_pyramid(backend, len(ref.hiz_dims(w, h)))
-    # level 0 is the min over the samples (resolve_depth_min.wgsl:18-27), which is what the depth resolve keeps as well
-    depth = backend.readback_depth()
-    assert np.array_equal(levels[0].view(np.uint32), depth.view(np.uint32)), f"{w}x{h}x{samples}: level 0 is not the resolved depth"
-    backend.last_hiz_launches = launches
-    return levels
-
-
-def assert_pyramid(levels, w, h, what):
-    want = ref.hiz_pyramid(levels[0])
-    assert [l.shape[::-1] for l in levels] == ref.hiz_dims(w, h), f"{what}: level sizes"
-    for m in range(1, len(levels)):
-        bad = levels[m].view(np.uint32) != want[m].view(np.uint32)
-        assert not bad.any(), f"{what}: level {m} differs from hi_z.wgsl at {np.count_nonzero(bad)} texels, first {np.argwhere(bad)[0]}"
-
-
-@pytest.mark.parametrize("w,h,samples", HIZ_CASES)
+@pytest.mark.parametrize("w,h,samples", scenes.HIZ_CASES)
 def test_oracle_hiz_matches_reference(w, h, samples):
-    levels = render_hiz(load_oracle_backend(), w, h, samples)
-    assert_pyramid(levels, w, h, f"oracle {w}x{h}x{samples}")
-    if (w, h) in FUSED:
-        assert ref.hiz_fused_levels(w, h)[0] == FUSED[(w, h)]
+    levels = scenes.render_hiz(load_oracle_backend(), w, h, samples)
+    scenes.assert_pyramid(levels, w, h, f"oracle {w}x{h}x{samples}")
+    if (w, h) in scenes.FUSED:
+        assert ref.hiz_fused_levels(w, h)[0] == scenes.FUSED[(w, h)]
     assert len(np.unique(levels[0])) > 3 or w * h < 16, "the depth buffer holds too few values"
     # the last row and column hold the one-pixel quads, below everything else that was drawn
     edge = np.concatenate([levels[0][-1, :], levels[0][:, -1]])
     assert (edge > 0).all() and (edge < 0.45).all(), "the last row and column must hold the quads"
 
 
-def exact_runs(backend, samples):
-    """The exact decision scene under every flag combination and a shadow camera: yields (what, got, want, header)."""
-    pyramid = scenes.draw_occluders(backend, samples)
-    tris, z, labels = scenes.exact_decision_triangles()
-    s = scenes.triangle_scene(tris, z)
-    scenes.upload(backend, s)
-    n = len(s.objects)
-    for flags in scenes.EXACT_FLAGS:
-        for cam in (CAMERA_VIEWPORT, 0):
-            hdr = scenes.ortho_header(256, 256, flags, n, shadow_index=cam)
-            got = scenes.run_cull(backend, s, hdr, cam)
-            want = scenes.reference_for(got, s, hdr, pyramid if cam == CAMERA_VIEWPORT else None)
-            yield f"flags {flags} camera {cam:#x}", s, got, want, labels, pyramid
-
-
-def check_exact(what, s, got, want, labels):
-    # the f32 path is exact here: float64 decides every triangle the same way
-    diff = np.nonzero(want["pass32"] != want["pass64"])[0]
-    assert not len(diff), f"{what}: f32 and float64 differ on {[labels[i] for i in diff[:5]]}"
-    scenes.assert_matches(got, want, s, what)
-
-
 @pytest.mark.parametrize("samples", [1, 4])
 def test_oracle_exact_decisions_match_reference(samples):
     orc = load_oracle_backend()
     stages = set()
-    for what, s, got, want, labels, pyramid in exact_runs(orc, samples):
-        assert_pyramid(pyramid, 256, 256, "occluders")
-        check_exact(what, s, got, want, labels)
+    for what, s, got, want, labels, pyramid in scenes.exact_runs(orc, samples):
+        scenes.assert_pyramid(pyramid, 256, 256, "occluders")
+        scenes.check_exact(what, s, got, want, labels)
         st = want["stage"][want["invocations"]]
         stages |= set(st.tolist())
         lab = {l: i for i, l in enumerate(labels)}
@@ -222,111 +142,20 @@ def test_oracle_exact_decisions_match_reference(samples):
     assert stages == {ref.BACKFACE, ref.PIXEL_CENTRE, ref.OCCLUDED, ref.PASS}, stages
 
 
-def perspective_runs(backend):
-    tris, labels, proj = scenes.perspective_scene()
-    s = scenes.world_triangle_scene(tris)
-    backend.set_render_target(64, 64, 1, (0, 0, 0, 0))
-    backend.forward_begin()
-    backend.hiz_build()                                   # an empty depth buffer: a uniform pyramid of 0.0
-    pyramid = scenes.read_pyramid(backend, len(ref.hiz_dims(64, 64)))
-    scenes.upload(backend, s)
-    for flags in (0, PCU_POSITIVE_AREA_VISIBLE, PCU_MULTISAMPLED):
-        hdr = scenes.ortho_header(64, 64, flags, len(s.objects), proj=proj)
-        got = scenes.run_cull(backend, s, hdr)
-        yield f"perspective flags {flags}", s, got, scenes.reference_for(got, s, hdr, pyramid), labels
-
-
-def check_perspective(what, s, got, want, labels, margin_floor=1.0):
-    """Decisions equal the f32 reference everywhere; float64 is checked where the margin allows.  Returns the excluded labels."""
-    scenes.assert_matches(got, want, s, what)
-    m = ref.decision_margin(want["q64"], want["stage64"], want["flags"], want["viewport"])
-    near = m <= margin_floor
-    bad = (want["pass32"] != want["pass64"]) & ~near
-    assert not bad.any(), f"{what}: f32 and float64 differ beyond the margin on {[labels[i] for i in np.nonzero(bad)[0][:5]]}"
-    unit = [i for i, l in enumerate(labels) if l == "unit w"]
-    assert (want["q64"]["clip"][0][unit, 3] == 1).all(), "the unit-w triangles must have w == 1.0 exactly"
-    return sorted(labels[i] for i in np.nonzero(near)[0])
-
-
 def test_oracle_perspective_edges_match_reference():
     orc = load_oracle_backend()
-    for what, s, got, want, labels in perspective_runs(orc):
-        excluded = check_perspective(what, s, got, want, labels)
+    for what, s, got, want, labels in scenes.perspective_runs(orc):
+        excluded = scenes.check_perspective(what, s, got, want, labels)
         assert len(excluded) < 30, f"{what}: {len(excluded)} margin exclusions: {excluded}"
         assert {ref.BACKFACE, ref.PASS} <= set(want["stage"][want["invocations"]].tolist())
 
 
-def structural_runs(backend):
-    """Yields (what, scene, got, want, census): the ragged scene over two frames (NO_PREVIOUS, then in range / past the partition),
-    superblock-boundary scenes of 4 x 32768 + {-256, 0, 256} invocations, the mesh-end scene in a fresh context and again after a
-    larger mesh left stale words behind the smaller one."""
-    s = scenes.ragged_scene()
-    scenes.upload(backend, s)
-    n = len(s.objects)
-    hdr = scenes.ortho_header(256, 256, 0, n)
-    got = scenes.run_cull(backend, s, hdr)
-    yield "ragged frame 0", s, got, scenes.reference_for(got, s, hdr, None)
-    first = {}
-    for b in s.batches:
-        for info in b["object_culling_information"][:int(b["total_objects"])]:
-            first[int(info["object_id"])] = int(b["batch_base_invocation"]) + int(info["invocation_start"])
-    total = scenes.total_invocations(s.batches)
-    prev = [NO_PREVIOUS if i % 3 == 0 else (first[i] if i % 3 == 1 else total + 4096 * 32 + i) for i in range(n)]
-    counts = [int(c) // 3 for c in s.objects["index_count"]]
-    atomic = [0 if i in (0, 1, 254, 255) else 1 for i in range(n)]
-    keys = [2 if i in (0, 1, 254, 255) else 0 for i in range(n)]
-    b2, r2 = scenes.build_tables(counts, atomic=atomic, keys=keys, prev=prev)
-    s2 = scenes.Scene(s.objects, s.mesh, b2, r2)
-    got = scenes.run_cull(backend, s2, hdr)
-    yield "ragged frame 1", s2, got, scenes.reference_for(got, s2, hdr, None)
-    for delta in (0, -256, 256):
-        s = scenes.superblock_scene(delta)
-        scenes.upload(backend, s)
-        hdr = scenes.ortho_header(256, 256, PCU_POSITIVE_AREA_VISIBLE, len(s.objects))
-        got = scenes.run_cull(backend, s, hdr)
-        yield f"superblock {delta:+d}", s, got, scenes.reference_for(got, s, hdr, None)
-
-
-def mesh_end_runs(make_backend):
-    """The mesh-end scene in a fresh context, and again after a larger mesh buffer whose words past the smaller one's end are stale
-    (the allocation is kept, so the bulk copy of the index runs reads them).  Closes the contexts it makes."""
-    s, end, stale = scenes.mesh_end_scene()
-    for with_stale in (False, True):
-        b = make_backend()
-        try:
-            if with_stale:
-                b.set_mesh_buffer(stale)
-            scenes.upload(b, s)
-            hdr = scenes.ortho_header(256, 256, PCU_MULTISAMPLED, len(s.objects))
-            got = scenes.run_cull(b, s, hdr)
-            yield f"mesh end stale={with_stale}", s, got, scenes.reference_for(got, s, hdr, None)
-        finally:
-            b.close()
-
-
-def stale_triangles(s, stale, got, hdr):
-    """The decisions of object 2's triangle 37 and object 3's first triangle when robust access is honoured, and when the stale words
-    past mesh_words were read instead."""
-    robust = scenes.reference_for(got, s, hdr, None)
-    stale_view = scenes.Scene(s.objects, stale, s.batches, s.regions)
-    wrong = scenes.reference_for(got, stale_view, hdr, None)
-    picks = []
-    for b in s.batches:
-        for info in b["object_culling_information"][:int(b["total_objects"])]:
-            g = int(b["batch_base_invocation"]) + int(info["invocation_start"])
-            if int(info["object_id"]) == 2:
-                picks.append(g + 37)
-            if int(info["object_id"]) == 3:
-                picks.append(g)
-    return robust["stage"][picks], wrong["stage"][picks]
-
-
 def test_oracle_structural_scenes_match_reference():
     orc = load_oracle_backend()
-    for what, s, got, want in structural_runs(orc):
+    for what, s, got, want in scenes.structural_runs(orc):
         scenes.assert_matches(got, want, s, what)
         assert want["pass32"].any() and not want["pass32"].all(), what
-    for what, s, got, want in mesh_end_runs(load_oracle_backend):
+    for what, s, got, want in scenes.mesh_end_runs(load_oracle_backend):
         scenes.assert_matches(got, want, s, what)
         assert want["pass32"][:2].all(), f"{what}: the triangles at the end of the allocation must survive to be compared"
 
@@ -341,86 +170,31 @@ def test_mesh_end_scene_reaches_the_guard_and_the_robust_reads():
     assert int(s.objects["first_index"][2]) + 120 > end
     hdr = scenes.ortho_header(256, 256, PCU_MULTISAMPLED, len(s.objects))
     got = {"mvps": np.repeat(hdr["view_proj"].reshape(1, 16), 4, 0), "prev": np.zeros(0, np.uint32)}
-    robust, wrong = stale_triangles(s, stale, got, hdr)
+    robust, wrong = scenes.stale_triangles(s, stale, got, hdr)
     assert robust.tolist() == [ref.PASS, ref.PASS] and wrong.tolist() == [ref.BACKFACE, ref.BACKFACE], (robust, wrong)
 
 
-def pingpong_runs(backend):
-    """The three frames of scenes.pingpong_frames, each compared as it comes (no second cull): yields (what, scene, got, want)."""
-    s, frames = scenes.pingpong_frames()
-    scenes.upload(backend, s)
-    hdr = scenes.ortho_header(256, 256, 0, len(s.objects))
-    for k, (b, r) in enumerate(frames):
-        fs = scenes.Scene(s.objects, s.mesh, b, r)
-        got = scenes.run_cull(backend, fs, hdr, settle=False)
-        yield f"ping-pong frame {k}", fs, got, scenes.reference_for(got, fs, hdr, None)
-
-
-def pingpong_census(frames):
-    """The index buffer is reallocated for frame 1 (next_pow2 of its elements grows) and frame 1 and 2 read previous bits in range."""
-    inv = [scenes.total_invocations(b) for b, _ in frames]
-    pow2 = lambda v: 1 << (int(v) - 1).bit_length()
-    assert inv[0] < inv[1] > inv[2] and pow2(3 * inv[1]) > pow2(3 * inv[0])
-    for b, _ in frames[1:]:
-        prev = [int(i["previous_global_invocation"]) for bb in b for i in bb["object_culling_information"][:int(bb["total_objects"])]]
-        assert sum(p != NO_PREVIOUS for p in prev) >= 20
-
-
 def test_oracle_pingpong_frames_match_reference():
-    pingpong_census(scenes.pingpong_frames()[1])
-    for what, s, got, want in pingpong_runs(load_oracle_backend()):
+    scenes.pingpong_census(scenes.pingpong_frames()[1])
+    for what, s, got, want in scenes.pingpong_runs(load_oracle_backend()):
         scenes.assert_matches(got, want, s, what)
         if what != "ping-pong frame 0":
             resid = want["dc_resid"]["vertex_count"].sum()
             assert 0 < resid < want["dc_pred"]["vertex_count"].sum(), f"{what}: some triangles must be residual and some not"
 
 
-def high_id_run(backend):
-    s = scenes.high_vertex_id_scene()
-    scenes.upload(backend, s)
-    hdr = scenes.ortho_header(256, 256, PCU_MULTISAMPLED, len(s.objects))
-    got = scenes.run_cull(backend, s, hdr)
-    return s, got, scenes.reference_for(got, s, hdr, None), hdr
-
-
-def check_high_id(s, got, want, hdr, what):
-    scenes.assert_matches(got, want, s, what)
-    assert want["pass32"].all(), f"{what}: the triangles behind ids >= 2^24 face the camera"
-    masked = s.mesh.copy()
-    masked[64:70] &= 0xFFFFFF
-    low = scenes.reference_for(got, scenes.Scene(s.objects, masked, s.batches, s.regions), hdr, None)
-    assert not low["pass32"].any(), "fetching the positions through the masked ids must decide differently"
-    assert want["idx_pred"][:6].tolist() == [0, 1, 2, (1 << 24) | 0, (1 << 24) | 1, (1 << 24) | 2]
-    assert want["idx_resid"][3 * 512:3 * 512 + 3].tolist() == [(2 << 24) | 3, (2 << 24) | 4, (2 << 24) | 5]
-
-
 def test_oracle_high_vertex_ids_match_reference():
     orc = load_oracle_backend()
     try:
-        s, got, want, hdr = high_id_run(orc)
-        check_high_id(s, got, want, hdr, "oracle, ids >= 2^24")
+        s, got, want, hdr = scenes.high_id_run(orc)
+        scenes.check_high_id(s, got, want, hdr, "oracle, ids >= 2^24")
     finally:
         orc.close()
 
 
-def big_census(s, ends):
-    """More than two passes of the persistent grid (4224 workgroups at 4 CTAs / SM, 5280 at 5), and the end-of-buffer objects lie in
-    workgroups past the first pass, on both sides of the staging guard."""
-    total = scenes.total_invocations(s.batches)
-    assert total // 256 > 2 * scenes.WARP_STRIDE
-    end = len(s.mesh)
-    wgs = {}
-    for b in s.batches:
-        for info in b["object_culling_information"][:int(b["total_objects"])]:
-            wgs[int(info["object_id"])] = (int(b["batch_base_invocation"]) + int(info["invocation_start"])) // 256
-    assert min(wgs[o] for o in ends) > 132 * 5 * 8
-    runs = [(int(s.objects[o]["first_index"]) & ~3) + 100 for o in ends]
-    assert (end + 4) in runs and any(r > end + 4 for r in runs) and any(r < end + 4 for r in runs)
-
-
 def test_oracle_big_scene_matches_reference():
     s, ends = scenes.big_scene()
-    big_census(s, ends)
+    scenes.big_census(s, ends)
     orc = load_oracle_backend()
     scenes.upload(orc, s)
     hdr = scenes.ortho_header(256, 256, 0, len(s.objects))
@@ -430,31 +204,9 @@ def test_oracle_big_scene_matches_reference():
     assert want["pass32"].any() and not want["pass32"].all()
 
 
-def batched_frame_runs(backend):
-    """One whole frame of a small cube field through BaseRenderGraph (the batch tables from batch_objects, host- or device-built),
-    then each camera's cull compared with the reference fed the tables, MVPs and pyramid that cull used."""
-    from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings, per_camera_header
-    from rend3_b200.scenes import cube_field_scene
-    res = (480, 270)
-    ev = cube_field_scene(n_objects=1500, seed=5, resolution=res, n_point_lights=0, shadow_resolution=256, pull_back=12.0, extent=30.0)
-    BaseRenderGraph(backend).add_to_graph(ev, res, 1, BaseRenderGraphSettings())
-    pyramid = scenes.read_pyramid(backend, len(ref.hiz_dims(*res)))
-    n = len(ev.object_buffer)
-    cams = [(CAMERA_VIEWPORT, per_camera_header(ev.camera, CAMERA_VIEWPORT, res, 1, n), pyramid)]
-    cams += [(i, per_camera_header(sh.camera, i, (sh.size, sh.size), 1, n), None) for i, sh in enumerate(ev.shadows)]
-    for cam, hdr, pyr in cams:
-        batches, regions = backend.readback_batches(cam)
-        s = scenes.Scene(ev.object_buffer, np.asarray(ev.mesh_buffer, np.uint32), batches, regions)
-        got = dict(words=backend.readback_culling_results(cam, 0), prev=backend.readback_culling_results(cam, 1),
-                   dc_pred=backend.readback_draw_calls(cam, 0), dc_resid=backend.readback_draw_calls(cam, 1),
-                   idx_pred=backend.readback_indices(cam, 0), idx_resid=backend.readback_indices(cam, 1),
-                   mvps=backend.readback_object_matrices(cam, 0, n)["model_view_proj"].reshape(n, 16))
-        yield f"frame camera {cam:#x}", s, got, scenes.reference_for(got, s, hdr, pyr)
-
-
 def test_oracle_host_batched_frame_matches_reference():
     stages = set()
-    for what, s, got, want in batched_frame_runs(load_oracle_backend()):
+    for what, s, got, want in scenes.batched_frame_runs(load_oracle_backend()):
         scenes.assert_matches(got, want, s, what)
         stages |= set(want["stage"][want["invocations"]].tolist())
     assert {ref.BACKFACE, ref.PASS} <= stages

@@ -5,7 +5,6 @@ r3_set_directional_light_sources; they stay one graph launch; they match the ora
 documented checks and state rules."""
 import ctypes
 import os
-import re
 import subprocess
 import tempfile
 
@@ -13,12 +12,12 @@ import numpy as np
 import pytest
 
 from directional_change_case import NAN_FRAMES, RES, STEPS, C, camera, same_bits, world
+from harness import ROOT, check_declared_and_exported, unbound_backend
 from rend3_b200 import layouts
-from rend3_b200.backend import Backend, R3Error
+from rend3_b200.backend import R3Error, load_cuda_backend
 from rend3_b200.layouts import DIRECTIONAL_LIGHT_CHANGE_DTYPE, LIGHT_SOURCE_DTYPE
 from rend3_b200.world import LEFT, DirectionalLight, Renderer
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 R3_E_INVALID, R3_E_STATE = -1, -5
 DECLS = ("int r3_update_directional_light_sources(r3_ctx*, const r3_directional_light_change* changes, uint32_t n);",
          "int r3_update_directional_light_sources_device(r3_ctx*, const r3_directional_light_change* d_changes, uint32_t n);")
@@ -26,15 +25,7 @@ DECLS = ("int r3_update_directional_light_sources(r3_ctx*, const r3_directional_
 
 # ------------------------------------------------------------------ CPU
 def test_new_symbols_are_exported_and_declared():
-    from rend3_b200.backend import CUDA_LIB_PATH, ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
-    for decl in DECLS:
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        assert getattr(lib, name)(None, None, 1) == R3_E_INVALID   # no context: rejected before anything is touched
+    check_declared_and_exported(DECLS, (None, None, 1))
 
 
 def test_change_record_layout_matches_c_header():
@@ -51,13 +42,6 @@ def test_change_record_layout_matches_c_header():
     assert out[1:1 + len(fields)] == [DIRECTIONAL_LIGHT_CHANGE_DTYPE.fields[f][1] for f in fields] == [0, 4, 8, 20, 24, 36]
     assert out[1 + len(fields):] == [layouts.DIR_CHANGE_COLOR, layouts.DIR_CHANGE_INTENSITY, layouts.DIR_CHANGE_DIRECTION,
                                      layouts.DIR_CHANGE_DISTANCE] == [1, 2, 4, 8]
-
-
-def unbound_backend():
-    """A Backend with no library: a wrapper that rejects its arguments never reaches the C call."""
-    b = Backend.__new__(Backend)
-    b.lib, b.prefix, b.ctx = None, "r3_", None
-    return b
 
 
 def test_wrappers_reject_wrong_dtype_shape_and_stride():
@@ -130,12 +114,6 @@ def test_change_records_name_shadow_indices_and_refuse_resolution():
 
 
 # ------------------------------------------------------------------ GPU
-def cuda(parity=False):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, parity_target=parity)
-
-
 def device_records(b, recs):
     """The records as a CUDA tensor produced on the context's stream."""
     import torch
@@ -181,7 +159,7 @@ def test_gpu_updates_equal_re_setting_the_lights(left, graph):
 
     r = world(left)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0), ambient_color=(0.02, 0.02, 0.02, 0.0))
-    a, hb, db = cuda(True), cuda(True), cuda(True)
+    a, hb, db = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     set_a = SetInFrame(a)
     ga, gh, gd = BaseRenderGraph(set_a), BaseRenderGraph(hb), BaseRenderGraph(db)
     keep = []
@@ -228,7 +206,7 @@ def test_gpu_device_form_matches_the_oracle():
 
     r = world(True)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0), ambient_color=(0.02, 0.02, 0.02, 0.0))
-    db, orc = cuda(True), load_lights_oracle_backend()
+    db, orc = load_cuda_backend(0, parity_target=True), load_lights_oracle_backend()
     gd, go = BaseRenderGraph(db), BaseRenderGraph(orc)
     keep = []
     compared = 0
@@ -288,7 +266,7 @@ def test_gpu_calls_and_state():
     r.set_camera_data(camera(0, True))
     ev = r.evaluate()
     one = r.directional_change_records([(0, C(intensity=0.2))])
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     # no sources yet, and the host-evaluated path: R3_E_STATE from both forms
     for set_first in (False, True):
         if set_first:
@@ -330,7 +308,7 @@ def test_gpu_calls_and_state():
     keep = device_records(b, mixed)
     b.update_directional_light_sources_device(keep)
     b.evaluate_shadow_cameras(ev.camera.location())
-    want_b = cuda()
+    want_b = load_cuda_backend(0, parity_target=False)
     want_b.set_directional_light_sources(ev.directional_sources, *ev.shadow_target_size, True)
     want_b.update_directional_light_sources(recs)
     want_b.evaluate_shadow_cameras(ev.camera.location())
@@ -338,7 +316,7 @@ def test_gpu_calls_and_state():
     assert same_bits(got[0], want[0]) and same_bits(got[1], want[1]), "the device form did not drop exactly its bad entries"
     for h, c in good:
         r.update_directional_light(h, c)
-    fresh = cuda()
+    fresh = load_cuda_backend(0, parity_target=False)
     set_world(fresh, r)
     fresh.evaluate_shadow_cameras(ev.camera.location())
     ref = fresh.readback_shadow_cameras(n)

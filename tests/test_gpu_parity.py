@@ -11,6 +11,7 @@ import os
 import numpy as np
 import pytest
 
+from harness import TOL, compare_frame_state, hdr_close
 from rend3_b200 import glam
 from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE, CB_CULL, load_cuda_backend
 from rend3_b200.layouts import OBJECT_DTYPE
@@ -21,7 +22,6 @@ from rend3_b200.world import Camera
 from oracle import load_oracle_backend
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-4
 
 
 @pytest.fixture()
@@ -30,19 +30,6 @@ def cuda():
     b = load_cuda_backend(0)
     yield b
     b.close()
-
-
-def hdr_close(a, b, what="", f16_samples=False):
-    """TOL = 1e-4 (north_star), relative above 1.0.  With SampleCount::Four the samples live in an rgba16f target BEFORE the
-    box filter (base.rs:245-255), so a 1e-6 difference in a shaded colour can land on the other side of a half-precision
-    rounding boundary: there the bound is TOL plus one f16 ulp of the value."""
-    ref = np.abs(b.astype(np.float64))
-    err = np.abs(a.astype(np.float64) - b.astype(np.float64)) / np.maximum(1.0, ref)
-    bound = TOL + (np.maximum(ref * 2.0 ** -10, 2.0 ** -24) / np.maximum(1.0, ref) if f16_samples else 0.0)
-    bad = np.nan_to_num(err, nan=np.inf) > bound
-    both_nan = np.isnan(a) & np.isnan(b)
-    bad &= ~both_nan
-    assert not bad.any(), f"{what}: {bad.sum()} channel values differ by more than {TOL} (max {np.nanmax(err):.3e})"
 
 
 # ------------------------------------------------------------------ object cull + uniform bake
@@ -190,44 +177,6 @@ def test_gpu_skinning_is_bit_exact(cuda):
 
 
 # ------------------------------------------------------------------ whole frames
-def compare_frame_state(cuda, orc, ev, cameras, check_pixels=True, what="", f16_samples=False):
-    for cam in cameras:
-        bc, rc = cuda.readback_batches(cam)
-        bo, ro = orc.readback_batches(cam)
-        assert len(bc) == len(bo) and rc.tobytes() == ro.tobytes(), f"{what} camera {cam}: batch / region tables differ"
-        for k in range(len(bo)):   # slots past total_objects are unspecified (the reference reuses its scratch array, batching.rs:186)
-            n_obj = int(bo[k]["total_objects"])
-            for f in ("total_objects", "total_invocations", "batch_base_invocation"):
-                assert bc[k][f] == bo[k][f], f"{what} camera {cam}: batch {k} {f}"
-            assert bc[k]["object_culling_information"][:n_obj].tobytes() == bo[k]["object_culling_information"][:n_obj].tobytes(), \
-                f"{what} camera {cam}: batch {k} object table differs"
-        for part in (0, 1):
-            # the CUDA path sizes its buffers with device-side upper bounds: compare what the oracle defines, the rest stays cleared
-            dc, do = cuda.readback_draw_calls(cam, part), orc.readback_draw_calls(cam, part)
-            assert dc[:len(do)].tobytes() == do.tobytes(), f"{what} camera {cam}: draw calls (partition {part}) differ"
-            assert not dc[len(do):].view(np.uint8).any(), f"{what} camera {cam}: stray draw calls"
-            ic, io = cuda.readback_indices(cam, part), orc.readback_indices(cam, part)
-            for r in range(len(do)):   # only the listed part of each region is defined
-                b0, cnt = int(do[r]["base_index"]), int(do[r]["vertex_count"])
-                if part == 1 and cam != CAMERA_VIEWPORT:
-                    continue
-                assert np.array_equal(ic[b0:b0 + cnt], io[b0:b0 + cnt]), f"{what} camera {cam}: index list of region {r} differs"
-        ro_bits = orc.readback_culling_results(cam, 0)
-        assert np.array_equal(cuda.readback_culling_results(cam, 0)[:len(ro_bits)], ro_bits), f"{what}: visibility bits differ"
-    if check_pixels:
-        assert np.array_equal(cuda.readback_depth().view(np.uint32), orc.readback_depth().view(np.uint32)), f"{what}: depth differs"
-        hdr_close(cuda.readback_hdr_f32(), orc.readback_hdr_f32(), what + " hdr f32", f16_samples)
-        h16c, h16o = cuda.readback_hdr_f16().astype(np.float32), orc.readback_hdr_f16().astype(np.float32)
-        ulp = np.maximum(np.abs(h16o) * 2.0 ** -10, 2.0 ** -24)
-        assert np.all(np.abs(h16c - h16o) <= ulp + TOL * np.maximum(1.0, np.abs(h16o))), f"{what}: rgba16f target differs by more than 1 ulp"
-        lc, lo = cuda.readback_ldr().astype(int), orc.readback_ldr().astype(int)
-        assert np.abs(lc - lo).max() <= 1, f"{what}: 8-bit output differs by more than 1 LSB"
-        assert np.count_nonzero(lc != lo) <= 1e-3 * lc.size
-        if ev.shadows:
-            w, h = ev.shadow_target_size
-            assert np.array_equal(cuda.readback_shadow_atlas(w, h).view(np.uint32), orc.readback_shadow_atlas(w, h).view(np.uint32)), f"{what}: shadow atlas differs"
-
-
 def test_cube_field_frame_matches_oracle(cuda):
     """C1-shaped scene at reduced size: 2000 cubes, directional light with shadow map, 3 point lights."""
     res = (480, 270)
@@ -395,22 +344,24 @@ def test_empty_and_ragged_inputs(cuda):
 
 
 # ------------------------------------------------------------------ the reference's golden scenes through the CUDA path
-def test_reference_goldens_on_cuda(cuda, monkeypatch):
-    import test_oracle_golden as g
+def test_reference_goldens_on_cuda(cuda):
+    from functools import partial
 
-    monkeypatch.setattr(g, "load_oracle_backend", lambda: load_cuda_backend(0))
-    g.test_empty()
+    import reference_goldens as g
+
+    load = partial(load_cuda_backend, 0)
+    g.empty(load)
     for args in [("Left", "Cw", True), ("Left", "Ccw", False), ("Right", "Cw", False), ("Right", "Ccw", True)]:
-        g.test_triangle(*args)
-    g.test_coordinate_space()
-    g.test_sample_coverage(1)
-    g.test_sample_coverage(4)
-    g.test_msaa_four()
-    g.test_multi_frame_add()
-    g.test_duplicate_object_retain()
-    g.test_shadow_plane()
-    g.test_shadow_cube()
-    g.test_cube_example_screenshot()
+        g.triangle(load, *args)
+    g.coordinate_space(load)
+    g.sample_coverage(load, 1)
+    g.sample_coverage(load, 4)
+    g.msaa_four(load)
+    g.multi_frame_add(load)
+    g.duplicate_object_retain(load)
+    g.shadow_plane(load)
+    g.shadow_cube(load)
+    g.cube_example_screenshot(load)
 
 
 def test_error_paths(cuda):

@@ -4,28 +4,21 @@ validation, their order against r3_pose_skeletons, r3_skin_posed from what they 
 with the oracle handed the expected joint buffer through r3o_set_skeletons."""
 import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
 
 from anim_reference import _mul, same_bits
+from harness import ROOT, check_declared_and_exported, expect_error, unbound_backend
 from rend3_b200 import glam
-from rend3_b200.backend import CUDA_LIB_PATH, Backend, R3Error
+from rend3_b200.backend import load_cuda_backend
 from rend3_b200.layouts import ATTR_ABSENT, JOINT_WRITE_DTYPE, SKINNING_INPUT_DTYPE
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 f32 = np.float32
 E_INVALID, E_STATE = -1, -5
 NO_SKELETONS = np.zeros(0, dtype=SKINNING_INPUT_DTYPE)
 # IEEE edges the copy form must keep bit for bit: -0.0, +inf, -inf, quiet NaNs with payloads and sign, a signalling NaN
 SPECIAL_BITS = np.array([0x80000000, 0x7F800000, 0xFF800000, 0x7FC01234, 0xFFC00001, 0x7F800001, 0x7FBFFFFF], dtype=np.uint32)
-
-
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
 
 
 def writes_of(rows):
@@ -82,18 +75,11 @@ def copy_case(seed=0):
 
 # ------------------------------------------------------------------ without a GPU
 def test_library_exports_both_entry_points_with_the_headers_signatures():
-    from rend3_b200.backend import ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
-    for decl in ("int r3_set_joint_matrices(r3_ctx*, const r3_joint_write* writes, uint32_t n_writes, const float* mat4s, uint32_t n_mat4s, "
-                 "const float* inverse_binds_or_null, uint32_t n_inverse_binds);",
-                 "int r3_set_joint_matrices_device(r3_ctx*, const r3_joint_write* d_writes, uint32_t n_writes, const float* d_mat4s, "
-                 "uint32_t n_mat4s, const float* d_inverse_binds_or_null, uint32_t n_inverse_binds);"):
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        assert getattr(lib, name)(None, None, 0, None, 0, None, 0) == E_INVALID   # no context: rejected before anything is touched
+    check_declared_and_exported(("int r3_set_joint_matrices(r3_ctx*, const r3_joint_write* writes, uint32_t n_writes, const float* mat4s, "
+                                 "uint32_t n_mat4s, const float* inverse_binds_or_null, uint32_t n_inverse_binds);",
+                                 "int r3_set_joint_matrices_device(r3_ctx*, const r3_joint_write* d_writes, uint32_t n_writes, const float* d_mat4s, "
+                                 "uint32_t n_mat4s, const float* d_inverse_binds_or_null, uint32_t n_inverse_binds);"),
+                                (None, None, 0, None, 0, None, 0))
 
 
 def test_joint_write_layout_matches_c_header():
@@ -113,21 +99,6 @@ def test_joint_write_layout_matches_c_header():
     assert 'R3_STATIC_ASSERT(sizeof(r3_joint_write) == 16, "r3_joint_write");' in open(os.path.join(ROOT, "include", "r3_layouts.h")).read()
 
 
-class _NoCalls:
-    """Stands in for the library: any call through it fails the test."""
-
-    def __getattr__(self, name):
-        def call(*args):
-            raise AssertionError(f"{name} was called")
-        return call
-
-
-def _unbound_backend():
-    b = Backend.__new__(Backend)
-    b.lib, b.prefix, b.ctx = _NoCalls(), "r3_", None
-    return b
-
-
 W1 = writes_of([(0, 1, 0, 0)])
 
 
@@ -142,7 +113,7 @@ W1 = writes_of([(0, 1, 0, 0)])
 ], ids=["words", "2d-writes", "float64", "1d-mats", "12-floats", "3x4-binds", "int-binds"])
 def test_host_wrapper_rejects_bad_shapes_and_dtypes_before_calling(writes, mat4s, inverse_binds):
     with pytest.raises(AssertionError, match="writes|mat4s|inverse_binds"):
-        _unbound_backend().set_joint_matrices(writes, mat4s, inverse_binds)
+        unbound_backend().set_joint_matrices(writes, mat4s, inverse_binds)
 
 
 class _FakeCuda:
@@ -171,7 +142,7 @@ class _FakeCuda:
 
 
 def test_device_wrapper_rejects_host_misaligned_and_mistyped_tensors_before_calling():
-    b = _unbound_backend()
+    b = unbound_backend()
     w, m = _FakeCuda((2, 4), "torch.int32"), _FakeCuda((2, 16), "torch.float32")
     bad = [
         (_FakeCuda((2, 4), "torch.int32", cuda=False), m, None),                   # host writes
@@ -192,12 +163,6 @@ def test_device_wrapper_rejects_host_misaligned_and_mistyped_tensors_before_call
 
 
 # ------------------------------------------------------------------ GPU
-def cuda():
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0)
-
-
 def upload(b, buf, inputs=NO_SKELETONS):
     b.set_skeletons(inputs, buf)
     return b
@@ -210,7 +175,7 @@ def bits(a):
 @pytest.mark.gpu
 def test_gpu_copy_form_keeps_every_bit():
     buf, writes, mats, _ = copy_case(1)
-    b = upload(cuda(), buf)
+    b = upload(load_cuda_backend(0), buf)
     b.set_joint_matrices(writes, mats)
     got = b.readback_joint_matrices(0, len(buf))
     b.close()
@@ -227,7 +192,7 @@ def test_gpu_copy_form_keeps_every_bit():
 def test_gpu_product_form_equals_float32_restatement():
     buf, writes, mats, binds = copy_case(2)
     writes["first_inverse_bind"][-1] = writes["first_inverse_bind"][-2] = 0   # the 65- and 600-joint writes share one inverse-bind range
-    b = upload(cuda(), buf)
+    b = upload(load_cuda_backend(0), buf)
     b.set_joint_matrices(writes, mats, binds)
     got = b.readback_joint_matrices(0, len(buf))
     b.close()
@@ -261,11 +226,11 @@ def test_gpu_device_form_equals_host_form_and_drops_bad_writes_whole(product):
                     + ([(0, 4, 0, n_m - 2), (0, 2, 0, 0xFFFFFFFF)] if product else []))
     mixed = np.concatenate([bad[:2], writes[:4], bad[2:], writes[4:]])
     ib = binds if product else None
-    host = upload(cuda(), buf)
+    host = upload(load_cuda_backend(0), buf)
     host.set_joint_matrices(writes, mats, ib)
     want = host.readback_joint_matrices(0, n_buf)
     host.close()
-    dev = upload(cuda(), buf)
+    dev = upload(load_cuda_backend(0), buf)
     d = _device_sources(dev, mixed.view(np.int32).reshape(-1, 4), mats, binds)
     dev.set_joint_matrices_device(d[0], d[1], d[2] if product else None)
     got = dev.readback_joint_matrices(0, n_buf)
@@ -282,7 +247,7 @@ def test_gpu_device_form_equals_host_form_and_drops_bad_writes_whole(product):
 @pytest.mark.gpu
 def test_gpu_rejections_leave_the_buffer_unchanged():
     buf, writes, mats, binds = copy_case(4)
-    b = cuda()
+    b = load_cuda_backend(0)
     expect_error(E_STATE, b.set_joint_matrices, writes, mats)
     expect_error(E_STATE, b.set_joint_matrices_device, 4096, 4096, None, n_writes=1, n_mat4s=1)
     upload(b, buf)
@@ -329,7 +294,7 @@ def test_gpu_later_of_pose_and_write_wins():
     writes = writes_of([(t0 + 5, 10, 0, 0), (free, 1, 11, 0)])   # inside target 0's range, and a range no job targets
 
     def run(order):
-        b = cuda()
+        b = load_cuda_backend(0)
         b.set_animations(*library.arrays())
         b.set_skeletons(NO_SKELETONS, buf)
         b.set_pose_jobs(jobs, targets)
@@ -372,14 +337,14 @@ def test_gpu_skin_posed_from_written_matrices_equals_skin_and_oracle():
     start = np.zeros((72, 16), f32)
     want = expected(start, writes, globals_, binds)
     assert np.isfinite(want).all()
-    b = upload(cuda(), start, inputs)
+    b = upload(load_cuda_backend(0), start, inputs)
     b.set_mesh_buffer(words)
     b.set_joint_matrices(writes, globals_, binds)
     b.skin_posed()
     mesh, jm = b.readback_mesh_buffer(len(words)), b.readback_joint_matrices(0, 72)
     b.close()
     assert np.array_equal(bits(jm), bits(want))
-    ref = cuda()
+    ref = load_cuda_backend(0)
     ref.set_mesh_buffer(words)
     ref.skin(inputs, want)
     assert np.array_equal(ref.readback_mesh_buffer(len(words)), mesh)

@@ -3,39 +3,25 @@ world.py's full table (bit for bit) and the CPU oracle given the full tables (wi
 alpha-testing rule after the device form, the frame graph, the transparency-change recipe, growth and the calls' validation."""
 import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
 
+from harness import (ROOT, assert_same_frame, assert_same_ldr, check_declared_and_exported, expect_error, hdr_close, on_stream, settings,
+                     to_device, unbound_backend)
 from material_update_case import CUTOUT_VALUE, EMISSIVE, OPAQUE_VALUE, MaterialWorld, frames, updates
-from rend3_b200.backend import CAMERA_VIEWPORT, CUDA_LIB_PATH, Backend, R3Error
+from rend3_b200.backend import CAMERA_VIEWPORT, load_cuda_backend
 from rend3_b200.layouts import MATERIAL_DTYPE
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E_INVALID, E_STATE = -1, -5
 RES = (256, 160)
 
 
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
-
-
 # ------------------------------------------------------------------ without a GPU
 def test_library_exports_the_three_entry_points_with_the_headers_signatures():
-    from rend3_b200.backend import ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
-    for decl in ("int r3_update_materials(r3_ctx*, const uint32_t* indices_or_null, const r3_material* records, uint32_t n);",
-                 "int r3_update_materials_device(r3_ctx*, const uint32_t* d_indices_or_null, const r3_material* d_records, uint32_t n);",
-                 "int r3_readback_materials(r3_ctx*, r3_material* out, uint32_t first, uint32_t n);"):
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        assert getattr(lib, name)(None, None, None, 0) == E_INVALID   # no context: rejected before anything is touched
+    check_declared_and_exported(("int r3_update_materials(r3_ctx*, const uint32_t* indices_or_null, const r3_material* records, uint32_t n);",
+                                 "int r3_update_materials_device(r3_ctx*, const uint32_t* d_indices_or_null, const r3_material* d_records, uint32_t n);",
+                                 "int r3_readback_materials(r3_ctx*, r3_material* out, uint32_t first, uint32_t n);"),
+                                (None, None, None, 0))
 
 
 def test_material_record_layout():
@@ -49,21 +35,6 @@ def test_material_record_layout():
     assert offsets["alpha_cutout"] == 200 and offsets["flags"] == 204
 
 
-class _NoCalls:
-    """Stands in for the library: any call through it fails the test."""
-
-    def __getattr__(self, name):
-        def call(*args):
-            raise AssertionError(f"{name} was called")
-        return call
-
-
-def _unbound_backend():
-    b = Backend.__new__(Backend)
-    b.lib, b.prefix, b.ctx = _NoCalls(), "r3_", None
-    return b
-
-
 @pytest.mark.parametrize("records,indices", [
     (np.zeros(4, np.uint8), None),                                     # bytes, not records
     (np.zeros((2, 2), MATERIAL_DTYPE), None),                          # 2-d records
@@ -75,12 +46,12 @@ def _unbound_backend():
 ], ids=["bytes", "2d-records", "length", "float-indices", "2d-indices", "negative", "wide"])
 def test_host_wrapper_rejects_bad_shapes_and_dtypes_before_calling(records, indices):
     with pytest.raises(AssertionError, match="records|indices"):
-        _unbound_backend().update_materials(records, indices)
+        unbound_backend().update_materials(records, indices)
 
 
 def test_device_wrapper_rejects_host_and_mistyped_tensors_before_calling():
     torch = pytest.importorskip("torch")
-    b = _unbound_backend()
+    b = unbound_backend()
     for records, indices in ((torch.zeros(2, 208, dtype=torch.uint8), None),          # a host tensor
                              (np.zeros(2, MATERIAL_DTYPE), None)):                     # a numpy array
         with pytest.raises(AssertionError):
@@ -124,9 +95,6 @@ def test_world_update_material_marks_exactly_the_stale_indices():
 
 
 # ------------------------------------------------------------------ GPU
-from test_object_presence import assert_same_ldr, cuda, settings, to_device  # noqa: E402
-
-
 def device_updates(b, indices, records):
     """(indices as int32 or None, records as uint8 (n, 208)) CUDA tensors on the context's stream."""
     rec = to_device(b, np.ascontiguousarray(records).view(np.uint8).reshape(-1, 208))
@@ -146,10 +114,8 @@ def test_gpu_updates_equal_the_full_upload_and_the_oracle(monkeypatch, samples, 
     the host form equal r3_set_materials of world.py's full table in every artefact, bit for bit; r3_readback_materials returns that
     table; with device batching the oracle, given the full table, agrees within the parity tolerance plus one rgba16f step (the
     blend routine's layers are stored in rgba16f)."""
-    import test_gpu_parity as parity
     from oracle import load_oracle_backend
     from rend3_b200.routines import BaseRenderGraph
-    from test_world_updates import assert_same_frame
 
     if host:
         monkeypatch.setenv("R3_HOST_BATCHING", "1")
@@ -157,7 +123,7 @@ def test_gpu_updates_equal_the_full_upload_and_the_oracle(monkeypatch, samples, 
         monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = MaterialWorld()
     ev = w.r.evaluate()
-    ctx = {"full": cuda(), "host": cuda(), "device": cuda()}
+    ctx = {"full": load_cuda_backend(0, parity_target=True), "host": load_cuda_backend(0, parity_target=True), "device": load_cuda_backend(0, parity_target=True)}
     graphs = {k: BaseRenderGraph(x) for k, x in ctx.items()}
     orc = None if host else load_oracle_backend()
     go = None if host else BaseRenderGraph(orc)
@@ -186,7 +152,7 @@ def test_gpu_updates_equal_the_full_upload_and_the_oracle(monkeypatch, samples, 
             assert np.array_equal(ctx["device"].readback_depth().view(np.uint32), orc.readback_depth().view(np.uint32)), f"{what}: oracle depth"
             # the blend routine stores every layer in rgba16f (at 1x too), so a 1e-7 difference in a layer's shaded colour can land on
             # the other side of a half-precision rounding: the bound is TOL plus one rgba16f step, as for 4x samples
-            parity.hdr_close(ctx["device"].readback_hdr_f32(), orc.readback_hdr_f32(), f"{what}: oracle hdr", True)
+            hdr_close(ctx["device"].readback_hdr_f32(), orc.readback_hdr_f32(), f"{what}: oracle hdr", True)
     for x in ctx.values():
         x.close()
     if orc is not None:
@@ -201,7 +167,7 @@ def test_gpu_dense_form_equals_sparse_form(count):
     rng = np.random.default_rng(count)
     mat = lambda u8: np.ascontiguousarray(u8).view(MATERIAL_DTYPE).reshape(-1)       # raw rows as records, padding included
     table = rng.integers(0, 256, (count, 208), dtype=np.uint8)
-    ctx = {k: cuda(False) for k in ("device-dense", "device-sparse", "host-dense", "host-sparse", "full")}
+    ctx = {k: load_cuda_backend(0, parity_target=False) for k in ("device-dense", "device-sparse", "host-dense", "host-sparse", "full")}
     for x in ctx.values():
         x.set_materials(mat(table))
     keep = []
@@ -233,12 +199,11 @@ def test_gpu_conservative_alpha_testing_is_safe(monkeypatch, samples):
     frames bit for bit.  Then a device update that turns the cutout material into a per-fragment cutout (alpha from a texture) discards
     in the shadow and forward passes exactly where the full-upload path does — and the frame differs from the one before."""
     from rend3_b200.routines import BaseRenderGraph
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = MaterialWorld(discard=False)
     ev = w.r.evaluate()
-    host, dev = cuda(), cuda()
+    host, dev = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gh, gd = BaseRenderGraph(host), BaseRenderGraph(dev)
     gh.add_to_graph(ev, RES, samples, settings())
     gd.add_to_graph(ev, RES, samples, settings())
@@ -274,13 +239,11 @@ def test_gpu_graph_frames_stay_one_launch(monkeypatch):
     import torch
 
     from rend3_b200.routines import BaseRenderGraph
-    from test_object_presence import on_stream
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = MaterialWorld(discard=False, blend=False)
     ev = w.r.evaluate()
-    graph_b, full = cuda(), cuda()
+    graph_b, full = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gg, gf = BaseRenderGraph(graph_b), BaseRenderGraph(full)
     gg.add_to_graph(ev, RES, 1, settings())
     gf.add_to_graph(ev, RES, 1, settings())
@@ -325,13 +288,12 @@ def test_gpu_transparency_change_by_the_documented_recipe(monkeypatch, device):
 
     from rend3_b200.routines import BaseRenderGraph
     from rend3_b200.world import BLEND
-    from test_world_updates import assert_same_frame
     from world_update_scene import sort_flags
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = MaterialWorld(blend=False)
     ev0 = w.r.evaluate()
-    recipe, full = cuda(), cuda()
+    recipe, full = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gr, gf = BaseRenderGraph(recipe), BaseRenderGraph(full)
     gr.add_to_graph(ev0, RES, 1, settings())
     gf.add_to_graph(ev0, RES, 1, settings())
@@ -370,18 +332,17 @@ def test_gpu_validation_growth_and_dropped_indices(monkeypatch):
     a misaligned record pointer, and out-of-range indices are dropped."""
     from rend3_b200.routines import BaseRenderGraph
     from rend3_b200.world import PbrMaterial
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = MaterialWorld(n_objects=300)
     ev = w.r.evaluate()
     n = len(ev.material_buffer)
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=True)
     one = ev.material_buffer[:1].copy()
     keep = [device_updates(b, None, one)]
     expect_error(E_STATE, b.update_materials_device, keep[0][1], None)                # empty table
     b.update_materials(one[:0])                                                      # n == 0: R3_OK on an empty table
-    ref = cuda()
+    ref = load_cuda_backend(0, parity_target=True)
     g, gref = BaseRenderGraph(b), BaseRenderGraph(ref)
     g.add_to_graph(ev, RES, 1, settings())
     gref.add_to_graph(ev, RES, 1, settings())

@@ -3,55 +3,25 @@ restatement (tests/mesh_deform_reference.py) of rebuilding each mesh from the ne
 the mesh spheres, the records with their sort locations, and whole frames against a context (and the oracle) fed the rebuilt world."""
 import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
 
 import mesh_deform_case as case
 import mesh_deform_reference as ref
+from harness import ROOT, assert_same_frame, check_declared_and_exported, expect_error, on_stream, to_device, unbound_backend
+from mesh_deform_case import bits, canon, canon_records
 from rend3_b200 import world
-from rend3_b200.backend import CUDA_LIB_PATH, Backend, R3Error
+from rend3_b200.backend import load_cuda_backend
 from rend3_b200.layouts import ATTR_ABSENT, DEFORM_NORMALS, DEFORM_TANGENTS, DEFORMABLE_MESH_DTYPE, OBJECT_DTYPE
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 f32 = np.float32
 E_INVALID, E_STATE = -1, -5
 RES = (256, 160)
 
 
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
-
-
-def bits(a):
-    return np.ascontiguousarray(a, dtype=f32).view(np.uint32)
-
-
-def canon(a):
-    """float32 bits with every NaN as 0x7FC00000: the bits of a NaN that arithmetic makes are not part of R15 (x86 and the GPU make
-    different default NaNs); copied values keep theirs and are compared as they are"""
-    a = np.array(a, dtype=f32)
-    a[np.isnan(a)] = np.float32(np.nan)
-    return a.view(np.uint32)
-
-
-def canon_records(r):
-    out = np.frombuffer(bytearray(np.ascontiguousarray(r).tobytes()), dtype=r.dtype)
-    for f in ("transform", "sphere_center", "sphere_radius"):
-        v = out[f]
-        v[np.isnan(v)] = np.float32(np.nan)
-    return out.tobytes()
-
-
 # ------------------------------------------------------------------ without a GPU
 def test_library_exports_the_entry_points_with_the_headers_signatures():
-    from rend3_b200.backend import ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
     decls = {
         "int r3_set_deformable_meshes(r3_ctx*, const r3_deformable_mesh* meshes, uint32_t n_meshes, const uint32_t* object_slots, "
         "const uint32_t* object_meshes, uint32_t n_objects);": (None, None, 0, None, None, 0),
@@ -59,11 +29,7 @@ def test_library_exports_the_entry_points_with_the_headers_signatures():
         "int r3_deform_meshes_device(r3_ctx*, const float* d_positions, uint64_t n_floats);": (None, None, ctypes.c_uint64(0)),
         "int r3_readback_deformable_mesh_spheres(r3_ctx*, float* out , uint32_t first, uint32_t n);": (None, None, 0, 0),
     }
-    for decl, args in decls.items():
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        assert getattr(lib, name)(*args) == E_INVALID   # no context: rejected before anything is touched
+    check_declared_and_exported(decls, decls.get)
 
 
 def test_deformable_mesh_layout_matches_c_header():
@@ -147,17 +113,8 @@ def test_mesh_sphere_agrees_with_bounding_sphere_from_mesh_where_that_is_exact()
     assert np.array_equal(bits(ref.mesh_sphere(np.zeros((0, 3), f32))), np.zeros(4, np.uint32))
 
 
-def _unbound_backend():
-    class _NoCalls:
-        def __getattr__(self, name):
-            raise AssertionError(f"{name} called")
-    b = Backend.__new__(Backend)
-    b.lib, b.prefix, b.ctx = _NoCalls(), "r3_", None
-    return b
-
-
 def test_wrappers_reject_bad_arrays_before_calling():
-    b = _unbound_backend()
+    b = unbound_backend()
     with pytest.raises(AssertionError, match="meshes"):
         b.set_deformable_meshes(np.zeros(4, np.uint32))
     with pytest.raises(AssertionError, match="one mesh per slot"):
@@ -172,12 +129,6 @@ def test_wrappers_reject_bad_arrays_before_calling():
 
 
 # ------------------------------------------------------------------ on the GPU
-def cuda(**kw):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, **kw)
-
-
 def check_state(b, w, new_pos, what):
     """the mesh buffer, per-mesh spheres, records and sort locations against the restatement; returns the expected arrays"""
     ev = w.ev
@@ -208,7 +159,7 @@ def test_gpu_edge_cases_equal_the_restatement(handedness, form):
     unreferenced vertices, r = inf, authored normals, no uv0, an empty mesh) deformed twice, the second time with NaN, inf and ±0
     positions, bit for bit against R15"""
     w = case.build_world(case.edge_specs(), handedness=handedness)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     b.set_deformable_meshes(w.meshes, w.slots, w.object_meshes)
     for k, specials in enumerate((False, True)):
@@ -217,7 +168,6 @@ def test_gpu_edge_cases_equal_the_restatement(handedness, form):
         if form == "host":
             b.deform_meshes(pos)
         else:
-            from test_object_presence import to_device
             d = to_device(b, pos)
             b.deform_meshes_device(d)
             b.sync()
@@ -233,7 +183,7 @@ def test_gpu_edge_cases_equal_the_restatement(handedness, form):
 def test_gpu_one_million_vertex_grid():
     """the ocean of tools/mesh_deform_cost.py: 1024 x 1024 vertices with uv0, 2 093 058 triangles, normals and tangents recomputed"""
     w = case.build_world([case.grid(1024, 1024, size=200.0)], objects_per_mesh=1, undeformed_objects=0, vectorised=True)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     b.set_deformable_meshes(w.meshes, w.slots, w.object_meshes)
     new_pos = positions_for(w, 1.3)
@@ -253,7 +203,7 @@ def test_gpu_identity_deform_leaves_the_uploaded_world():
         m = subdivided_cube_mesh(k, with_uv=uv)
         specs.append(case.MeshSpec(m.attributes[0][1], m.indices, next((a for s, a in m.attributes if s == 3), None)))
     w = case.build_world(specs, objects_per_mesh=5)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     b.set_deformable_meshes(w.meshes, w.slots, w.object_meshes)
     b.deform_meshes(np.concatenate(w.rest))
@@ -267,7 +217,7 @@ def test_gpu_identity_deform_leaves_the_uploaded_world():
 @pytest.mark.gpu
 def test_gpu_deform_then_move_takes_the_moves_location_with_the_new_mesh_sphere():
     w = case.build_world([case.grid(9, 9), case.fan(64)], objects_per_mesh=3)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     b.set_deformable_meshes(w.meshes, w.slots, w.object_meshes)
     new_pos = positions_for(w, 2.0)
@@ -304,18 +254,16 @@ def test_gpu_cloth_frames_in_one_graph_equal_the_rebuilt_world_and_the_oracle(mo
 
     import oracle
     from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings
-    from test_object_presence import on_stream, to_device
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
     w, specs = cloth_world()
-    dev, host = cuda(parity_target=True), cuda(parity_target=True)
+    dev, host = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gd, gh = BaseRenderGraph(dev), BaseRenderGraph(host)
     for b, g in ((dev, gd), (host, gh)):
         g.add_to_graph(w.ev, RES, 1, settings, movable_objects=True)
         b.set_deformable_meshes(w.meshes, w.slots, w.object_meshes)
-    full = cuda(parity_target=True)                  # fed the rebuilt world every frame, as the reference would be
+    full = load_cuda_backend(0, parity_target=True)                  # fed the rebuilt world every frame, as the reference would be
     gf = BaseRenderGraph(full)
     gf.add_to_graph(w.ev, RES, 1, settings)
     rest = np.concatenate(w.rest)
@@ -356,7 +304,7 @@ def test_gpu_validation_leaves_the_context_unchanged():
     import torch
 
     w = case.build_world([case.grid(6, 5), case.fan(16), case.grid(4, 4, uv=False)], objects_per_mesh=2)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     n_v = sum(int(m["vertex_count"]) for m in w.meshes)
     pos = np.concatenate(positions_for(w, 0.3))
@@ -394,7 +342,6 @@ def test_gpu_validation_leaves_the_context_unchanged():
 
     b.set_deformable_meshes(w.meshes, w.slots, w.object_meshes)
     expect_error(E_INVALID, b.deform_meshes, pos[:-1])                                # wrong n_floats
-    from test_object_presence import to_device
     d = to_device(b, pos)
     expect_error(E_INVALID, b.deform_meshes_device, d.data_ptr() + 2, 3 * n_v)         # misaligned
     expect_error(E_INVALID, b.deform_meshes_device, d.data_ptr(), 3 * n_v + 3)         # wrong n_floats

@@ -7,12 +7,15 @@ import os
 import numpy as np
 import pytest
 
+import animation_case
 import object_animation_case as cases
 from anim_reference import same_bits
+from harness import cull_and_batch_defined
+from object_animation_case import run, sort_info
 from object_anim_reference import node_matrix, pose_objects, posed_records, set_object_transform
 from rend3_b200 import glam
 from rend3_b200.animation import NodeChannels
-from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE, CB_CULL, R3Error
+from rend3_b200.backend import CAMERA_VIEWPORT, R3Error, load_cuda_backend
 from rend3_b200.layouts import ANIM_NODE_CHANNEL_DTYPE, ANIM_NODE_CLIP_DTYPE, ANIM_NODE_DTYPE, OBJECT_POSE_TARGET_DTYPE
 
 from oracle.objanim import load_objanim_oracle_backend
@@ -21,19 +24,6 @@ f32 = np.float32
 E_INVALID, E_STATE = -1, -5
 CASES = {"right": lambda: cases.case(seed=1), "left": lambda: cases.case(seed=2, left_handed=True),
          "many_jobs_left": lambda: cases.case(seed=3, left_handed=True, instances=300)}
-
-
-def sort_info(n):
-    return np.zeros(n, np.uint64), np.ones(n, np.uint8)
-
-
-def run(b, data, jobs, targets, records, loc):
-    b.set_objects(records)
-    b.set_object_sort_info(*sort_info(len(records)), loc)
-    data.upload(b)
-    b.set_object_pose_jobs(jobs, targets)
-    b.pose_objects()
-    return b.readback_objects(0, len(records))
 
 
 def words(r):
@@ -280,12 +270,6 @@ def test_object_animation_layouts_match_c_header():
 
 
 # ------------------------------------------------------------------ GPU
-def cuda():
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
 def test_gpu_pose_equals_oracle_bit_for_bit(name):
@@ -293,7 +277,7 @@ def test_gpu_pose_equals_oracle_bit_for_bit(name):
     orc = load_objanim_oracle_backend()
     want_r, want_l = run(orc, data, jobs, targets, records, loc)
     orc.close()
-    b = cuda()
+    b = load_cuda_backend(0)
     got_r, got_l = run(b, data, jobs, targets, records, loc)
     b.close()
     assert same_records(got_r, want_r) and same_bits(got_l, want_l)
@@ -309,7 +293,7 @@ def test_gpu_crowd_equals_oracle():
     orc = load_objanim_oracle_backend()
     want = run(orc, data, jobs, targets, records, loc)
     orc.close()
-    b = cuda()
+    b = load_cuda_backend(0)
     got = run(b, data, jobs, targets, records, loc)
     b.close()
     assert same_records(got[0], want[0]) and same_bits(got[1], want[1])
@@ -318,14 +302,14 @@ def test_gpu_crowd_equals_oracle():
 @pytest.mark.gpu
 def test_gpu_rejects_every_invalid_input_and_keeps_its_state():
     for check in (check_rejections, check_state_errors):
-        b = cuda()
+        b = load_cuda_backend(0)
         check(b)
         b.close()
     # a borrowed object buffer: every object-animation call but the readback is refused, and nothing changes
     import torch
 
     data, jobs, targets, records, loc = cases.case(seed=9)
-    b = cuda()
+    b = load_cuda_backend(0)
     b.set_objects(records)
     data.upload(b)
     b.set_object_pose_jobs(jobs, targets)
@@ -369,23 +353,6 @@ def cloud_scene(left, seed=11, n=4000, blend_pair=False):
     return rec, key, flags, rec["sphere_center"].copy(), data
 
 
-def cull_and_batch(b, n, vp=(1.0, 2.0, 3.0)):
-    from rend3_b200.routines import per_camera_header
-    from rend3_b200.scenes import cloud_camera
-
-    header = per_camera_header(cloud_camera(pull_back=12.0), CAMERA_VIEWPORT, (640, 360), 1, n)
-    b.object_uniform_upload(CAMERA_VIEWPORT, header, CB_BAKE | CB_CULL)
-    b.batch_objects(CAMERA_VIEWPORT, np.array(vp, dtype=f32))
-    bt, rg = b.readback_batches(CAMERA_VIEWPORT)
-    info = bt["object_culling_information"].copy()
-    for k in range(len(bt)):   # the entries past total_objects are not part of a batch (the device and the oracle leave different bytes)
-        info[k, int(bt[k]["total_objects"]):] = 0
-    # field by field: the batch records end in padding, which numpy's structured copies do not carry
-    batches = b"".join(bt[f].tobytes() for f in ("total_objects", "total_invocations", "batch_base_invocation")) + info.tobytes()
-    regions = b"".join(rg[f].tobytes() for f in rg.dtype.names)
-    return (b.readback_visible(CAMERA_VIEWPORT).tobytes(), b.readback_object_matrices(CAMERA_VIEWPORT, 0, n).tobytes(), batches, regions)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("left", [False, True], ids=["right", "left"])
 def test_gpu_cull_bake_after_pose_equals_oracle_and_host_posed_upload(monkeypatch, left):
@@ -399,7 +366,7 @@ def test_gpu_cull_bake_after_pose_equals_oracle_and_host_posed_upload(monkeypatc
         jobs, targets = data.pose_jobs([(0, t, 0)])
         want_r, want_l = posed_records(data.library, jobs, targets, rec, loc)
         slots = np.sort(targets["slot"])
-        for name, b in (("cuda", cuda()), ("oracle", load_objanim_oracle_backend()), ("host", cuda())):
+        for name, b in (("cuda", load_cuda_backend(0)), ("oracle", load_objanim_oracle_backend()), ("host", load_cuda_backend(0))):
             b.set_objects(rec)
             b.set_object_sort_info(key, flags, loc)
             if name == "host":
@@ -409,7 +376,7 @@ def test_gpu_cull_bake_after_pose_equals_oracle_and_host_posed_upload(monkeypatc
                 data.upload(b)
                 b.set_object_pose_jobs(jobs, targets)
                 b.pose_objects()
-            out[name] = cull_and_batch(b, n)
+            out[name] = cull_and_batch_defined(b, n)
             b.close()
         assert out["cuda"][:2] == out["oracle"][:2], f"t={t}: visible list / MV / MVP differ from the oracle"
         assert out["cuda"] == out["host"], f"t={t}: differs from the host-posed upload"
@@ -429,7 +396,7 @@ def test_gpu_batching_sorts_by_posed_locations(monkeypatch, host):
         monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     rec, key, flags, loc, data = cloud_scene(True, blend_pair=True)
     n = len(rec)
-    b, orc = cuda(), load_objanim_oracle_backend()
+    b, orc = load_cuda_backend(0), load_objanim_oracle_backend()
     for x in (b, orc):
         x.set_objects(rec)
         x.set_object_sort_info(key, flags, loc)
@@ -441,7 +408,7 @@ def test_gpu_batching_sorts_by_posed_locations(monkeypatch, host):
         for x in (b, orc):
             x.set_object_pose_jobs(*data.pose_jobs([(0, t, 0)]))
             x.pose_objects()
-        got, want = cull_and_batch(b, n, vp), cull_and_batch(orc, n, vp)
+        got, want = cull_and_batch_defined(b, n, vp), cull_and_batch_defined(orc, n, vp)
         assert got == want, f"t={t}: batches differ from the oracle"
         assert b.batching_info(CAMERA_VIEWPORT)["path"] == ("host" if host else "device")
         bt, _ = b.readback_batches(CAMERA_VIEWPORT)
@@ -457,11 +424,9 @@ def test_gpu_posed_frames_stay_one_graph():
     no early flush, graph == eager bit for bit, the oracle's shading within 1e-4.  Between frames 2 and 3 the graphed context gets an
     r3_update_objects of the posed slots with their stale add-time records, and still renders the posed frame."""
     from rend3_b200.animation import Animation, Node, ObjectAnimationData
-    from rend3_b200.backend import load_cuda_backend
     from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings
-    from test_animation import _posed_cube_world
 
-    ev, rec, skel = _posed_cube_world()
+    ev, rec, skel = animation_case._posed_cube_world()
     rng = np.random.default_rng(3)
     slots = rng.choice(len(ev.object_buffer), 40, replace=False)
     nodes, channels = [], {}

@@ -2,53 +2,24 @@
 r3_update_objects + r3_update_object_sort_info (bit for bit) and the CPU oracle given the states as full uploads (within the parity
 tolerance), plus the blend routine's bookkeeping, the frame graph, the dense form's bit words and the calls' validation."""
 import ctypes
-import os
-import re
 
 import numpy as np
 import pytest
 
+from harness import (assert_same_frame, assert_same_ldr, check_declared_and_exported, cull_and_batch, expect_error, hdr_close,
+                     settings, to_device, unbound_backend)
 from object_presence_case import pool_state, pool_world, state_eval, switch_script, update_path
-from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE, CB_CULL, CUDA_LIB_PATH, Backend, R3Error
+from rend3_b200.backend import CAMERA_VIEWPORT, load_cuda_backend
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E_INVALID, E_STATE = -1, -5
 RES = (256, 160)
 
 
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
-
-
 # ------------------------------------------------------------------ without a GPU
 def test_library_exports_both_entry_points_with_the_headers_signatures():
-    from rend3_b200.backend import ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
-    for decl in ("int r3_set_objects_enabled(r3_ctx*, const uint32_t* slots_or_null, const uint8_t* enabled, uint32_t n);",
-                 "int r3_set_objects_enabled_device(r3_ctx*, const uint32_t* d_slots_or_null, const uint8_t* d_enabled, uint32_t n);"):
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        assert getattr(lib, name)(None, None, None, 0) == E_INVALID   # no context: rejected before anything is touched
-
-
-class _NoCalls:
-    """Stands in for the library: any call through it fails the test."""
-
-    def __getattr__(self, name):
-        def call(*args):
-            raise AssertionError(f"{name} was called")
-        return call
-
-
-def _unbound_backend():
-    b = Backend.__new__(Backend)
-    b.lib, b.prefix, b.ctx = _NoCalls(), "r3_", None
-    return b
+    check_declared_and_exported(("int r3_set_objects_enabled(r3_ctx*, const uint32_t* slots_or_null, const uint8_t* enabled, uint32_t n);",
+                                 "int r3_set_objects_enabled_device(r3_ctx*, const uint32_t* d_slots_or_null, const uint8_t* d_enabled, uint32_t n);"),
+                                (None, None, None, 0))
 
 
 @pytest.mark.parametrize("enabled,slots", [
@@ -63,12 +34,12 @@ def _unbound_backend():
 ], ids=["2d-flags", "float-flags", "int32-flags", "length", "float-slots", "2d-slots", "negative", "wide"])
 def test_host_wrapper_rejects_bad_shapes_and_dtypes_before_calling(enabled, slots):
     with pytest.raises(AssertionError, match="enabled|slots"):
-        _unbound_backend().set_objects_enabled(enabled, slots)
+        unbound_backend().set_objects_enabled(enabled, slots)
 
 
 def test_device_wrapper_rejects_host_and_mistyped_tensors_before_calling():
     torch = pytest.importorskip("torch")
-    b = _unbound_backend()
+    b = unbound_backend()
     for enabled, slots in ((torch.ones(4, dtype=torch.uint8), None),                  # a host tensor
                            (np.ones(4, np.uint8), None)):                             # a numpy array
         with pytest.raises(AssertionError):
@@ -113,26 +84,6 @@ def test_pool_state_equals_world_add_and_remove():
 
 
 # ------------------------------------------------------------------ GPU
-def cuda(parity=True):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, parity_target=parity)
-
-
-def on_stream(b, fn):
-    import torch
-
-    with torch.cuda.stream(torch.cuda.ExternalStream(b.stream())):
-        return fn()
-
-
-def to_device(b, array, dtype=None):
-    import torch
-
-    host = torch.from_numpy(np.ascontiguousarray(array).copy())
-    return on_stream(b, lambda: host.to("cuda", dtype=dtype, non_blocking=False))
-
-
 def device_entries(b, present, slots):
     """(slots as int32, enabled as uint8) CUDA tensors on the context's stream; slots None stays None (dense)."""
     flags = np.ascontiguousarray(present[slots] if slots is not None else present).astype(np.uint8)
@@ -145,16 +96,6 @@ def same_fields(a, b):
     return len(a) == len(b) and all(a[f].tobytes() == b[f].tobytes() for f in a.dtype.names)
 
 
-def assert_same_ldr(a, b, what):
-    assert a.readback_ldr().tobytes() == b.readback_ldr().tobytes(), f"{what}: LDR differs"
-
-
-def settings():
-    from rend3_b200.routines import BaseRenderGraphSettings
-
-    return BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0), ambient_color=(0.02, 0.02, 0.02, 1.0))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("samples,host", [(1, False), (4, False), (1, True)], ids=["x1", "x4", "x1-host-batching"])
 def test_gpu_switches_equal_the_update_path_and_the_oracle(monkeypatch, samples, host):
@@ -162,10 +103,8 @@ def test_gpu_switches_equal_the_update_path_and_the_oracle(monkeypatch, samples,
     word edges, one visible slot off / on / off in successive frames.  The device form (sparse lists) and the host form (dense) equal a
     context fed the same states through r3_update_objects + r3_update_object_sort_info in every artefact, bit for bit; with device
     batching the oracle, given each state as a full upload, agrees within the parity tolerance."""
-    import test_gpu_parity as parity
     from oracle import load_oracle_backend
     from rend3_b200.routines import BaseRenderGraph
-    from test_world_updates import assert_same_frame
 
     if host:
         monkeypatch.setenv("R3_HOST_BATCHING", "1")
@@ -173,7 +112,7 @@ def test_gpu_switches_equal_the_update_path_and_the_oracle(monkeypatch, samples,
         monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = pool_world(n_objects=2000)
     ev, n = w.ev, len(w.ev.object_buffer)
-    ctx = {"update": cuda(), "host": cuda(), "device": cuda()}
+    ctx = {"update": load_cuda_backend(0, parity_target=True), "host": load_cuda_backend(0, parity_target=True), "device": load_cuda_backend(0, parity_target=True)}
     graphs = {k: BaseRenderGraph(x) for k, x in ctx.items()}
     orc = None if host else load_oracle_backend()
     go = None if host else BaseRenderGraph(orc)
@@ -201,7 +140,7 @@ def test_gpu_switches_equal_the_update_path_and_the_oracle(monkeypatch, samples,
             for cam in [CAMERA_VIEWPORT] + list(range(len(ev.shadows))):
                 assert np.array_equal(ctx["device"].readback_visible(cam), orc.readback_visible(cam)), f"frame {frame} camera {cam}: oracle"
             assert np.array_equal(ctx["device"].readback_depth().view(np.uint32), orc.readback_depth().view(np.uint32)), f"frame {frame}: oracle depth"
-            parity.hdr_close(ctx["device"].readback_hdr_f32(), orc.readback_hdr_f32(), f"frame {frame}: oracle hdr", samples != 1)
+            hdr_close(ctx["device"].readback_hdr_f32(), orc.readback_hdr_f32(), f"frame {frame}: oracle hdr", samples != 1)
         if frame == 2:
             assert ctx["device"].visible_count(CAMERA_VIEWPORT) == 0, "all off"
     for x in ctx.values():
@@ -216,12 +155,11 @@ def test_gpu_despawned_object_leaves_the_predicted_pass_and_a_spawned_one_joins_
     X is not drawn (vs_main's disabled-object test).  Frame N+1 spawns it again: the predicted list (frame N's) lacks X and the residual
     pass draws it.  Depth is compared with the frames before, images with the update path, bit for bit."""
     from rend3_b200.routines import BaseRenderGraph
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = pool_world(n_objects=600, blend=False)
     ev, n = w.ev, len(w.ev.object_buffer)
-    dev, upd = cuda(), cuda()
+    dev, upd = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gd, gu = BaseRenderGraph(dev), BaseRenderGraph(upd)
     for g in (gd, gu):
         g.add_to_graph(ev, RES, 1, settings())
@@ -257,7 +195,6 @@ def test_gpu_switching_frames_stay_one_graph(monkeypatch):
     from rend3_b200.animation import Animation, Node, NodeChannels, ObjectAnimationData
     from rend3_b200.routines import BaseRenderGraph
     from rend3_b200.scenes import cube_field_scene
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     res = (256, 144)
@@ -275,7 +212,7 @@ def test_gpu_switching_frames_stay_one_graph(monkeypatch):
         nodes.append(Node(None, t, anim_cases._unit_quat(rng), (0.7, 0.7, 0.7), [(int(s), ms[s, :3].copy(), np.float32(ms[s, 3]))]))
         channels[i] = NodeChannels(anim_cases.key_track([0.0, 2.0], [t, t + rng.uniform(-1, 1, 3).astype(np.float32)]))
     data = ObjectAnimationData(nodes, [Animation(channels, 2.0)], left_handed=True)
-    graph_b, eager_b = cuda(), cuda()
+    graph_b, eager_b = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     graphs = {id(x): BaseRenderGraph(x) for x in (graph_b, eager_b)}
     for x in (graph_b, eager_b):
         graphs[id(x)].upload_world(ev, device_shadow_cameras=True, movable_objects=True)
@@ -317,7 +254,6 @@ def test_gpu_blend_routine_bookkeeping(monkeypatch):
     it on.  Device form: with key-2 slots, none present, the image equals the one the exact rule gives, bit for bit, though the routine
     runs (the recorded frame flushes).  After r3_set_object_sort_info the exact rule is back."""
     from rend3_b200.routines import BaseRenderGraph
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = pool_world(n_objects=800, blend=True)
@@ -326,7 +262,7 @@ def test_gpu_blend_routine_bookkeeping(monkeypatch):
     assert len(blend) >= 2
     present = np.ones(n, dtype=bool)
     present[blend[1:]] = False                                           # one key-2 object present
-    exact, dev = cuda(), cuda()
+    exact, dev = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     ge, gd = BaseRenderGraph(exact), BaseRenderGraph(dev)
 
     def frame(g, b, **kw):
@@ -366,20 +302,6 @@ def cloud(n, seed=3):
     return rec, key, flags, rec["sphere_center"].copy()
 
 
-def cull_and_batch(b, n, batch=True):
-    from rend3_b200.routines import per_camera_header
-    from rend3_b200.scenes import cloud_camera
-
-    header = per_camera_header(cloud_camera(pull_back=12.0), CAMERA_VIEWPORT, (640, 360), 1, n)
-    b.object_uniform_upload(CAMERA_VIEWPORT, header, CB_BAKE | CB_CULL)
-    out = [b.readback_visible(CAMERA_VIEWPORT).tobytes(), b.readback_object_matrices(CAMERA_VIEWPORT, 0, n).tobytes()]
-    if batch:
-        b.batch_objects(CAMERA_VIEWPORT, np.array([1.0, 2.0, 3.0], dtype=np.float32))
-        bt, rg = b.readback_batches(CAMERA_VIEWPORT)
-        out += [bt.tobytes(), rg.tobytes()]
-    return out
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", [1000, 1024, 33])
 def test_gpu_dense_form_equals_sparse_form(monkeypatch, n):
@@ -388,7 +310,7 @@ def test_gpu_dense_form_equals_sparse_form(monkeypatch, n):
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     rec, key, flags, loc = cloud(n)
     rng = np.random.default_rng(n)
-    ctx = {"dense": cuda(False), "sparse": cuda(False), "update": cuda(False)}
+    ctx = {"dense": load_cuda_backend(0, parity_target=False), "sparse": load_cuda_backend(0, parity_target=False), "update": load_cuda_backend(0, parity_target=False)}
     for x in ctx.values():
         x.set_objects(rec)
         x.set_object_sort_info(key, flags, loc)
@@ -424,7 +346,7 @@ def test_gpu_without_sort_info_the_enabled_bits_decide(monkeypatch):
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     n = 1000
     rec, _, _, _ = cloud(n, seed=9)
-    ctx = {"host": cuda(False), "device": cuda(False), "update": cuda(False)}
+    ctx = {"host": load_cuda_backend(0, parity_target=False), "device": load_cuda_backend(0, parity_target=False), "update": load_cuda_backend(0, parity_target=False)}
     for x in ctx.values():
         x.set_objects(rec)
     rng = np.random.default_rng(1)
@@ -454,13 +376,13 @@ def test_gpu_validation_and_dropped_slots(monkeypatch):
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     n = 500
     rec, key, flags, loc = cloud(n, seed=4)
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     one = np.ones(1, np.uint8)
     b.set_objects_enabled(np.zeros(0, np.uint8))                                    # n == 0: R3_OK before any state exists
     expect_error(E_STATE, b.set_objects_enabled, one, np.array([0]))
     d_one = to_device(b, one)
     expect_error(E_STATE, b.set_objects_enabled_device, d_one, None)
-    ref = cuda(False)                                                               # the same frames without the rejected calls
+    ref = load_cuda_backend(0, parity_target=False)                                                               # the same frames without the rejected calls
     for x in (b, ref):
         x.set_objects(rec)
         x.set_object_sort_info(key, flags, loc)

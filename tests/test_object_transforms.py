@@ -1,29 +1,19 @@
 """Objects moved in bulk — r3_set_object_mesh_spheres, r3_set_object_transforms, r3_set_object_transforms_device — against the numpy
 float32 restatement of rule R12's object half (tests/object_transform_case.py), the CPU oracle and, on the GPU, a context fed the same
 bytes through r3_update_objects + r3_update_object_sort_info."""
-import ctypes
-import os
-import re
-
 import numpy as np
 import pytest
 
 import object_transform_case as cases
+from harness import assert_same_frame, check_declared_and_exported, cull_and_batch_defined, expect_error, on_stream, to_device
 from object_anim_reference import set_object_transform
-from object_transform_case import move_objects, moved_records, same_bits, same_records
-from rend3_b200.backend import CAMERA_VIEWPORT, CUDA_LIB_PATH, R3Error
+from object_transform_case import apply, move_objects, moved_records, same_bits, same_records
+from rend3_b200.backend import CAMERA_VIEWPORT, load_cuda_backend
 
 from oracle.objtransforms import load_objtransforms_oracle_backend
 
 f32 = np.float32
 E_INVALID, E_STATE = -1, -5
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
 
 
 def setup_world(b, rec, key, flags, loc, ms):
@@ -130,52 +120,13 @@ def test_oracle_rejections_and_state_rules():
 
 
 def test_library_exports_the_three_entry_points_with_the_headers_signatures():
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S)
-    header = re.sub(r"\s+", " ", header)
-    for decl in ("int r3_set_object_mesh_spheres(r3_ctx*, const uint32_t* slots_or_null, const float* center_radius , uint32_t n);",
-                 "int r3_set_object_transforms(r3_ctx*, const uint32_t* slots_or_null, const float* mat4s , uint32_t n);",
-                 "int r3_set_object_transforms_device(r3_ctx*, const uint32_t* d_slots_or_null, const float* d_mat4s, uint32_t n);"):
-        assert decl in header, decl
-        assert hasattr(lib, decl.split("(")[0].split()[-1])
-    # no context: the calls fail with R3_E_INVALID instead of touching anything
-    assert lib.r3_set_object_transforms(None, None, None, 0) == E_INVALID
-    assert lib.r3_set_object_transforms_device(None, None, None, 0) == E_INVALID
-    assert lib.r3_set_object_mesh_spheres(None, None, None, 0) == E_INVALID
+    check_declared_and_exported(("int r3_set_object_mesh_spheres(r3_ctx*, const uint32_t* slots_or_null, const float* center_radius , uint32_t n);",
+                                 "int r3_set_object_transforms(r3_ctx*, const uint32_t* slots_or_null, const float* mat4s , uint32_t n);",
+                                 "int r3_set_object_transforms_device(r3_ctx*, const uint32_t* d_slots_or_null, const float* d_mat4s, uint32_t n);"),
+                                (None, None, None, 0))
 
 
 # ------------------------------------------------------------------ GPU
-def cuda(parity=False):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, parity_target=parity)
-
-
-def on_stream(b, fn):
-    """Run torch work on the context's stream, so that it is ordered before the library's next kernel."""
-    import torch
-
-    with torch.cuda.stream(torch.cuda.ExternalStream(b.stream())):
-        return fn()
-
-
-def to_device(b, array, dtype=None):
-    import torch
-
-    host = torch.from_numpy(np.ascontiguousarray(array).copy())
-    return on_stream(b, lambda: host.to("cuda", dtype=dtype, non_blocking=False))
-
-
-def apply(b, form, mats, slots):
-    """One move through the host or the device form; returns what must stay alive until the stream has drained."""
-    if form == "host":
-        b.set_object_transforms(mats, slots)
-        return None
-    keep = (to_device(b, mats.reshape(-1, 16)), None if slots is None else to_device(b, np.asarray(slots, dtype=np.uint32).view(np.int32)))
-    b.set_object_transforms_device(keep[0], keep[1])
-    return keep
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("form", ["host", "device"])
 def test_gpu_records_equal_the_oracle(form):
@@ -188,7 +139,7 @@ def test_gpu_records_equal_the_oracle(form):
     mats[:len(em)] = em
     ms[:len(em)] = es
     rng = np.random.default_rng(17)
-    b, orc = cuda(), load_objtransforms_oracle_backend()
+    b, orc = load_cuda_backend(0, parity_target=False), load_objtransforms_oracle_backend()
     for x in (b, orc):
         setup_world(x, rec, key, flags, loc, ms)
     steps = [(k, None) for k in (1, 31, 32, 33, 1000, n)]
@@ -215,14 +166,13 @@ def test_gpu_records_equal_the_oracle(form):
 def test_gpu_cull_bake_after_moves_equals_oracle_and_the_update_path(monkeypatch):
     """Visible list and every MV / MVP word after a move == the oracle's == a context fed the same bytes through r3_update_objects +
     r3_update_object_sort_info, for both forms; a slot goes affine -> non-affine -> affine, and a disabled slot moves and stays disabled."""
-    from test_object_animation import cull_and_batch
-
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     n = 4000
     rec, key, flags, loc, ms = cases.world(n, seed=11)
     disabled = int(np.flatnonzero(rec["enabled"] == 0)[0])
     rng = np.random.default_rng(23)
-    ctx = {"host": cuda(), "device": cuda(), "update": cuda(), "oracle": load_objtransforms_oracle_backend()}
+    ctx = {"host": load_cuda_backend(0, parity_target=False), "device": load_cuda_backend(0, parity_target=False),
+           "update": load_cuda_backend(0, parity_target=False), "oracle": load_objtransforms_oracle_backend()}
     for x in ctx.values():
         setup_world(x, rec, key, flags, loc, ms)
     cur_r, cur_l = rec, loc
@@ -241,7 +191,7 @@ def test_gpu_cull_bake_after_moves_equals_oracle_and_the_update_path(monkeypatch
                 x.update_object_sort_info(slots, key[slots], flags[slots], cur_l[slots])
             else:
                 keep.append(apply(x, "device" if name == "device" else "host", mats, slots))
-            out[name] = cull_and_batch(x, n)
+            out[name] = cull_and_batch_defined(x, n)
         for name in ("host", "device"):
             assert out[name][:2] == out["oracle"][:2], f"step {step}, {name} form: visible list / MV / MVP differ from the oracle"
             assert out[name] == out["update"], f"step {step}, {name} form: differs from the update path"
@@ -260,8 +210,6 @@ def test_gpu_cull_bake_after_moves_equals_oracle_and_the_update_path(monkeypatch
 def test_gpu_batching_sorts_by_moved_locations(monkeypatch, host):
     """Batch and region tables == the oracle's on both batching paths while two back-to-front blend objects swap places by being moved
     with the device form; the host path takes the moved locations from the device in the drain it makes for the visible list."""
-    from test_object_animation import cull_and_batch
-
     if host:
         monkeypatch.setenv("R3_HOST_BATCHING", "1")
     else:
@@ -271,7 +219,7 @@ def test_gpu_batching_sorts_by_moved_locations(monkeypatch, host):
     pair = np.array([100, 2000], dtype=np.uint32)
     rec["enabled"][pair] = 1
     key[pair], flags[pair] = 2, 1 | 4
-    b, orc = cuda(), load_objtransforms_oracle_backend()
+    b, orc = load_cuda_backend(0, parity_target=False), load_objtransforms_oracle_backend()
     for x in (b, orc):
         setup_world(x, rec, key, flags, loc, ms)
     vp = (0.0, 0.0, -30.0)
@@ -281,7 +229,7 @@ def test_gpu_batching_sorts_by_moved_locations(monkeypatch, host):
         mats[:, 14] = z
         keep.append(apply(b, "device", mats, pair))
         orc.set_object_transforms(mats, pair)
-        got, want = cull_and_batch(b, n, vp), cull_and_batch(orc, n, vp)
+        got, want = cull_and_batch_defined(b, n, vp), cull_and_batch_defined(orc, n, vp)
         assert got == want, f"z={z}: batches differ from the oracle"
         assert b.batching_info(CAMERA_VIEWPORT)["path"] == ("host" if host else "device")
         bt, _ = b.readback_batches(CAMERA_VIEWPORT)
@@ -297,13 +245,13 @@ def test_gpu_rejections_dropped_slots_and_growth():
     drops out-of-range slots and changes nothing else; after r3_resize_objects a new slot (zero mesh sphere until set) can be moved."""
     import torch
 
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     check_rejections(b)
     b.close()
     n = 1000
     rec, key, flags, loc, ms = cases.world(n)
     mats = cases.seeded_matrices(64)
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     setup_world(b, rec, key, flags, loc, ms)
     slots = np.array([5, n, 77, 0xFFFFFFFF, n + 31, 999], dtype=np.uint32)
     keep = apply(b, "device", mats[:6], slots)
@@ -349,7 +297,6 @@ def test_gpu_moved_frames_stay_one_graph():
     from rend3_b200.animation import Animation, Node, NodeChannels, ObjectAnimationData
     from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings
     from rend3_b200.scenes import cube_field_scene
-    from test_world_updates import assert_same_frame
 
     res = (256, 144)
     ev = cube_field_scene(n_objects=300, seed=7, resolution=res, n_dir_lights=2, shadow_resolution=256)
@@ -366,7 +313,8 @@ def test_gpu_moved_frames_stay_one_graph():
         channels[i] = NodeChannels(anim_cases.key_track([0.0, 2.0], [t, t + rng.uniform(-1, 1, 3).astype(f32)]))
     data = ObjectAnimationData(nodes, [Animation(channels, 2.0)], left_handed=True)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
-    graph_b, eager_b, update_b, orc = cuda(True), cuda(True), cuda(True), load_objtransforms_oracle_backend()
+    graph_b, eager_b, update_b = (load_cuda_backend(0, parity_target=True) for _ in range(3))
+    orc = load_objtransforms_oracle_backend()
     graphs = {id(x): BaseRenderGraph(x) for x in (graph_b, eager_b, update_b, orc)}
     for x in (graph_b, eager_b, update_b, orc):
         dsc = x is not orc

@@ -9,11 +9,11 @@ import re
 import numpy as np
 import pytest
 
+from harness import ROOT, assert_same_frame, check_declared_and_exported, cull_and_batch, expect_error, settings, to_device, unbound_backend
 from object_variant_case import PARTNER_OPAQUE, VariantWorld, expected_bound, update_path
-from rend3_b200.backend import CAMERA_VIEWPORT, CUDA_LIB_PATH, Backend, R3Error
+from rend3_b200.backend import CAMERA_VIEWPORT, load_cuda_backend
 from rend3_b200.layouts import OBJECT_VARIANT_DTYPE, VARIANT_GROUP_DTYPE, VARIANT_NONE
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E_INVALID, E_STATE = -1, -5
 RES = (256, 160)
 DECLS = (
@@ -24,24 +24,9 @@ DECLS = (
 )
 
 
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
-
-
 # ------------------------------------------------------------------ without a GPU
 def test_library_exports_the_four_entry_points_with_the_headers_signatures():
-    from rend3_b200.backend import ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
-    for decl in DECLS:
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        n_args = decl.count(",") + 1
-        assert getattr(lib, name)(*([None] * (n_args - 1)), 0) == E_INVALID   # no context: rejected before anything is touched
+    check_declared_and_exported(DECLS, lambda decl: [None] * decl.count(",") + [0])
 
 
 def test_variant_record_layout_equals_the_c_header():
@@ -56,19 +41,6 @@ def test_variant_record_layout_equals_the_c_header():
             assert f"offsetof(r3_object_variant, {name}) == {offsets[name]}" in text, name
 
 
-class _NoCalls:
-    def __getattr__(self, name):
-        def call(*args):
-            raise AssertionError(f"{name} was called")
-        return call
-
-
-def _unbound_backend():
-    b = Backend.__new__(Backend)
-    b.lib, b.prefix, b.ctx = _NoCalls(), "r3_", None
-    return b
-
-
 @pytest.mark.parametrize("choices,slots", [
     (np.zeros((4, 2), np.uint32), None),                        # 2-d choices
     (np.zeros(4, np.float32), None),                            # float choices
@@ -78,12 +50,12 @@ def _unbound_backend():
 ], ids=["2d", "float", "length", "negative", "wide"])
 def test_host_wrappers_reject_bad_shapes_and_dtypes_before_calling(choices, slots):
     with pytest.raises(AssertionError, match="choices|slots"):
-        _unbound_backend().switch_object_variants(choices, slots)
+        unbound_backend().switch_object_variants(choices, slots)
 
 
 def test_set_and_device_wrappers_reject_bad_arguments_before_calling():
     torch = pytest.importorskip("torch")
-    b = _unbound_backend()
+    b = unbound_backend()
     v, g = np.zeros(2, OBJECT_VARIANT_DTYPE), np.zeros(1, VARIANT_GROUP_DTYPE)
     for args in ((np.zeros(2, np.uint32), g), (v, np.zeros(1, np.uint32)), (v, g, np.arange(3), np.zeros(2)), (v, g, np.arange(2), None)):
         with pytest.raises(AssertionError):
@@ -128,32 +100,12 @@ def test_expected_state_equals_world_readd_object():
 
 
 # ------------------------------------------------------------------ GPU
-def cuda(parity=True):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, parity_target=parity)
-
-
-def to_device(b, array):
-    import torch
-
-    host = torch.from_numpy(np.ascontiguousarray(array).copy())
-    with torch.cuda.stream(torch.cuda.ExternalStream(b.stream())):
-        return host.to("cuda", non_blocking=False)
-
-
 def u32_tensor(b, a):
     return to_device(b, np.asarray(a, dtype=np.uint32).view(np.int32))
 
 
 def same_fields(a, b):
     return len(a) == len(b) and all(a[f].tobytes() == b[f].tobytes() for f in a.dtype.names)
-
-
-def settings():
-    from rend3_b200.routines import BaseRenderGraphSettings
-
-    return BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0), ambient_color=(0.02, 0.02, 0.02, 1.0))
 
 
 def prepare(graph, b, w, samples=1):
@@ -172,7 +124,6 @@ def test_gpu_switches_equal_the_update_path_and_the_oracle(monkeypatch, samples,
     device batching the oracle, given the re-added world, gives the same visible lists and depth."""
     from oracle import load_oracle_backend
     from rend3_b200.routines import BaseRenderGraph
-    from test_world_updates import assert_same_frame
 
     if host:
         monkeypatch.setenv("R3_HOST_BATCHING", "1")
@@ -180,7 +131,7 @@ def test_gpu_switches_equal_the_update_path_and_the_oracle(monkeypatch, samples,
         monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = VariantWorld(n_objects=2000)
     n = w.n
-    ctx = {"update": cuda(), "host": cuda(), "device": cuda()}
+    ctx = {"update": load_cuda_backend(0, parity_target=True), "host": load_cuda_backend(0, parity_target=True), "device": load_cuda_backend(0, parity_target=True)}
     graphs = {k: BaseRenderGraph(x) for k, x in ctx.items()}
     for k, x in ctx.items():
         prepare(graphs[k], x, w, samples)
@@ -233,13 +184,12 @@ def test_gpu_device_picked_lods_stay_one_graph(monkeypatch):
     import torch
 
     from rend3_b200.routines import BaseRenderGraph
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = VariantWorld(n_objects=1500, blend=False, partner=PARTNER_OPAQUE)
     assert not (w.variants["material_key"] == 2).any()
     n = w.n
-    graph_b, eager_b = cuda(), cuda()
+    graph_b, eager_b = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     graphs = {id(x): BaseRenderGraph(x) for x in (graph_b, eager_b)}
     for x in (graph_b, eager_b):
         prepare(graphs[id(x)], x, w)
@@ -275,7 +225,7 @@ def test_gpu_invocation_bound_takes_the_groups_largest_level(monkeypatch):
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = VariantWorld(n_objects=1200, blend=False, partner=PARTNER_OPAQUE)
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     g = BaseRenderGraph(b)
     g.add_to_graph(w.ev, RES, 1, settings())
     b.set_object_mesh_spheres(w.mesh_spheres)
@@ -310,7 +260,7 @@ def test_gpu_blend_routine_bookkeeping(monkeypatch):
     w = VariantWorld(n_objects=600, blend=False, partner={0: 2, 1: 0, 2: 0, 3: 1})   # group 0 swaps to blend
     opaque0 = np.flatnonzero(w.slot_groups == 0)
     vis = None
-    hb, db = cuda(), cuda()
+    hb, db = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gh, gd = BaseRenderGraph(hb), BaseRenderGraph(db)
     for g, b in ((gh, hb), (gd, db)):
         prepare(g, b, w)
@@ -352,22 +302,9 @@ def cloud_world(n):
     return rec, key, flags, rec["sphere_center"].copy(), variants, groups
 
 
-def cull_and_batch(b, n):
-    from rend3_b200.backend import CB_BAKE, CB_CULL
-    from rend3_b200.routines import per_camera_header
-    from rend3_b200.scenes import cloud_camera
-
-    header = per_camera_header(cloud_camera(pull_back=12.0), CAMERA_VIEWPORT, (640, 360), 1, n)
-    b.object_uniform_upload(CAMERA_VIEWPORT, header, CB_BAKE | CB_CULL)
-    out = [b.readback_visible(CAMERA_VIEWPORT).tobytes(), b.readback_object_matrices(CAMERA_VIEWPORT, 0, n).tobytes()]
-    b.batch_objects(CAMERA_VIEWPORT, np.array([1.0, 2.0, 3.0], dtype=np.float32))
-    bt, rg = b.readback_batches(CAMERA_VIEWPORT)
-    return out + [bt.tobytes(), rg.tobytes()]
-
-
 def cloud_context(n, mesh_words):
     rec, key, flags, loc, variants, groups = cloud_world(n)
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     b.set_objects(rec)
     b.set_object_sort_info(key, flags, loc)
     b.set_mesh_buffer(mesh_words)
@@ -420,7 +357,7 @@ def test_gpu_validation_leaves_the_context_unchanged(monkeypatch):
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     n = 500
     words = np.arange(4096, dtype=np.uint32) % 3
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     rec, key, flags, loc, variants, groups = cloud_world(n)
     one = np.zeros(1, np.uint32)
     expect_error(E_STATE, b.set_object_variants, variants, groups, np.array([0]), one)          # before r3_set_objects

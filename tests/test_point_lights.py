@@ -10,10 +10,11 @@ import tempfile
 import numpy as np
 import pytest
 
+from harness import same_bytes
 from oracle.points import load_points_oracle_backend
 from point_light_case import apply_to_world, as_update, records, same_buffer, sequence
 from rend3_b200 import glam
-from rend3_b200.backend import ENTRY_POINTS, R3Error
+from rend3_b200.backend import ENTRY_POINTS, R3Error, load_cuda_backend
 from rend3_b200.layouts import POINT_LIGHT_SOURCE_DTYPE
 from rend3_b200.world import BLEND, LEFT, RIGHT, Camera, DirectionalLight, MeshBuilder, Object, PbrMaterial, PointLight, Renderer
 
@@ -144,15 +145,9 @@ def check_switching(b):
 
 
 # ------------------------------------------------------------------ GPU
-def cuda(parity=False):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, parity_target=parity)
-
-
 @pytest.mark.gpu
 def test_gpu_evaluated_buffer_equals_world_host_form():
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     check_sequences(b)
     b.close()
 
@@ -176,7 +171,7 @@ def device_update(b, ops, extra_handles=()):
 @pytest.mark.gpu
 def test_gpu_evaluated_buffer_equals_world_device_form():
     """The same sequences through the device form over a table sized up front; out-of-range handles are dropped, the others written."""
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     for seed in range(6):
         steps = sequence(seed)
         size = max(h for ops in steps for h, _ in ops) + 1
@@ -198,14 +193,14 @@ def test_gpu_evaluated_buffer_equals_world_device_form():
 
 @pytest.mark.gpu
 def test_gpu_rejects_invalid_calls_and_keeps_its_state():
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     check_rejections(b)
     b.close()
 
 
 @pytest.mark.gpu
 def test_gpu_set_point_lights_and_the_sources_replace_each_other():
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     check_switching(b)
     b.close()
 
@@ -270,10 +265,6 @@ def frame_outputs(b):
     return b.readback_hdr_f16().copy(), b.readback_hdr_f32().copy(), b.readback_depth().copy()
 
 
-def same_bits(a, b):
-    return a.shape == b.shape and np.array_equal(np.ascontiguousarray(a).view(np.uint8), np.ascontiguousarray(b).view(np.uint8))
-
-
 ENQUEUE_ONLY = {"frame_begin", "frame_end", "clear_shadow_atlas", "set_frame_uniforms", "evaluate_shadow_cameras", "shadow_uniform_upload",
                 "object_uniform_upload", "batch_objects", "cull", "shadow_pass", "forward_begin", "forward_pass", "hiz_build", "forward_resolve",
                 "forward_blend", "tonemap", "update_point_light_sources_device", "evaluate_point_lights"}
@@ -308,7 +299,8 @@ def test_gpu_graphed_walkthrough_with_moving_point_lights(left):
 
     r = walk_world(left)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0), ambient_color=(0.02, 0.02, 0.02, 0.0))
-    graph_b, eager_b, host_b, orc = cuda(True), cuda(True), cuda(True), load_points_oracle_backend()
+    graph_b, eager_b, host_b = (load_cuda_backend(0, parity_target=True) for _ in range(3))
+    orc = load_points_oracle_backend()
     log = CallLog(graph_b)
     g_graph, g_eager, g_host, g_orc = BaseRenderGraph(log), BaseRenderGraph(eager_b), BaseRenderGraph(host_b), BaseRenderGraph(orc)
     res = (192, 108)
@@ -362,7 +354,7 @@ def test_gpu_graphed_walkthrough_with_moving_point_lights(left):
         og, oe, oh = frame_outputs(graph_b), frame_outputs(eager_b), frame_outputs(host_b)
         for what, x, y in (("eager", og, oe), ("host r3_set_point_lights", og, oh)):
             for name, a, c in zip(("rgba16f", "f32", "depth"), x, y):
-                assert same_bits(a, c), f"frame {frame}: graph vs {what}: {name} differs"
+                assert same_bytes(a, c), f"frame {frame}: graph vs {what}: {name} differs"
         ho = orc.readback_hdr_f32()
         ok = np.isfinite(ho)
         err = np.abs(og[1][ok] - ho[ok]) / np.maximum(1.0, np.abs(ho[ok]))
@@ -387,7 +379,7 @@ def test_gpu_resolve_after_an_update_without_evaluation_is_a_state_error():
     for h in range(8):
         r.update_point_light(h, PointLight((float(h), 1.0, 0.0), (1.0, 0.5, 0.2), 4.0, 2.0))
     ev = r.evaluate()
-    b = cuda(True)
+    b = load_cuda_backend(0, parity_target=True)
     g = BaseRenderGraph(b)
     g.add_to_graph(ev, (192, 108), 1, BaseRenderGraphSettings(), device_point_lights=True)
     g.add_to_graph(ev, (192, 108), 1, BaseRenderGraphSettings(), upload=False, device_point_lights=True)   # last frame's lists predict
@@ -399,12 +391,12 @@ def test_gpu_resolve_after_an_update_without_evaluation_is_a_state_error():
             call()
         assert e.value.code == R3_E_STATE
     assert b.readback_point_lights() == before
-    assert all(same_bits(x, y) for x, y in zip(frame_outputs(b), want)), "a rejected resolve changed the frame"
+    assert all(same_bytes(x, y) for x, y in zip(frame_outputs(b), want)), "a rejected resolve changed the frame"
     b.set_point_light_sources(*ev.point_sources)
     with pytest.raises(R3Error) as e:
         b.forward_resolve()
     assert e.value.code == R3_E_STATE
     b.evaluate_point_lights()
     g.add_to_graph(ev, (192, 108), 1, BaseRenderGraphSettings(), upload=False, device_point_lights=True)
-    assert all(same_bits(x, y) for x, y in zip(frame_outputs(b), want))
+    assert all(same_bytes(x, y) for x, y in zip(frame_outputs(b), want))
     b.close()

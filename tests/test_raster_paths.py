@@ -94,8 +94,6 @@ def test_watertight_blend_grid(cuda, cell, samples):
     assert np.array_equal(hdr, np.broadcast_to(want, hdr.shape)), f"{np.count_nonzero((hdr != want).any(axis=1))} pixels are not one layer"
 
 
-# a quad twice across the target in both directions would not be clipped; this one reaches 400x past the guard band
-GUARD_QUAD = [((-1.0e5, -1.0e5), (1.0e5, -1.0e5), (1.0e5, 1.0e5)), ((-1.0e5, -1.0e5), (1.0e5, 1.0e5), (-1.0e5, 1.0e5))]
 # Along the shared diagonal the two triangles are clipped with clip_lerp from opposite ends, so in general the two clipped copies
 # of the diagonal may round apart and leave gaps or double cover.  For this quad they do not: the oracle covers every sample exactly
 # once at one and at four samples (measured), and the kernels must match it.
@@ -106,10 +104,10 @@ GUARD_QUAD_SLACK = 0
 def test_guard_band_clipping(cuda, samples):
     """Two triangles with vertices far beyond the 64x guard band, and long triangles whose clipped on-screen part has a medium
     pixel box: parity with the oracle, and the clipped quad covers the target once up to a stated slack along its diagonal."""
-    subs = [s for t in GUARD_QUAD for s in ref.clip_to_guard_band(t, 256, 256)]
+    subs = [s for t in scenes.GUARD_QUAD for s in ref.clip_to_guard_band(t, 256, 256)]
     census = ref.path_census(subs, samples, (0, 0, 256, 256), clipped=[True] * len(subs))
     assert census["band"] > 0, census
-    orc, _ = render_both(cuda, 256, 256, GUARD_QUAD, [0.5, 0.5], samples)
+    orc, _ = render_both(cuda, 256, 256, scenes.GUARD_QUAD, [0.5, 0.5], samples)
     assert_parity(cuda, orc, "guard-band quad")
     assert abs(cuda.forward_stats()[1] - 256 * 256 * samples) <= GUARD_QUAD_SLACK * samples
     assert np.count_nonzero(cuda.readback_depth() == 0.0) == 0

@@ -4,36 +4,25 @@ indices and re-adding its objects: the mesh buffer, the mesh spheres, the record
 invocation bound, and whole frames against a context fed the rebuilt world."""
 import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
 
 import remesh_case as case
+from harness import ROOT, assert_same_frame, check_declared_and_exported, expect_error, on_stream, to_device, unbound_backend
+from mesh_deform_case import bits, canon, canon_records
 from rend3_b200 import world
-from rend3_b200.backend import CUDA_LIB_PATH, Backend, R3Error
+from rend3_b200.backend import R3Error, load_cuda_backend
 from rend3_b200.layouts import (ATTR_ABSENT, DEFORM_TANGENTS, REMESH_APPLIED, REMESH_INDEX_OUT_OF_RANGE, REMESH_NOT_TRIANGLES,
                                 REMESH_OVER_CAPACITY, REMESHABLE_MESH_DTYPE)
-from test_mesh_deform import bits, canon, canon_records
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 f32 = np.float32
 E_INVALID, E_STATE = -1, -5
 RES = (256, 160)
 
 
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
-
-
 # ------------------------------------------------------------------ without a GPU
 def test_library_exports_the_entry_points_with_the_headers_signatures():
-    from rend3_b200.backend import ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
     u64 = ctypes.c_uint64(0)
     decls = {
         "int r3_set_remeshable_meshes(r3_ctx*, const r3_remeshable_mesh* meshes, uint32_t n_meshes, const uint32_t* object_slots, "
@@ -47,11 +36,7 @@ def test_library_exports_the_entry_points_with_the_headers_signatures():
         "int r3_readback_remesh_status(r3_ctx*, uint32_t* status, uint32_t* counts_or_null , uint32_t first, uint32_t n);": (None, None, None, 0, 0),
         "int r3_debug_invocation_bound(r3_ctx*, uint64_t out[2]);": (None, None),
     }
-    for decl, args in decls.items():
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        assert getattr(lib, name)(*args) == E_INVALID   # no context: rejected before anything is touched
+    check_declared_and_exported(decls, decls.get)
 
 
 def test_remeshable_mesh_layout_matches_c_header():
@@ -75,9 +60,7 @@ def test_remeshable_mesh_layout_matches_c_header():
 
 
 def test_wrappers_reject_bad_arrays_before_calling():
-    from test_mesh_deform import _unbound_backend
-
-    b = _unbound_backend()
+    b = unbound_backend()
     with pytest.raises(AssertionError, match="meshes"):
         b.set_remeshable_meshes(np.zeros(4, np.uint32))
     with pytest.raises(AssertionError, match="one mesh per slot"):
@@ -127,12 +110,6 @@ def test_restatement_equals_world_rebuild_on_finite_meshes(left):
 
 
 # ------------------------------------------------------------------ on the GPU
-def cuda(**kw):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, **kw)
-
-
 def byte_copy(records):
     """a copy that keeps the bytes between the fields, which numpy's copy of a structured array need not"""
     return np.frombuffer(bytearray(np.ascontiguousarray(records).tobytes()), dtype=records.dtype)
@@ -173,7 +150,6 @@ def remesh(b, form, s):
     if form == "host":
         b.remesh_meshes(**s)
         return
-    from test_object_presence import to_device
 
     b.remesh_meshes_device(**{k: to_device(b, v) for k, v in s.items()})
     b.sync()
@@ -188,7 +164,7 @@ def test_gpu_edge_cases_equal_the_restatement(handedness, form):
     positions, bit for bit"""
     ks = case.kinds()
     w = case.build_world(ks, handedness=handedness)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     b.set_remeshable_meshes(w.records, w.slots, w.object_meshes)
     st = State(w)
@@ -207,7 +183,7 @@ def test_gpu_validation_leaves_failing_meshes_and_their_objects_as_they_were():
     others; the host form rejects the whole call and writes nothing"""
     ks = case.kinds()
     w = case.build_world(ks)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     b.set_remeshable_meshes(w.records, w.slots, w.object_meshes)
     st = State(w)
@@ -244,7 +220,7 @@ def test_gpu_set_rejects_bad_input_and_the_state_rules_hold():
 
     ks = case.kinds()[:3]
     w = case.build_world(ks, objects_per_mesh=2)
-    b = cuda()
+    b = load_cuda_backend(0)
     case.upload(b, w.ev)
     frames = [case.frame_for(k, 1) for k in ks]
     s = case.streams(w, frames)
@@ -327,7 +303,7 @@ def test_gpu_deform_keeps_a_rewritten_index_count_within_the_bound(how):
     import mesh_deform_case as dcase
 
     w = dcase.build_world([dcase.grid(9, 9), dcase.fan(64)], objects_per_mesh=2)
-    b = cuda()
+    b = load_cuda_backend(0)
     dcase.upload(b, w.ev)
     b.set_deformable_meshes(w.meshes, w.slots, w.object_meshes)
     recs = byte_copy(w.ev.object_buffer)
@@ -366,7 +342,7 @@ def test_gpu_invocation_bound_keeps_the_capacities_and_frames_equal_the_rebuilt_
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
     ks = case.kinds()
     w = case.build_world(ks, objects_per_mesh=3, extent=3.0)
-    b, full = cuda(parity_target=True), cuda(parity_target=True)
+    b, full = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     g, gf = BaseRenderGraph(b), BaseRenderGraph(full)
     g.add_to_graph(w.ev, RES, 1, settings, movable_objects=True)
     gf.add_to_graph(w.ev, RES, 1, settings)
@@ -407,10 +383,9 @@ class _RangesOnly:
 
 
 def assert_same_frame_within_bound(a, b, ev, what):
-    """test_world_updates.assert_same_frame, with the index lists compared over the draw calls' ranges only and the culling results
+    """harness.assert_same_frame, with the index lists compared over the draw calls' ranges only and the culling results
     over their common length: the remeshed context sizes those buffers by the capacities (the invocation floors), the rebuilt one by
     the counts"""
-    from test_world_updates import assert_same_frame
 
     ra, rb = a.readback_indices, b.readback_indices
     ca, cb = a.readback_culling_results, b.readback_culling_results
@@ -445,14 +420,13 @@ def test_gpu_isosurface_frames_in_one_graph_equal_the_rebuilt_world(monkeypatch)
     import torch
 
     from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings
-    from test_object_presence import on_stream
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
     nx, ny = 24, 16
     ks = [case.Kind("grid", case.masked_grid(nx, ny, np.ones((ny - 1, nx - 1), bool), size=4.0), True, False, False, False)]
     w = case.build_world(ks, objects_per_mesh=2, extent=2.0)
-    dev, full = cuda(parity_target=True), cuda(parity_target=True)
+    dev, full = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gd, gf = BaseRenderGraph(dev), BaseRenderGraph(full)
     gd.add_to_graph(w.ev, RES, 1, settings, movable_objects=True)
     dev.set_remeshable_meshes(w.records, w.slots, w.object_meshes)

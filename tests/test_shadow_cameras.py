@@ -6,9 +6,11 @@ import numpy as np
 import pytest
 
 import shadow_camera_reference as ref
+from harness import same_words_nan_equal
 from oracle.lights import load_lights_oracle_backend
+from reference_goldens import GOLD
 from rend3_b200 import glam
-from rend3_b200.backend import CAMERA_VIEWPORT, R3Error
+from rend3_b200.backend import CAMERA_VIEWPORT, R3Error, load_cuda_backend
 from rend3_b200.layouts import LIGHT_SOURCE_DTYPE, OBJECT_DTYPE
 from rend3_b200.routines import BaseRenderGraphSettings
 from rend3_b200.world import (CUTOUT, LEFT, RIGHT, Camera, CameraState, DirectionalLight, MeshBuilder, Object, PbrMaterial, Renderer,
@@ -19,18 +21,10 @@ R3_E_INVALID, R3_E_STATE = -1, -5
 ATLAS = (512, 256)
 
 
-def sources(rows):
-    """rows: (direction, distance, resolution); placements packed along the atlas' first row, 64 texels each."""
-    s = np.zeros(len(rows), dtype=LIGHT_SOURCE_DTYPE)
-    for i, (d, dist, res) in enumerate(rows):
-        s[i] = ((1.0, 0.9, 0.8), 1.0 + 0.5 * i, d, dist, res, (64 * i, 0), 64)
-    return s
-
-
 def random_sources(seed, n=6):
     rng = np.random.default_rng(seed)
     rows = [(tuple(rng.normal(size=3)), float(rng.uniform(0.5, 500.0)), int(rng.integers(16, 4096))) for _ in range(n)]
-    s = sources(rows)
+    s = ref.sources(rows)
     s["color"] = rng.random((n, 3))
     s["intensity"] = rng.uniform(0.0, 4.0, n)
     return s
@@ -38,7 +32,7 @@ def random_sources(seed, n=6):
 
 # the edges R13 has to survive: a light along +-Y (a NaN camera), L on a texel boundary, negative coordinates (the sign of fmod),
 # |L| around 1e6, a distance / resolution that is not a power of two, distance 0 (a NaN offset), a non-finite L
-EDGE_SOURCES = sources([((0.0, -1.0, 0.0), 40.0, 512), ((0.0, 1.0, 0.0), 40.0, 512), ((-1.0, -4.0, 2.0), 40.0, 512),
+EDGE_SOURCES = ref.sources([((0.0, -1.0, 0.0), 40.0, 512), ((0.0, 1.0, 0.0), 40.0, 512), ((-1.0, -4.0, 2.0), 40.0, 512),
                         ((0.3, -0.8, -0.5), 10.0, 300), ((1.0, -1.0, 1.0), 0.0, 256), ((2.0, -3.0, -1.0), 400.0, 2048)])
 EDGE_LOCATIONS = [(0.0, 0.0, 0.0), (1.5, 2.0, -3.0), (-7.25, -0.0390625, -13.5), (0.078125, 0.15625, 0.0), (-3.3, -17.9, -0.01),
                   (1.0e6, -3.0e5, 7.0), (-999999.9, 123456.7, -1.0e6), (np.inf, 0.0, 1.0), (np.nan, 1.0, 2.0)]
@@ -53,13 +47,6 @@ def cases():
     return out
 
 
-def same_bits(a, b):
-    """Bit-identical float32 words, any NaN equal to any NaN."""
-    a, b = np.ascontiguousarray(a).view(np.uint32).ravel(), np.ascontiguousarray(b).view(np.uint32).ravel()
-    fa, fb = a.view(np.float32), b.view(np.float32)
-    return bool(np.all((a == b) | (np.isnan(fa) & np.isnan(fb))))
-
-
 def evaluate(b, src, loc, left):
     b.set_directional_light_sources(src, ATLAS[0], ATLAS[1], left)
     b.evaluate_shadow_cameras(loc)
@@ -71,8 +58,8 @@ def check_equals_reference(b):
         for name, src, loc in cases():
             heads, lights = evaluate(b, src, loc, left)
             want_h, want_l = ref.evaluate(src, ATLAS[0], ATLAS[1], loc, left)
-            assert same_bits(heads, want_h), f"{name} {loc} left={left}: cameras differ"
-            assert same_bits(lights, want_l), f"{name} {loc} left={left}: light records differ"
+            assert same_words_nan_equal(heads, want_h), f"{name} {loc} left={left}: cameras differ"
+            assert same_words_nan_equal(lights, want_l), f"{name} {loc} left={left}: light records differ"
 
 
 def test_oracle_equals_numpy_r13_bit_for_bit():
@@ -96,11 +83,11 @@ def test_degenerate_cases_are_the_rules():
 def test_texel_snapping_and_the_sign_of_fmod():
     """Moving the viewer within one texel leaves the camera's xy as it was; the offset keeps the dividend's sign, so a negative
     coordinate snaps towards zero like a positive one."""
-    src = sources([((0.0, 0.0, 1.0), 64.0, 64)])   # looking along +z: view xy = world xy (left-handed), texel = 1
+    src = ref.sources([((0.0, 0.0, 1.0), 64.0, 64)])   # looking along +z: view xy = world xy (left-handed), texel = 1
     for x0, x1 in ((3.25, 3.75), (-3.25, -3.75)):
         a, _ = ref.evaluate(src, ATLAS[0], ATLAS[1], (x0, 0.5, 0.0), True)
         b, _ = ref.evaluate(src, ATLAS[0], ATLAS[1], (x1, 0.5, 0.0), True)
-        assert same_bits(a["view"], b["view"])
+        assert same_words_nan_equal(a["view"], b["view"])
         assert a["view"][0][12] == -np.trunc(x0)
 
 
@@ -180,8 +167,7 @@ def render_device(r, backend, resolution, settings=BaseRenderGraphSettings()):
 
 
 def check_goldens(make_backend):
-    """tests/test_oracle_golden.py's shadow/cube and examples/cube criteria, with the cameras evaluated by R13."""
-    from test_oracle_golden import GOLD
+    """tests/reference_goldens.py's shadow/cube and examples/cube criteria, with the cameras evaluated by R13."""
     from rend3_b200.runner import TestRunner
     from rend3_b200.world import PointLight
 
@@ -225,12 +211,12 @@ def test_static_light_fields_equal_world_buffer():
         host = np.frombuffer(ev.directional_buffer[16:], dtype=lights.dtype)
         assert len(host) == len(lights) == 2
         for f in ("color", "direction", "inv_resolution", "atlas_offset", "atlas_size"):
-            assert same_bits(lights[f], host[f]), f
+            assert same_words_nan_equal(lights[f], host[f]), f
 
 
 def check_rejections(b):
     """Every rejected call returns its code and leaves the context as it was."""
-    src = sources([((-1.0, -2.0, 0.5), 20.0, 256), ((0.3, -1.0, 0.2), 30.0, 128)])
+    src = ref.sources([((-1.0, -2.0, 0.5), 20.0, 256), ((0.3, -1.0, 0.2), 30.0, 128)])
     b.set_objects(np.zeros(8, dtype=OBJECT_DTYPE))
     with pytest.raises(R3Error) as e:
         b.evaluate_shadow_cameras((0.0, 0.0, 0.0))
@@ -264,7 +250,7 @@ def check_rejections(b):
         b.readback_shadow_cameras(3)
     assert e.value.code == R3_E_INVALID
     got = b.readback_shadow_cameras(2)
-    assert same_bits(got[0], want[0]) and same_bits(got[1], want[1]), "a rejected call changed the cameras or the light buffer"
+    assert same_words_nan_equal(got[0], want[0]) and same_words_nan_equal(got[1], want[1]), "a rejected call changed the cameras or the light buffer"
     b.shadow_uniform_upload(1, 8)
     # r3_set_directional_lights replaces the sources: the device cameras are gone until sources are set again
     b.set_directional_lights(np.zeros(4, np.uint32).tobytes(), ATLAS[0], ATLAS[1])
@@ -299,29 +285,23 @@ def test_light_source_layout_matches_c_header():
 
 
 # ------------------------------------------------------------------ GPU
-def cuda(parity=False):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, parity_target=parity)
-
-
 @pytest.mark.gpu
 def test_gpu_cameras_equal_oracle_bit_for_bit():
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     check_equals_reference(b)
     b.close()
 
 
 @pytest.mark.gpu
 def test_gpu_rejects_invalid_calls_and_keeps_its_state():
-    b = cuda()
+    b = load_cuda_backend(0, parity_target=False)
     check_rejections(b)
     b.close()
 
 
 @pytest.mark.gpu
 def test_gpu_goldens_with_device_cameras():
-    check_goldens(lambda: cuda())
+    check_goldens(lambda: load_cuda_backend(0, parity_target=False))
 
 
 def frame_products(b, ev, n_lights):
@@ -341,7 +321,7 @@ def frame_products(b, ev, n_lights):
 
 def assert_same_products(a, b, what):
     for k in a:
-        assert a[k].shape == b[k].shape and same_bits(a[k], b[k]), f"{what}: {k} differs"
+        assert a[k].shape == b[k].shape and same_words_nan_equal(a[k], b[k]), f"{what}: {k} differs"
 
 
 def assert_matches_oracle(c, o, what):
@@ -359,7 +339,7 @@ def assert_matches_oracle(c, o, what):
                 b0, cnt = int(r["base_index"]), int(r["vertex_count"])
                 assert np.array_equal(c[k][b0:b0 + cnt], o[k][b0:b0 + cnt]), f"{what}: {k} differs"
         else:
-            assert c[k].shape == o[k].shape and same_bits(c[k], o[k]), f"{what}: {k} differs"
+            assert c[k].shape == o[k].shape and same_words_nan_equal(c[k], o[k]), f"{what}: {k} differs"
 
 
 class CallLog:
@@ -394,7 +374,8 @@ def test_gpu_walkthrough_with_device_cameras(left):
 
     r = walkthrough_world(left)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
-    graph_b, eager_b, host_b, orc = cuda(True), cuda(True), cuda(True), load_lights_oracle_backend()
+    graph_b, eager_b, host_b = (load_cuda_backend(0, parity_target=True) for _ in range(3))
+    orc = load_lights_oracle_backend()
     log = CallLog(graph_b)
     graphs = {id(b): BaseRenderGraph(b) for b in (graph_b, eager_b, host_b, orc)}
     graphs[id(graph_b)] = BaseRenderGraph(log)
@@ -445,10 +426,10 @@ def test_gpu_walkthrough_with_device_cameras(left):
         po, hdr_o = frame_products(orc, ev, 2)
         ph, hdr_h = frame_products(host_b, ev, 2)
         assert_same_products(pg, pe, f"frame {frame}: graph vs eager")
-        assert same_bits(hdr_g, hdr_e), f"frame {frame}: graph vs eager HDR"
+        assert same_words_nan_equal(hdr_g, hdr_e), f"frame {frame}: graph vs eager HDR"
         assert_matches_oracle(pg, po, f"frame {frame}: device vs oracle")
         assert_same_products(pg, ph, f"frame {frame}: device vs host path")
-        assert same_bits(hdr_g, hdr_h), f"frame {frame}: device vs host path HDR"
+        assert same_words_nan_equal(hdr_g, hdr_h), f"frame {frame}: device vs host path HDR"
         ok = np.isfinite(hdr_o)
         err = np.abs(hdr_g[ok] - hdr_o[ok]) / np.maximum(1.0, np.abs(hdr_o[ok]))
         assert err.max() <= 1e-4, f"frame {frame}: HDR differs from the oracle by {err.max()}"
@@ -469,7 +450,7 @@ def test_gpu_switching_light_apis_mid_session():
 
     r = walkthrough_world(True, cutout=False)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
-    b, orc = cuda(True), load_lights_oracle_backend()
+    b, orc = load_cuda_backend(0, parity_target=True), load_lights_oracle_backend()
     gb, go = BaseRenderGraph(b), BaseRenderGraph(orc)
     for frame, device in enumerate([False, True, True, False, True]):
         r.set_camera_data(walkthrough_camera(frame, True))
@@ -498,7 +479,7 @@ def test_gpu_walkthrough_roughness0_grazing_light(left):
 
     r = walkthrough_world(left, quad_roughness=None)
     settings = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0))
-    b, orc = cuda(True), load_lights_oracle_backend()
+    b, orc = load_cuda_backend(0, parity_target=True), load_lights_oracle_backend()
     gb, go = BaseRenderGraph(b), BaseRenderGraph(orc)
     quad_alpha = np.float32(230.0 / 255.0)
     for frame in (0, 3):

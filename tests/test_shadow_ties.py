@@ -8,16 +8,13 @@ import pytest
 
 import shadow_lookup_reference as ref
 import shadow_tie_scenes as scenes
+from harness import same_bytes
 from oracle import load_oracle_backend
 
 SCENES = list(scenes.SCENES)
 # the probe's rounding: the kernels' n.l and diffuse term are within a few float32 ulps of the oracle's, so a recovered factor is
 # good to about 1e-6; a flipped tap moves it by 0.2 x its bilinear weight, so every flip with a weight of 1e-5 or more shows
 RECOVER_TOL = 1e-6
-
-
-def same_bits(a, b):
-    return np.array_equal(np.ascontiguousarray(a).view(np.uint32), np.ascontiguousarray(b).view(np.uint32))
 
 
 def draw(backend, name, samples, tex=False):
@@ -131,8 +128,8 @@ def test_gpu_lookup_at_ties(name, samples, tex):
     b = load_cuda_backend(0, parity_target=True)
     g = draw(b, name, samples, tex)
     b.close()
-    assert same_bits(g["atlas"], o["atlas"]), "shadow atlas differs from the oracle"
-    assert same_bits(g["depth"], o["depth"]), "depth differs from the oracle"
+    assert same_bytes(g["atlas"], o["atlas"]), "shadow atlas differs from the oracle"
+    assert same_bytes(g["depth"], o["depth"]), "depth differs from the oracle"
     if samples == 1:
         want = rs.factors()
         got = rs.recover(g["hdr"])

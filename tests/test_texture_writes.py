@@ -3,23 +3,17 @@ texture_write_case.py (blob bytes), r3_set_textures / r3_set_skybox of world.py'
 given that world, plus the calls' validation, the frame graph and the interplay with r3_update_textures / r3_set_textures."""
 import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
 
 import texture_write_case as twc
-from rend3_b200.backend import CUDA_LIB_PATH, Backend, R3Error
+from harness import (ROOT, assert_same_frame, assert_same_ldr, check_declared_and_exported, expect_error, hdr_close, settings, to_device,
+                     unbound_backend)
+from rend3_b200.backend import R3Error, load_cuda_backend
 from rend3_b200.layouts import SKYBOX_FACE, TEXTURE_REGION_DTYPE, texfmt_element_bytes, texfmt_is_block, texfmt_level_shape
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E_INVALID, E_STATE = -1, -5
-
-
-def expect_error(code, fn, *args, **kw):
-    with pytest.raises(R3Error) as e:
-        fn(*args, **kw)
-    assert e.value.code == code, str(e.value)
 
 
 # ------------------------------------------------------------------ without a GPU
@@ -29,15 +23,7 @@ DECLS = ("int r3_write_texture_regions(r3_ctx*, const r3_texture_region* regions
 
 
 def test_library_exports_the_three_entry_points_with_the_headers_signatures():
-    from rend3_b200.backend import ENTRY_POINTS
-
-    lib = ctypes.CDLL(CUDA_LIB_PATH)
-    header = re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rend3_b200.h")).read(), flags=re.S))
-    for decl in DECLS:
-        assert decl in header, decl
-        name = decl.split("(")[0].split()[-1]
-        assert hasattr(lib, name) and name[3:] in ENTRY_POINTS
-        assert getattr(lib, name)(None, None, ctypes.c_uint32(1), None, ctypes.c_uint64(0)) == E_INVALID   # no context
+    check_declared_and_exported(DECLS, (None, None, ctypes.c_uint32(1), None, ctypes.c_uint64(0)))
 
 
 def test_region_record_layout():
@@ -67,19 +53,6 @@ def test_format_helpers_match_the_header_macros():
     assert rows == [(int(texfmt_is_block(f)), texfmt_element_bytes(f)) for f in range(31)]
 
 
-class _NoCalls:
-    def __getattr__(self, name):
-        def call(*args):
-            raise AssertionError(f"{name} was called")
-        return call
-
-
-def _unbound_backend():
-    b = Backend.__new__(Backend)
-    b.lib, b.prefix, b.ctx = _NoCalls(), "r3_", None
-    return b
-
-
 @pytest.mark.parametrize("regions,texels", [
     (np.zeros(40, np.uint8), np.zeros(4, np.uint8)),                       # bytes, not records
     (np.zeros((2, 2), TEXTURE_REGION_DTYPE), np.zeros(4, np.uint8)),       # 2-d records
@@ -89,12 +62,12 @@ def _unbound_backend():
 ], ids=["bytes", "2d", "strided", "strided-texels", "bytes-object"])
 def test_host_wrapper_rejects_bad_inputs_before_calling(regions, texels):
     with pytest.raises(AssertionError, match="regions|texels"):
-        _unbound_backend().write_texture_regions(regions, texels)
+        unbound_backend().write_texture_regions(regions, texels)
 
 
 def test_device_wrapper_rejects_host_mistyped_and_misaligned_tensors_before_calling():
     torch = pytest.importorskip("torch")
-    b = _unbound_backend()
+    b = unbound_backend()
     good_host = torch.zeros(2, 40, dtype=torch.uint8)
     for regions, texels in ((good_host, good_host),                                         # host tensors
                             (np.zeros(2, TEXTURE_REGION_DTYPE), good_host),                 # a numpy array
@@ -203,26 +176,6 @@ def test_world_skybox_writes_equal_the_restatement(dtype):
 
 
 # ------------------------------------------------------------------ GPU
-def cuda(parity=True):
-    from rend3_b200.backend import load_cuda_backend
-
-    return load_cuda_backend(0, parity_target=parity)
-
-
-def on_stream(b, fn):
-    import torch
-
-    with torch.cuda.stream(torch.cuda.ExternalStream(b.stream())):
-        return fn()
-
-
-def to_device(b, array):
-    import torch
-
-    host = torch.from_numpy(np.ascontiguousarray(array).copy())
-    return on_stream(b, lambda: host.to("cuda", non_blocking=False))
-
-
 def device_args(b, regions, texels):
     """(regions as uint8 (n, 40), texels as uint8) CUDA tensors made on the context's stream."""
     return to_device(b, np.ascontiguousarray(regions).view(np.uint8).reshape(-1, 40)), to_device(b, np.ascontiguousarray(texels).reshape(-1).view(np.uint8))
@@ -250,7 +203,7 @@ def test_gpu_blob_bytes_equal_the_restatement():
     r.set_skybox(sky_faces(rng, 32, np.float32), srgb=False)
     ev = r.evaluate()
     descs, sky = ev.texture_descs, ev.skybox_desc
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     b.set_textures(descs, ev.texture_texels)
     b.set_skybox(sky, ev.skybox_texels)
     table, sky_blob = ev.texture_texels.copy(), ev.skybox_texels.copy()
@@ -341,7 +294,7 @@ def test_gpu_device_form_drops_each_invalid_region_and_applies_the_others():
     r.set_skybox(sky_faces(rng, 8, np.uint8), srgb=True)
     ev = r.evaluate()
     descs, sky = ev.texture_descs, ev.skybox_desc
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     b.set_textures(descs, ev.texture_texels)
     b.set_skybox(sky, ev.skybox_texels)
     table, sky_blob = ev.texture_texels.copy(), ev.skybox_texels.copy()
@@ -359,7 +312,7 @@ def test_gpu_device_form_drops_each_invalid_region_and_applies_the_others():
         assert np.array_equal(got_table, want_table) and np.array_equal(got_sky, want_sky), f"{label}: the drop differs"
         table, sky_blob = want_table, want_sky
     # faces without a skybox are dropped; a table alone is enough state
-    nosky = cuda(False)
+    nosky = load_cuda_backend(0, parity_target=False)
     nosky.set_textures(descs, ev.texture_texels)
     regions, texels = twc.pack_regions([(0, 0, 0, 0, 1, 1, 1, 1)], [0], rng)
     face = regions.copy()
@@ -378,7 +331,7 @@ def test_gpu_host_form_rejects_each_invalid_call_and_leaves_the_blobs():
     r.set_skybox(sky_faces(rng, 8, np.float32), srgb=False)
     ev = r.evaluate()
     descs, sky = ev.texture_descs, ev.skybox_desc
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     b.set_textures(descs, ev.texture_texels)
     b.set_skybox(sky, ev.skybox_texels)
     before = blobs(b, len(ev.texture_texels), len(ev.skybox_texels))
@@ -409,7 +362,7 @@ def test_gpu_host_form_rejects_each_invalid_call_and_leaves_the_blobs():
     expect_error(E_INVALID, b.readback_texels, False, len(ev.texture_texels) - 3, 4)
     expect_error(E_INVALID, b.readback_texels, True, 0, len(ev.skybox_texels) + 1)
     # R3_E_STATE without a table or a skybox; n == 0 is still R3_OK
-    empty = cuda(False)
+    empty = load_cuda_backend(0, parity_target=False)
     expect_error(E_STATE, empty.write_texture_regions, regions, texels)
     expect_error(E_STATE, empty.write_texture_regions_device, *device_args(empty, regions, texels))
     empty.write_texture_regions(regions[:0], texels)
@@ -457,19 +410,16 @@ def test_gpu_frames_equal_a_full_reupload_and_the_oracle(monkeypatch, scene, sam
     """Five frames of texture writes (in the cutout world the albedo alpha of the per-fragment cutout material is rewritten, so the forward
     discard and the shadow pass's cutout change).  The writing context equals a context given r3_set_textures of world.py's patched table
     every frame in depth, rgba16f, the f32 parity target, LDR and the shadow atlas, bit for bit; the oracle given the same table agrees."""
-    import test_gpu_parity as parity
     from oracle import load_oracle_backend
     from rend3_b200.backend import CAMERA_VIEWPORT
     from rend3_b200.routines import BaseRenderGraph
-    from test_object_presence import assert_same_ldr, settings
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     res = (96, 64)
     r, handles = cutout_world() if scene == "cutout" else quad_world(scene.split("-")[1])
     rng = np.random.default_rng(samples)
     ev = r.evaluate()
-    wr, full, orc = cuda(), cuda(), load_oracle_backend()
+    wr, full, orc = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True), load_oracle_backend()
     gw, gf, go = BaseRenderGraph(wr), BaseRenderGraph(full), BaseRenderGraph(orc)
     for g in (gw, gf):
         g.add_to_graph(ev, res, samples, settings())
@@ -494,7 +444,7 @@ def test_gpu_frames_equal_a_full_reupload_and_the_oracle(monkeypatch, scene, sam
         assert np.array_equal(wr.readback_depth().view(np.uint32), orc.readback_depth().view(np.uint32)), f"{what}: oracle depth"
         for cam in [CAMERA_VIEWPORT] + list(range(len(ev.shadows))):
             assert np.array_equal(wr.readback_visible(cam), orc.readback_visible(cam)), f"{what} camera {cam}: oracle"
-        parity.hdr_close(wr.readback_hdr_f32(), orc.readback_hdr_f32(), f"{what}: oracle hdr", scene == "cutout" or samples == 4)
+        hdr_close(wr.readback_hdr_f32(), orc.readback_hdr_f32(), f"{what}: oracle hdr", scene == "cutout" or samples == 4)
     wr.close(), full.close(), orc.close()
 
 
@@ -506,8 +456,6 @@ def test_gpu_skybox_writes_equal_set_skybox(dtype):
     from rend3_b200.routines import BaseRenderGraph
     from rend3_b200.world import LEFT, Camera, Renderer
     from skybox_case import random_rotation
-    from test_object_presence import assert_same_ldr, settings
-    from test_world_updates import assert_same_frame
 
     rng = np.random.default_rng(4)
     res = (96, 64)
@@ -515,7 +463,7 @@ def test_gpu_skybox_writes_equal_set_skybox(dtype):
     r.set_camera_data(Camera(("perspective", 90.0, 0.1), random_rotation(3)))
     r.set_skybox(sky_faces(rng, 16, dtype), srgb=dtype == np.uint8)
     ev = r.evaluate()
-    wr, full = cuda(), cuda()
+    wr, full = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gw, gf = BaseRenderGraph(wr), BaseRenderGraph(full)
     for g in (gw, gf):
         g.add_to_graph(ev, res, 1, settings())
@@ -549,8 +497,6 @@ def test_gpu_graph_frames_stay_one_launch(monkeypatch):
     and every frame equals a context given r3_set_textures of the patched table."""
     from material_update_case import MaterialWorld
     from rend3_b200.routines import BaseRenderGraph
-    from test_object_presence import assert_same_ldr, settings
-    from test_world_updates import assert_same_frame
 
     monkeypatch.delenv("R3_HOST_BATCHING", raising=False)
     w = MaterialWorld(n_objects=150, blend=False)   # a blend routine's fragment pool may grow (and flush) in any frame
@@ -558,7 +504,7 @@ def test_gpu_graph_frames_stay_one_launch(monkeypatch):
     big = r.add_texture_2d(twc.texture_for(0, 256, 256, np.random.default_rng(1)))
     ev = r.evaluate()
     res = (96, 64)
-    wr, full = cuda(), cuda()
+    wr, full = load_cuda_backend(0, parity_target=True), load_cuda_backend(0, parity_target=True)
     gw, gf = BaseRenderGraph(wr), BaseRenderGraph(full)
     for g in (gw, gf):
         g.add_to_graph(ev, res, 1, settings())
@@ -597,7 +543,7 @@ def test_gpu_writes_order_with_update_textures_and_set_textures():
     r = twc.every_format_world(seed=12)
     ev = r.evaluate()
     descs, table = ev.texture_descs, ev.texture_texels.copy()
-    b = cuda(False)
+    b = load_cuda_backend(0, parity_target=False)
     b.set_textures(descs, table)
     grown_tex = twc.texture_for(2, 64, 64, rng)
     lv = np.concatenate([np.ascontiguousarray(l).reshape(-1).view(np.uint8) for l in grown_tex.stored_levels()])

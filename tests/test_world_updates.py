@@ -7,8 +7,9 @@ import numpy as np
 import pytest
 
 import cull_scenes as scenes
+from harness import assert_same_frame, compare_frame_state, cull_and_batch, expect_error
 from world_update_scene import ChangingWorld, merge, upload_delta
-from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE, CB_CULL, R3Error, load_cuda_backend
+from rend3_b200.backend import CAMERA_VIEWPORT, CB_BAKE, CB_CULL, load_cuda_backend
 from rend3_b200.layouts import PCU_MULTISAMPLED, TEXTURE_DESC_DTYPE
 from rend3_b200.routines import BaseRenderGraph, BaseRenderGraphSettings, per_camera_header
 from rend3_b200.scenes import cloud_camera, object_cloud_records
@@ -19,35 +20,6 @@ pytestmark = pytest.mark.gpu
 RES = (256, 160)
 SETTINGS = BaseRenderGraphSettings(clear_color=(0.1, 0.05, 0.1, 1.0), ambient_color=(0.02, 0.02, 0.02, 1.0))
 E_INVALID, E_STATE = -1, -5
-
-
-def assert_same_frame(a, b, ev, what):
-    """Every artefact of the last frame, bit for bit."""
-    n = len(ev.object_buffer)
-    for cam in [CAMERA_VIEWPORT] + list(range(len(ev.shadows))):
-        w = f"{what} camera {cam}"
-        assert np.array_equal(a.readback_visible(cam), b.readback_visible(cam)), f"{w}: visible lists differ"
-        assert a.readback_object_matrices(cam, 0, n).tobytes() == b.readback_object_matrices(cam, 0, n).tobytes(), f"{w}: MV/MVP differ"
-        assert a.batching_info(cam) == b.batching_info(cam), f"{w}: batching path"
-        ba, ra = a.readback_batches(cam)
-        bb, rb = b.readback_batches(cam)
-        assert ba.tobytes() == bb.tobytes() and ra.tobytes() == rb.tobytes(), f"{w}: batches / regions differ"
-        for part in (0, 1):
-            da, db = a.readback_draw_calls(cam, part), b.readback_draw_calls(cam, part)
-            assert da.tobytes() == db.tobytes(), f"{w}: draw calls (partition {part}) differ"
-            ia, ib = a.readback_indices(cam, part), b.readback_indices(cam, part)
-            assert len(ia) == len(ib), f"{w}: index list lengths (partition {part})"
-            for r in da:
-                b0, cnt = int(r["base_index"]), int(r["vertex_count"])
-                assert np.array_equal(ia[b0:b0 + cnt], ib[b0:b0 + cnt]), f"{w}: index list (partition {part})"
-            assert a.readback_culling_results(cam, part).tobytes() == b.readback_culling_results(cam, part).tobytes(), f"{w}: culling results ({part})"
-    assert a.readback_depth().tobytes() == b.readback_depth().tobytes(), f"{what}: depth differs"
-    assert a.readback_hdr_f16().tobytes() == b.readback_hdr_f16().tobytes(), f"{what}: rgba16f differs"
-    assert a.readback_hdr_f32().tobytes() == b.readback_hdr_f32().tobytes(), f"{what}: f32 parity target differs"
-    sw, sh = ev.shadow_target_size
-    assert a.readback_shadow_atlas(sw, sh).tobytes() == b.readback_shadow_atlas(sw, sh).tobytes(), f"{what}: shadow atlas differs"
-    assert a.forward_stats() == b.forward_stats(), f"{what}: forward_stats"
-    assert a.forward_light_evaluations() == b.forward_light_evaluations(), f"{what}: light evaluations"
 
 
 def script(w: ChangingWorld, blend: bool = True):
@@ -83,8 +55,6 @@ def test_incremental_updates_equal_full_uploads(monkeypatch, frame_sort, host):
     batching path goes device -> host -> device, and on three frames B equals the oracle.  (Some later frames differ from the oracle with
     full uploads as well: the previous-invocation entries of the batch tables when the batching path changes or the object count grows,
     and the readable length of the residual index list after objects are revived.  A and B agree there, so those frames are held to A.)"""
-    import test_gpu_parity as parity
-
     monkeypatch.setenv("R3_FRAME_SORT", frame_sort)
     if host:
         monkeypatch.setenv("R3_HOST_BATCHING", "1")
@@ -107,7 +77,7 @@ def test_incremental_updates_equal_full_uploads(monkeypatch, frame_sort, host):
         if go is not None:
             go.add_to_graph(w.ev, RES, 1, SETTINGS)
             if frame in (0, 1, 6):   # the first frame; a move; blend objects
-                parity.compare_frame_state(b, orc, w.ev, [CAMERA_VIEWPORT, 0, 1], what=f"oracle, frame {frame}", f16_samples=True)
+                compare_frame_state(b, orc, w.ev, [CAMERA_VIEWPORT, 0, 1], what=f"oracle, frame {frame}", f16_samples=True)
     assert paths == (["host"] * 12 if host else [device] * 7 + ["host"] + [device] * 4), paths
     assert len(w.ev.object_buffer) == 3064 and b.visible_count(CAMERA_VIEWPORT) > 0
     a.close(), b.close()
@@ -122,20 +92,11 @@ def cloud_world(n, seed=3):
     return rec, key, flags, rec["sphere_center"].copy()
 
 
-def cull_and_batch(b, n):
-    header = per_camera_header(cloud_camera(pull_back=12.0), CAMERA_VIEWPORT, (640, 360), 1, n)
-    b.object_uniform_upload(CAMERA_VIEWPORT, header, CB_BAKE | CB_CULL)
-    b.batch_objects(CAMERA_VIEWPORT, np.array([1.0, 2.0, 3.0], dtype=np.float32))
-    bt, rg = b.readback_batches(CAMERA_VIEWPORT)
-    return (b.readback_visible(CAMERA_VIEWPORT).copy(), b.readback_object_matrices(CAMERA_VIEWPORT, 0, n).tobytes(), bt.tobytes(), rg.tobytes(),
-            b.batching_info(CAMERA_VIEWPORT)["path"])
-
-
 def assert_same_objects(a, b, n, what):
-    ra, rb = cull_and_batch(a, n), cull_and_batch(b, n)
+    ra, rb = (cull_and_batch(x, n) + [x.batching_info(CAMERA_VIEWPORT)["path"]] for x in (a, b))
     for k, name in enumerate(("visible list", "MV/MVP", "batches", "regions", "batching path")):
-        assert np.array_equal(ra[k], rb[k]) if k == 0 else ra[k] == rb[k], f"{what}: {name} differs"
-    return ra
+        assert ra[k] == rb[k], f"{what}: {name} differs"
+    return np.frombuffer(ra[0], np.uint32)
 
 
 def test_duplicate_slots_and_shared_live_words(monkeypatch):
@@ -188,17 +149,11 @@ def test_resize_1000_1001_70001(monkeypatch):
             full_rec[fill], full_key[fill], full_flags[fill], full_loc[fill] = rec[fill], key[fill], flags[fill], loc[fill]
             a.set_objects(full_rec)
             a.set_object_sort_info(full_key, full_flags, full_loc)
-            vis = assert_same_objects(a, b, new, f"filled to {new} (host={host})")[0]
+            vis = assert_same_objects(a, b, new, f"filled to {new} (host={host})")
             if new - cur > 1000:
                 assert np.any(vis >= cur), "some of the new objects are visible"
             cur = new
         a.close(), b.close()
-
-
-def expect_error(code, fn, *args):
-    with pytest.raises(R3Error) as e:
-        fn(*args)
-    assert e.value.code == code, str(e.value)
 
 
 def test_rejections_leave_the_context_unchanged(monkeypatch):
